@@ -1,13 +1,15 @@
 #!/usr/bin/env python
 """bench.py — MCTS simulations/second of the per-move simulation loop (select -> step/expand -> value net -> backup)
-over N concurrent games, on 1..8 B200 (one process per GPU), next to the reference's CPU path.
+over N concurrent games, on 1..8 H100 (one process per GPU), next to the reference's CPU path.
 
-  python bench.py --gpus 1 --steps K --warmup W            B200 arm (this repo's CUDA engine through its C-ABI)
+  python bench.py --gpus 1 --steps K --warmup W            GPU arm (this repo's CUDA engine through its C-ABI)
   python bench.py --impl reference --steps K --warmup W    reference arm: the reference's own compiled
                                                             agents/cppmodule/agent.cpp (oracle/_ref) on the host cores
 A "step" is one move of every game: `sims` simulations per game, then get_action, play, update_root (play.py:118-177).
 Workload (BASELINE.json configs[2], the one north_star's target sentence names: >= 16384 concurrent games, ValueSimLP +
-value net, 500 sims/move).  `--workload vanilla` selects configs[1] (Vanilla MCTS, 4096 games, 300 sims/move).
+value net, 500 sims/move; 8192 arena slots per game, so that the 16384 arenas (41 GB) fit an 80 GB H100).
+`--workload vanilla` selects configs[1] (Vanilla MCTS, 4096 games, 300 sims/move).
+`--dump-outputs DIR` writes what the last timed step returned (actions, game records) as DIR/*.npy.
 Prints ONE JSON line on rank 0."""
 import argparse
 import json
@@ -31,33 +33,8 @@ ENV_ARGS = ((20, 10), 1, 0, 0)                   # play.py:75 defaults
 BASE_SEED = 123                                  # SURVEY §8d (echoes agent.cpp:23)
 
 
-TC_ISSUED_FLOP_PER_BOARD = 2 * 128 * 16 * (96 * 36 + 64 * 2)   # k_tc_conv: 2x18 MMAs of 128x96x16 + 2 of 128x64x16 per board
+TC_ISSUED_FLOP_PER_BOARD = 2 * 64 * 16 * (96 * 18 * 4 + 64 * 3)   # k_tc_conv: 4 x 18 MMAs of 64x96x16 + 3 of 64x64x16 per board
 ARENA_BYTES_PER_SLOT = 304
-
-
-def _ncu_traffic_file():
-    for name in ("ncu_traffic_r2b.json", "ncu_traffic_r2.json", "ncu_traffic_r1.json"):
-        p = os.path.join(ROOT, "profiles", name)
-        if os.path.exists(p):
-            return p
-    return None
-
-
-def ncu_traffic(kernel):
-    """dram__bytes_read.sum + dram__bytes_write.sum of one launch, from the committed ncu --set full capture (profiles/)."""
-    try:
-        return json.load(open(_ncu_traffic_file())).get(kernel, {}).get("dram_bytes")
-    except Exception:
-        return None
-
-
-def ncu_traffic_src():
-    """Which capture `traffic` comes from and the regime it was taken in (bench window or not)."""
-    try:
-        p = _ncu_traffic_file()
-        return {"file": os.path.relpath(p, ROOT), "regime": json.load(open(p)).get("_regime", "round-1 capture: moves 0-1 at 100-150 sims (NOT the bench window)")}
-    except Exception:
-        return None
 
 
 def measured_peaks():
@@ -65,7 +42,7 @@ def measured_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], tensor_burst=d["bf16_tflops"], tensor=d.get("bf16_tflops_sustained", d["bf16_tflops"]), src="measured")
-    return dict(hbm=6650.0, tensor_burst=1590.0, tensor=1400.0, src="fallback")   # B200_PROFILING.md fallback
+    return dict(hbm=3350.0, tensor_burst=989.0, tensor=989.0, src="H100 SXM data sheet (700 W)")
 
 
 # ----------------------------------------------------------------------------------------------- clocks sampler
@@ -324,11 +301,11 @@ def run_reference(args, cfg):
             "vs_baseline": None, "dtype": "f32", "data": "synthetic", "config": cfg["config"],
             "cpu_baseline": {"value": value, "unit": "sims/s", "cores": pool.P, "kind": "reference", "sample": sample},
             "e2e": {"value": value, "unit": "sims/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}, "gpu_launches": 0,
-            "reference_arm": REF_ARM_NOTE + "; `config` is the B200 arm's, for the ratio"}
+            "reference_arm": REF_ARM_NOTE + "; `config` is the GPU arm's, for the ratio"}
     print(json.dumps(line), flush=True)
 
 
-# ----------------------------------------------------------------------------------------------- B200 arm
+# ----------------------------------------------------------------------------------------------- GPU arm
 def run_b200(args, cfg):
     """Three passes over the SAME workload: the search is deterministic given the seeds (SURVEY N3), so every pass builds an
     identical engine from the same seeds, plays the same W warm-up moves and then the same K moves:
@@ -376,11 +353,17 @@ def run_b200(args, cfg):
     torch.cuda.synchronize()
     with Clocks(local_rank) as clk:
         eng.timer_start()
+        last_actions = None
         for _ in range(args.steps):
-            eng.play_move(sims, auto_reset=True, want_stats=False)
+            last_actions, _ = eng.play_move(sims, auto_reset=True, want_stats=False)
         ms = eng.timer_stop()
     torch.cuda.synchronize()
     D.barrier()
+    if args.dump_outputs and rank == 0 and last_actions is not None:
+        # the arrays a caller of the timed path receives after its last step: the chosen actions and the games they were played in
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "actions.npy"), last_actions.astype(np.float64))
+        np.save(os.path.join(args.dump_outputs, "games.npy"), eng.get_games().astype(np.float64))
     c1 = eng.counters()
     longest_trace = c1.pop("max_trace_len", None)             # not cumulative: the longest trace of the last move
     c0.pop("max_trace_len", None)
@@ -467,26 +450,10 @@ def run_b200(args, cfg):
         tree_s = (sel_ms + bk_ms) / 1e3
         if tree_s > 0:
             ach = tree_bytes / tree_s / 1e9
-            tr_s, tr_b = ncu_traffic("k_select_expand"), ncu_traffic("k_backup")
             roof_tree = {"bound": "hbm", "achieved": ach, "peak": peaks["hbm"], "unit": "GB/s", "frac": ach / peaks["hbm"],
-                         "traffic": (tr_s + tr_b) if tr_s and tr_b else None, "traffic_src": ncu_traffic_src(),
                          "algorithmic_bytes_per_launch_pair": tree_bytes / max(sel_n, 1),
                          "kernels": "k_select_expand + k_backup", "mean_trace_len": D_mean, "ms_per_launch_pair": (sel_ms + bk_ms) / max(sel_n, 1),
                          "peak_src": peaks["src"]}
-            # The walk is a chain of RANDOM accesses, so the streaming-copy peak is not its ceiling.  scripts/probe/mem_probe.cu measured what this
-            # memory system delivers for independent random 64-byte bursts that miss L2 (profiles/mem_probe_r2.txt): 40 G bursts/s (2.6 TB/s) at
-            # 1 GB, 31-36 G/s at 8 GB — and 6-10 G/s over a 128 GB footprint (2 MB pages: TLB reach).  The kernels' own DRAM traffic (ncu, same
-            # regime) divided by 64 B and by the measured launch time is their burst rate against that ceiling.
-            if tr_s and tr_b:
-                cap = 40.0e9
-                roof_tree["random_access"] = {"ceiling_gbursts_per_s": cap / 1e9, "ceiling_src": "profiles/mem_probe_r2.txt: random 64-byte bursts, 1 GB footprint, 32-64 warps/SM",
-                                              "k_select_expand_gbursts_per_s": tr_s / 64.0 / (sel_ms / max(sel_n, 1) / 1e3) / 1e9,
-                                              "k_backup_gbursts_per_s": tr_b / 64.0 / (bk_ms / max(bk_n, 1) / 1e3) / 1e9,
-                                              "frac_select": tr_s / 64.0 / (sel_ms / max(sel_n, 1) / 1e3) / cap,
-                                              "frac_backup": tr_b / 64.0 / (bk_ms / max(bk_n, 1) / 1e3) / cap,
-                                              "note": "DRAM bytes of the ncu capture (traffic_src) / 64 B / this run's launch time.  With the path cache on most of "
-                                                      "k_select_expand's reads are sequential lines (config.path_cache), so its figure mixes streaming and random "
-                                                      "bursts; k_backup's trace records are sequential too (a ratio above 1 is not a contradiction)"}
         if cfg["mode"] == "dist":
             conv_ms, conv_n = phases["conv"]
             flop = 19 * 7 * 32 * 16 * 2 + 16 * 4 * 32 * 512 * 2   # conv1 (19x7 pixels) + conv2 (16x4) on the 22x10 input of model_distributional.py:27
@@ -496,7 +463,7 @@ def run_b200(args, cfg):
                     "kernel": "k_tdc_conv" if cfg["eval"] == "net_tc" else "k_dn_conv", "ms_per_launch": conv_ms / max(conv_n, 1),
                     "share_of_step": conv_ms / ms_instr, "peak_src": peaks["src"] + " bf16 dense, sustained",
                     "fc_kernel_tflops": pdelta["eval_requests"] * 2 * 2048 * 128 / (fc_ms / 1e3) / 1e12 if fc_ms > 0 else None,
-                    "note": "achieved counts ALGORITHMIC conv FLOPs (2 233 344 per board).  eval=net_tc: tcgen05 kind::f16 with the fp32 operands split into two "
+                    "note": "achieved counts ALGORITHMIC conv FLOPs (2 233 344 per board).  eval=net_tc: wgmma f16 with the fp32 operands split into two "
                             "scaled fp16 terms (k_tdc_conv / k_tdc_fc, csrc/distnet_tc.cuh); eval=net: fp32 CUDA cores (k_dn_conv / k_dn_fc)"}
         elif cfg["mode"] != "vanilla":
             conv_ms, conv_n = phases["conv"]
@@ -506,17 +473,16 @@ def run_b200(args, cfg):
                 ach = boards * CONV_FLOP / (conv_ms / 1e3) / 1e12
                 kname = "k_vn_conv" if cfg["eval"] == "net" else "k_tc_conv"
                 roof = {"bound": "tensor", "achieved": ach, "peak": peaks["tensor"], "unit": "TFLOP/s", "frac": ach / peaks["tensor"],
-                        "traffic": ncu_traffic(kname), "traffic_src": ncu_traffic_src(), "kernel": kname,
+                        "kernel": kname,
                         "mma_flops_issued_per_launch": boards * TC_ISSUED_FLOP_PER_BOARD / conv_n, "ms_per_launch": conv_ms / conv_n,
                         "flops_per_launch": boards * CONV_FLOP / conv_n, "boards_per_launch": boards / conv_n,
                         "fc_kernel_tflops": boards * FC_FLOP / (fc_ms / 1e3) / 1e12 if fc_ms > 0 else None,
                         "share_of_step": conv_ms / ms_instr, "peak_src": peaks["src"] + " bf16 dense, sustained",
                         "note": "achieved counts ALGORITHMIC conv FLOPs (SURVEY 8d: 2 884 608 per board).  fp32-faithful arithmetic (north_star 1e-5): "
-                                "eval=net is CUDA-core fp32 FMA; eval=net_tc is tcgen05 kind::f16 with every fp32 operand split into two scaled fp16 terms "
-                                "(3 products per algorithmic product; M=128 pixel tiles carry halo rows), so the tensor pipe executes "
-                                "mma_flops_issued_per_launch.  scripts/probe/mma_probe.cu measures SS-mode tcgen05.mma at (A+B operand bytes)/128 B/clk with a "
-                                "44.7 clk floor: these small-N MMAs are shared-memory operand-fetch bound, not tensor-rate bound; the bf16 peak is the "
-                                "driver-measured denominator, not this kernel's ceiling"}
+                                "eval=net is CUDA-core fp32 FMA; eval=net_tc is wgmma f16 with every fp32 operand split into two scaled fp16 terms "
+                                "(3 products per algorithmic product; 64-row pixel tiles carry halo rows), so the tensor pipe executes "
+                                "mma_flops_issued_per_launch.  These small-N MMAs from shared memory are not tensor-rate bound; the bf16 peak is "
+                                "the denominator, not this kernel's ceiling"}
         else:
             ro_ms, ro_n = phases["rollout"]
             roof = {"bound": "hbm", "achieved": 0.0, "peak": peaks["hbm"], "unit": "GB/s", "frac": 0.0, "traffic": None, "kernel": "k_rollout",
@@ -620,9 +586,9 @@ def run_b200(args, cfg):
                 out[tag] = {"workload": label, "value": d3["sims"] / (ms3 / 1e3), "unit": "sims/s", "ms_per_step": ms3 / moves, "moves_timed": moves,
                             "warmup_moves": warm, "mean_trace_len": d3["trace_levels"] / max(d3["sims"], 1), "tree_resets_per_step": d3["tree_resets"] / moves}
         short_run("also_configs3_8192_games_per_gpu", "BASELINE configs[3] per-GPU share: ValueSimLP + value net (net_tc), 8192 games/GPU (65536 over 8 GPUs), 500 sims/move",
-                  8192, 500, 16384, "lp", cfg["eval"], w=weights)
+                  8192, 500, cfg["max_nodes"], "lp", cfg["eval"], w=weights)
         from tetris_mcts_b200.agents.DistValueSimOnline import init_dist_weights
-        short_run("also_configs4_distributional", "BASELINE configs[4] per-GPU share: distributional head (agents/core_distributional.py; network on tcgen05: "
+        short_run("also_configs4_distributional", "BASELINE configs[4] per-GPU share: distributional head (agents/core_distributional.py; network on tensor cores: "
                   "k_tdc_conv / k_tdc_fc), 2048 games/GPU (16384 over 8 GPUs), 1500 sims/move", 2048, 1500, 32768, "dist", cfg["eval"],
                   dw=init_dist_weights(0, 50), moves=2, warm=2)
     if world > 1:
@@ -638,7 +604,7 @@ def main():
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=3)
     ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
+    ap.add_argument("--impl", default="b200", choices=["b200", "reference"])   # b200: this repo's CUDA engine
     ap.add_argument("--workload", default="valuesimlp", choices=["valuesimlp", "vanilla", "dist"])
     ap.add_argument("--games-per-gpu", type=int, default=None)
     ap.add_argument("--sims", type=int, default=None)
@@ -652,6 +618,8 @@ def main():
                     help="b200_set_path_cache (memory traffic only, results identical): auto = the engine's default where it applies (LP mode, max_nodes <= 65536)")
     ap.add_argument("--ref-moves-per-step", type=int, default=2)
     ap.add_argument("--exchange-rows", type=int, default=131072, help="rows (212 B) of the fixed-size replay block each rank contributes to the per-move all-gather")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last one returned (actions, game records) as DIR/<name>.npy (rank 0)")
     args = ap.parse_args()
     if args.workload == "vanilla":
         G, sims, M, mode = args.games_per_gpu or 4096, args.sims or 300, args.max_nodes or 8192, "vanilla"
@@ -660,7 +628,7 @@ def main():
         G, sims, M, mode = args.games_per_gpu or 2048, args.sims or 1500, args.max_nodes or 32768, "dist"
         name = "BASELINE configs[4]: distributional head (agents/core_distributional.py), %d games/GPU (16384 over 8 GPUs), %d sims/move" % (G, sims)
     else:
-        G, sims, M, mode = args.games_per_gpu or 16384, args.sims or 500, args.max_nodes or 16384, "lp"
+        G, sims, M, mode = args.games_per_gpu or 16384, args.sims or 500, args.max_nodes or 8192, "lp"
         name = "BASELINE configs[2]: ValueSimLP + value net, %d games/GPU, %d sims/move" % (G, sims)
     headroom = args.gc_headroom if args.gc_headroom is not None else M * 5 // 32
     cfg = dict(games_per_gpu=G, sims=sims, max_nodes=M, mode=mode, eval=args.eval, workload_key=args.workload, gc_headroom=headroom,

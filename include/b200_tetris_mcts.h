@@ -35,8 +35,8 @@ enum { B200_MODE_LP = 0,        /* agents/ValueSimLP.py:13-70 */
        B200_MODE_DIST = 3 };    /* agents/core_distributional.py:82-124 driven as agents/DistValueSimOnline.py:36-75 sketches */
 enum { B200_EVAL_SYNTHETIC = 0, /* test evaluator (hash of the observation), shared with the CPU oracle */
        B200_EVAL_NET = 1,       /* model/model_vv.py Model_VV.inference, fp32 CUDA cores */
-       B200_EVAL_NET_TC = 2 };  /* same network on tcgen05 tensor cores (fp16 x 2 operand split, 3 products per product); in B200_MODE_DIST:
-                                   model/model_distributional.py on tcgen05 (csrc/distnet_tc.cuh) instead of the fp32 CUDA-core kernels */
+       B200_EVAL_NET_TC = 2 };  /* same network on wgmma tensor cores (fp16 x 2 operand split, 3 products per product); in B200_MODE_DIST:
+                                   model/model_distributional.py on tensor cores (csrc/distnet_tc.cuh) instead of the fp32 CUDA-core kernels */
 
 typedef struct b200_engine b200_engine;
 

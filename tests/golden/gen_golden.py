@@ -1,5 +1,6 @@
 """Generate tests/golden/*.npz by RUNNING THE REFERENCE ITSELF in the build container (it cannot travel to the GPU box):
   core_golden.npz     outputs of the reference's own agents/cppmodule/core.cpp (compiled unchanged -> oracle/_ref/core*.so)
+  core_live_golden.npz  the same core.cpp's select_trace_obs / backup_trace_obs on the seeded arenas of test_cpu_oracle_pins.py
   valuenet_golden.npz outputs of the reference's own model/model_vv.py Model_VV (torch CPU) with seeded weights
   dist_golden.npz     outputs of the reference's own numba cores agents/core_distributional.py (fastmath: pinned to 1e-5)
   agent_golden.npz    per-move statistics of the reference's own agents/ValueSimLP.py + agents/agent.py driving
@@ -23,7 +24,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path[:0] = [os.path.join(ROOT, "oracle"), os.path.join(ROOT, "tests")]
 import oracle_py as O  # noqa: E402
-from arena_gen import make_arena, boards, state_to_obskey  # noqa: E402
+from arena_gen import make_arena, near_tie_arena, boards, state_to_obskey  # noqa: E402
 
 
 def gen_core(core):
@@ -67,6 +68,22 @@ def gen_core(core):
     out["n_cases"] = len(cases)
     np.savez_compressed(os.path.join(HERE, "core_golden.npz"), **out)
     print("core_golden: %d cases" % len(cases))
+
+
+def gen_core_live(core):
+    """core_live_golden.npz: the reference's own core.cpp on the seeded arenas of tests/test_cpu_oracle_pins.py
+    (arena_gen.make_arena / near_tie_arena, regenerated by the test): trace of select_trace_obs and the arrays after backup_trace_obs."""
+    out = {}
+    for seed in range(30):
+        a = make_arena(1000 + seed, M=1024, max_depth=4 + seed % 7) if seed % 5 else near_tie_arena(seed)
+        tr = np.asarray(core.select_trace_obs(1, a["child"], a["visit"], a["value"], a["variance"], a["score"], a["n2o"], 1), np.int32)
+        b = {k: a[k].copy() for k in ("visit", "value", "variance")}
+        core.backup_trace_obs(tr, b["visit"], b["value"], b["variance"], a["n2o"], a["score"], 123.456, 7.89, 0.999)
+        out["trace_%d" % seed] = tr
+        for k in b:
+            out["%s_%d" % (k, seed)] = b[k]
+    np.savez_compressed(os.path.join(HERE, "core_live_golden.npz"), **out)
+    print("core_live_golden: 30 arenas")
 
 
 def gen_valuenet():
@@ -587,8 +604,11 @@ if __name__ == "__main__":
         gen_agent_modes(pt)
     elif "--agent-cpp" in sys.argv:
         gen_agent_cpp(pt)
+    elif "--core-live" in sys.argv:
+        gen_core_live(core)
     else:
         gen_core(core)
+        gen_core_live(core)
         gen_valuenet()
         gen_agent(pt)
         gen_agent_explicit_gc(pt)

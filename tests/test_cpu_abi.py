@@ -29,9 +29,9 @@ def test_header_symbols_exported(built):
         assert re.search(r"\bT %s\b" % n, nm), n
 
 
-def test_sm100a_code_present(built):
+def test_sm90a_code_present(built):
     out = subprocess.run(["cuobjdump", "-lelf", built], capture_output=True, text=True).stdout
-    assert "sm_100a" in out, out[:300]
+    assert "sm_90a" in out, out[:300]
 
 
 def test_no_cpu_fallback(built):

@@ -1,10 +1,9 @@
-"""Pin the CPU oracle (oracle/*.c) to the reference: (a) against the committed golden vectors that were produced by
-running the reference itself (tests/golden/gen_golden.py), (b) when /root/reference is present, against the
-reference's own compiled core.cpp on fresh seeded arenas."""
+"""Pin the CPU oracle (oracle/*.c) to the reference: against the committed golden vectors that were produced by
+running the reference itself (tests/golden/gen_golden.py), including the reference's own compiled core.cpp on
+seeded arenas."""
 import os
 
 import numpy as np
-import pytest
 
 from arena_gen import make_arena, near_tie_arena, state_to_obskey
 
@@ -205,18 +204,15 @@ def test_synthetic_eval_is_plain_integer_hash(oracle):
     assert 0 <= v < 64 and 0.5 <= var < 64.5 and v * 256 == int(v * 256) and (var - 0.5) * 16 == int((var - 0.5) * 16)
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference"), reason="reference tree absent (GPU box)")
-def test_live_against_reference_core(oracle):
-    oracle.build(ref=True)
-    _, core = oracle.mount_reference()
+def test_seeded_arenas_against_reference_core(oracle):
+    """select_trace_obs / backup_trace_obs of the reference's own compiled core.cpp on 30 seeded arenas, recorded in
+    core_live_golden.npz (tests/golden/gen_golden.py --core-live), vs the C oracle on the same arenas (exact)."""
+    z = np.load(os.path.join(GOLD, "core_live_golden.npz"))
     for seed in range(30):
         a = make_arena(1000 + seed, M=1024, max_depth=4 + seed % 7) if seed % 5 else near_tie_arena(seed)
-        tr = core.select_trace_obs(1, a["child"], a["visit"], a["value"], a["variance"], a["score"], a["n2o"], 1)
         mine = oracle.select_trace_obs(1, a["child"], a["visit"], a["value"], a["variance"], a["score"], a["n2o"], 1)
-        assert np.array_equal(np.asarray(tr), mine), seed
-        b1 = {k: a[k].copy() for k in ("visit", "value", "variance")}
-        b2 = {k: a[k].copy() for k in ("visit", "value", "variance")}
-        core.backup_trace_obs(np.asarray(tr, np.int32), b1["visit"], b1["value"], b1["variance"], a["n2o"], a["score"], 123.456, 7.89, 0.999)
-        oracle.backup_trace_obs(mine, b2["visit"], b2["value"], b2["variance"], a["n2o"], a["score"], 123.456, 7.89, 0.999)
-        for k in b1:
-            assert np.array_equal(b1[k], b2[k]), (seed, k)
+        assert np.array_equal(z["trace_%d" % seed], mine), seed
+        b = {k: a[k].copy() for k in ("visit", "value", "variance")}
+        oracle.backup_trace_obs(mine, b["visit"], b["value"], b["variance"], a["n2o"], a["score"], 123.456, 7.89, 0.999)
+        for k in b:
+            assert np.array_equal(z["%s_%d" % (k, seed)], b[k]), (seed, k)

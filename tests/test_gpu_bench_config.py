@@ -1,5 +1,5 @@
-"""Oracle parity AT THE BENCHMARKED CONFIGURATION (BASELINE configs[2] as bench.py runs it): 16384 games, max_nodes 16384, 500 simulations
-per move, the tcgen05 network (eval net_tc), set_gc_headroom(2560), overflow_reset, the production path (one CUDA graph per simulation
+"""Oracle parity AT THE BENCHMARKED CONFIGURATION (BASELINE configs[2] as bench.py runs it): 16384 games, max_nodes 8192, 500 simulations
+per move, the tensor-core network (eval net_tc), set_gc_headroom(1280), overflow_reset, the production path (one CUDA graph per simulation
 step, b200_play_move).  The C oracle agent cannot shadow 16384 games, so a sample of them is shadowed game for game: the oracle agents are fed
 the GPU network's outputs for the same boards (the LP search is deterministic given evaluator and piece sequence, SURVEY N3), make the same
 remove_nodes() calls the head-room policy makes (agents/agent.py:246-257 driven as in tests/golden/gen_golden.py gen_agent_explicit_gc) and
@@ -23,7 +23,7 @@ def test_bench_config_sampled_games_exact(gpu_lib, oracle, deep_lane):
     from tetris_mcts_b200 import pyTetris as PT
     from tetris_mcts_b200.engine import BatchedEngine
     from tetris_mcts_b200.model.model_vv import init_weights
-    n, M, sims, moves, headroom, seed = 16384, 16384, 500, 14, 16384 * 5 // 32, 123
+    n, M, sims, moves, headroom, seed = 16384, 8192, 500, 14, 8192 * 5 // 32, 123
     recs = PT.new_games(n, ARGS, np.arange(seed, seed + n, dtype=np.uint32))
     w = init_weights(0)
     eng = BatchedEngine(n, max_nodes=M, mode="lp", eval_kind="net_tc", weights=w, seed=seed, overflow_reset=True)

@@ -89,7 +89,7 @@ def test_dist_engine_matches_oracle_agent(gpu_lib, oracle):
 @pytest.mark.parametrize("kind", ["net", "net_tc"])
 def test_dist_network_matches_reference_golden(gpu_lib, oracle, kind):
     """model/model_distributional.py Net (torch CPU) outputs recorded in tests/golden/distnet_golden.npz; fp32 CUDA cores ("net") and the
-    tcgen05 path ("net_tc": fp16 x 2 operand split, north_star's 1e-5 on the probabilities)."""
+    tensor-core path ("net_tc": fp16 x 2 operand split, north_star's 1e-5 on the probabilities)."""
     from tetris_mcts_b200.engine import BatchedEngine
     z = np.load(os.path.join(os.path.dirname(__file__), "golden", "distnet_golden.npz"))
     w = oracle.seeded_dist_weights(int(z["seed"]))

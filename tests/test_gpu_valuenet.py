@@ -65,7 +65,7 @@ def test_matches_reference_golden(gpu_lib, oracle, kind):
 
 
 def test_tensor_core_conv_stack_matches_cuda_core_path(gpu_lib, oracle):
-    """Layer-level check of the tcgen05 shift-GEMM convolutions: the flatten input of fc1 from both device paths."""
+    """Layer-level check of the tensor-core shift-GEMM convolutions: the flatten input of fc1 from both device paths."""
     import ctypes as C
     from tetris_mcts_b200.engine import BatchedEngine
     from tetris_mcts_b200 import _lib as L

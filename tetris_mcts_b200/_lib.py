@@ -41,7 +41,7 @@ def lib():
     global _lib
     if _lib is None:
         if not os.path.exists(LIB_PATH):
-            raise ImportError("%s is missing: run `python -m tetris_mcts_b200.build` (nvcc, sm_100a). "
+            raise ImportError("%s is missing: run `python -m tetris_mcts_b200.build` (nvcc, sm_90a). "
                               "tetris_mcts_b200 has no CPU fallback." % LIB_PATH)
         L = C.CDLL(LIB_PATH)
         L.b200_last_error.restype = C.c_char_p

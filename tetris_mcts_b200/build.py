@@ -1,4 +1,4 @@
-"""Build libb200_tetris_mcts.so in-tree with nvcc for sm_100a (no JIT cache: the .so must travel with the repo)."""
+"""Build libb200_tetris_mcts.so in-tree with nvcc for sm_90a (H100) (no JIT cache: the .so must travel with the repo)."""
 import os
 import subprocess
 import sys
@@ -8,7 +8,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libb200_tetris_mcts.so")
 SOURCES = ["capi.cu", "trainer.cu"]
 HEADERS = ["tetris_dev.cuh", "search_dev.cuh", "kernels.cuh", "valuenet_simt.cuh", "valuenet_tc.cuh", "dist_dev.cuh", "distnet_simt.cuh"]
-FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-Xcompiler", "-fPIC", "-shared"]
+FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-Xcompiler", "-fPIC", "-shared"]
 
 
 def _stale():

@@ -55,7 +55,7 @@ struct b200_engine {
     float *d_act3 = nullptr; size_t act3_rows = 0;
     void *tc_state = nullptr; void *dn_tc_state = nullptr;
     bool have_dist_weights = false; float *d_dnw = nullptr; DistNetWeights DW{}; float *d_dn_act = nullptr; size_t dn_rows = 0;
-    int n_sm = 148;
+    int n_sm = 132;
     // timing
     bool timing = false;
     std::vector<cudaEvent_t> ev; size_t ev_used = 0;

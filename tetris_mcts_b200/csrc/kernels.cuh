@@ -1,6 +1,6 @@
-// kernels.cuh — the __global__ entry points of the engine (sm_100a).  Launch geometry: one 8-lane group per game,
-// 128-thread blocks (16 games per block), so G games = G/16 blocks; at G >= 16384 that is >= 1024 blocks = ~7 CTAs
-// per SM on 148 SMs.  The tree walk is pointer chasing (latency bound); occupancy, not ILP, hides HBM latency here.
+// kernels.cuh — the __global__ entry points of the engine (sm_90a).  Launch geometry: one 8-lane group per game,
+// 128-thread blocks (16 games per block), so G games = G/16 blocks; at G >= 16384 that is >= 1024 blocks = ~8 CTAs
+// per SM on 132 SMs.  The tree walk is pointer chasing (latency bound); occupancy, not ILP, hides HBM latency here.
 #pragma once
 #include "search_dev.cuh"
 
@@ -8,8 +8,8 @@ namespace b200 {
 
 #ifndef B200_PV_PREFETCH
 #define B200_PV_PREFETCH 0         // 0 off; 1 one request per row / statistics line; 2 every sector of the row the walk reads + the neighbouring
-#endif                             // statistics lines; 3 denser statistics coverage.  Measured on B200 (profiles/exp_variants_r2e.txt): the walk's
-                                   // per-level time does not move (4.81 -> 4.65 k clk) and k_select_expand gets 10-18 % SLOWER: off
+#endif                             // statistics lines; 3 denser statistics coverage.  Off: the prefetches were
+                                   // slower than the plain walk where they were tried
 #ifndef B200_GAMES_PER_WARP
 #define B200_GAMES_PER_WARP 4      // development aid (A/B): k_select_expand with 1 or 2 games per warp (the other 8-lane groups idle) to measure
                                    // what independent walks sharing a warp cost each other (every load waits for the slowest group's miss)
@@ -202,7 +202,7 @@ __device__ __forceinline__ void select_expand_group(const Arena &A, const Grp &g
 #if B200_PV_PREFETCH
     // Principal-variation prefetch (performance hint only): a game's walk mostly retraces its previous simulation's path — deep, narrow
     // trees grow at the end of one line — and every level of the walk is two DEPENDENT misses (row line, then the children's statistics;
-    // ~3.5 k clk of the ~4.5 k clk per level).  The previous trace is known (A.trace, A.trace_meta), so its row lines and the statistics
+    // most of the time of a level).  The previous trace is known (A.trace, A.trace_meta), so its row lines and the statistics
     // lines around each chosen child's observation are requested from L2 all at once, before the walk: where the new walk follows the
     // old path it finds them in L2 instead of paying DRAM + TLB latency level after level.  Siblings' observation ids are consecutive
     // (allocated by consecutive pops of the free list), so the line of the chosen child's statistics and its neighbours cover them.
@@ -585,8 +585,8 @@ __global__ void k_gc_request(Arena A, int min_free) {
 }
 
 // ---------------------------------------------------------------- deep lane (b200_set_deep_lane)
-// A simulation step's k_select_expand lasts as long as its DEEPEST walk (every game is resident, a level costs ~4.8 k clk), and a game's trace
-// length is predictable from its previous one (correlation 0.98, profiles/exp_trace_corr_r2.txt).  Once per move the games whose last trace
+// A simulation step's k_select_expand lasts as long as its DEEPEST walk (every game is resident, a level costs thousands of clocks), and a game's trace
+// length is predictable from its previous one (strongly correlated).  Once per move the games whose last trace
 // was longest (at most deep_cap of them) get a lane of their own: their select / collect / resume kernels run on a second stream next to the
 // other games' select AND network kernels, and join them before the (small) second network launch.  One CTA: histogram, threshold, two lists.
 __global__ void __launch_bounds__(1024) k_classify(Arena A, int deep_cap, int32_t *glist0, int32_t *n0, int32_t *glist1, int32_t *n1) {
@@ -664,7 +664,7 @@ __global__ void k_rollout(Arena A) {
 // occurs twice among the levels in flight (statistics are shared between nodes, agent.py:116-128) the lanes fall back
 // to the scalar walk.  Everything the backup never writes (trace, row fields, evaluator outputs) is loaded as early as
 // possible: the first window's node fields together with the leaf's child row, the next window's while the current one
-// is folded, so that only the statistics loads sit on the dependent chain (a DRAM access is ~2.4 k clk here).
+// is folded, so that only the statistics loads sit on the dependent chain (a DRAM access costs thousands of clocks).
 //
 // Two callers, one code path:
 //   NL = 8   the game's 8-lane group at the START of k_select_expand: the backup of simulation s runs fused in front of the

@@ -1,4 +1,4 @@
-// search_dev.cuh — device side of the per-move MCTS simulation loop (sm_100a).
+// search_dev.cuh — device side of the per-move MCTS simulation loop (sm_90a).
 //
 // One 8-lane group (quarter warp) owns one game's tree for the whole kernel; lane a (0..6) is child slot /
 // action a, lane 7 carries the node's own fields.  Trees never share memory between games, so there are no
@@ -30,7 +30,7 @@ enum : int { ST_OK = 0, ST_ARENA_FULL = 1, ST_TRACE_FULL = 2, ST_NEED_GC = 3, ST
 enum : int { LEAF_TERMINAL = 0, LEAF_EXPANDED = 1, LEAF_SUSPENDED = 2, LEAF_DONE = 3 };   // DONE: the trace has been backed up
 #ifndef B200_FUSED_BACKUP
 #define B200_FUSED_BACKUP 0   // 1: the backup of a game's previous simulation runs at the start of k_select_expand (kernels.cuh: backup_game);
-                              // exact (59 GPU tests) but measured 4 % slower than the separate warp-per-game k_backup on B200, so off
+                              // exact (GPU tests); off by default, the separate warp-per-game k_backup is the default
 #endif
 enum : int { PEND_NONE = 0, PEND_EXPAND = 1, PEND_ROOT = 2 };
 enum : int { MODE_LP = 0, MODE_SINGLE = 1, MODE_VANILLA = 2, MODE_DIST = 3 };
@@ -98,7 +98,7 @@ struct Grp {
 
 // The same interface with the CONSTANT full mask: legal only where all 32 lanes of the warp are converged (the four groups of a warp
 // in lockstep).  A sub-warp mask held in a register makes nvcc guard every shuffle / vote with MATCH.ANY + REDUX + VOTEU + a divergence
-// branch (~70 clk on the dependent chain, ~16 of them per level of the walk); with the literal 0xffffffff the guard disappears.
+// branch on the dependent chain, many of them per level of the walk; with the literal 0xffffffff the guard disappears.
 struct GrpW {
     static constexpr unsigned mask = 0xffffffffu;
     int lane; unsigned shift;
@@ -200,7 +200,7 @@ __device__ __forceinline__ uint32_t link_word(const Uniq &u) {
 #define B200_WARM_SELECT 0   // round 1 (moves 0-3, shallow trees): -1 % on k_select_expand; round 2 (moves 0-5, mean depth 36-62): +13 % -> off
 #endif
 // L2 residency hints (performance only).  One simulation step streams ~200 MB of activations (conv -> fc) and ~20 MB of new
-// nodes through the 126 MB L2, so without hints nothing of the trees survives from one step to the next although every step
+// nodes through the 50 MB L2, so without hints nothing of the trees survives from one step to the next although every step
 // re-walks the same top levels.  The first B200_L2_HOT_LEVELS levels of every game's walk (row line + statistics, ~3.7 MB per
 // level at 16384 games) are loaded / stored with an evict_last policy, the activation stream with evict_first.
 #ifndef B200_L2_HOT_LEVELS
@@ -502,7 +502,7 @@ __device__ __forceinline__ int select_trace(const Acc &acc, bool active, int roo
     // (trace / trace_meta are overwritten level by level as this walk advances), so lanes 0..3 of a group request, every four levels, the row
     // lines and statistics lines of the old path's levels +2..+5 from L2: where the new walk follows the old path it finds them there.  A
     // short look-ahead keeps the footprint at ~16 MB for 16384 games (requesting the whole old path before the walk — B200_PV_PREFETCH —
-    // is 277 MB per step against a 126 MB L2 and was slower).  The old entries are loaded one batch earlier than they are used.
+    // is 277 MB per step, several times the L2, and was slower).  The old entries are loaded one batch earlier than they are used.
     const int prev_len = active ? acc.prev_trace_len() : 0;
     int pf_idx = 0, pf_o = 0, it = 0;
     if (gp.lane < 4 && 2 + gp.lane < prev_len) acc.prev_trace(2 + gp.lane, pf_idx, pf_o);
@@ -555,7 +555,7 @@ __device__ __forceinline__ int select_trace(const Acc &acc, bool active, int roo
         // ---- phase 1: the levels the path cache still holds (see "path cache" above), ONE LANE PER LEVEL.  Given its entry and the next
         // level's own record, the pick of a cached level does not depend on the levels above it, so the eight lanes of a group evaluate
         // eight consecutive levels at once, each lane running core.h:83-105 over the seven child slots serially (no shuffles: ~9 x fewer
-        // warp instructions per level than eight lanes per level, which was issue bound at ~1.5 k clk per level).  The walk follows the
+        // warp instructions per level than eight lanes per level, which was issue bound).  The walk follows the
         // cached path up to the first level that picks another child than last time (served, with the new pick), is a leaf (served: the
         // walk ends), or cannot be served (entry missing, a child below `low` visits: check_low draws from the RNG in the uncached form).
         const int pcl = (walking && acc.pcg) ? acc.pc_len : 0;          // group-uniform
@@ -849,7 +849,7 @@ __device__ __noinline__ void reset_tree(const Arena &A, const Grp &gp, int g, in
 // 36 words per lane in registers across the loop and moving them with 36 shuffles per child spilled at 64 registers.)
 // Cache warming (performance hint only; results discarded, so exactness is untouched).  One expansion is seven new_node calls in
 // the reference's order, each a chain of dependent probes (node table -> record compare -> free list -> observation table ->
-// key compare ...); at 16384 games the arenas span ~80 GB, every first touch is a DRAM access (~2.4 k clk measured) and the chain
+// key compare ...); at 16384 games the arenas span tens of GB, every first touch is a DRAM access and the chain
 // was ~50 of them per expansion.  Before the ordered loop, lane a touches everything child a's new_node will read first: its two
 // table slots, then (on a hash match) the candidate record / row / key; lane 7 touches the counters and the free-list tails.  The
 // ordered loop then runs on L1/L2 hits.  Real loads (volatile asm) are used: a prefetch instruction may be dropped.

@@ -1,4 +1,4 @@
-// tetris_dev.cuh — device-side Tetris board step for sm_100a (bitboard form of /SPEC_PYTETRIS.md).
+// tetris_dev.cuh — device-side Tetris board step for sm_90a (bitboard form of /SPEC_PYTETRIS.md).
 //
 // Replaces the pyTetris C++ env at the reference call sites agents/agent.py:103,114,143-144 (copy_from/play/
 // getState), agents/cppmodule/agent.cpp:205,233,243 and play.py:150.  The whole game lives in registers:

@@ -287,7 +287,7 @@ __global__ void k_yogi(float *__restrict__ p, const float *__restrict__ grad, fl
     }
 }
 
-inline int nblk(size_t n, int t = 256) { size_t b = (n + t - 1) / t; return (int)(b < 1 ? 1 : (b > 148 * 16 ? 148 * 16 : b)); }
+inline int nblk(size_t n, int t = 256) { size_t b = (n + t - 1) / t; return (int)(b < 1 ? 1 : (b > 132 * 16 ? 132 * 16 : b)); }
 
 }  // namespace
 
@@ -322,7 +322,7 @@ template <bool TA, bool TB>
 int gemm(b200_trainer *t, const float *A, const float *B, float *C, int M, int N, int K, const float *bias, int relu) {
     int splits = 1;
     const int tiles = ((M + 63) / 64) * ((N + 63) / 64);
-    if (K >= 4096 && tiles < 148 * 2) { splits = (148 * 4 + tiles - 1) / tiles; if (splits > (K + 511) / 512) splits = (K + 511) / 512; }
+    if (K >= 4096 && tiles < 132 * 2) { splits = (132 * 4 + tiles - 1) / tiles; if (splits > (K + 511) / 512) splits = (K + 511) / 512; }
     int kps = ((K + splits - 1) / splits + 15) / 16 * 16;
     splits = (K + kps - 1) / kps;
     dim3 grid((N + 63) / 64, (M + 63) / 64, splits);

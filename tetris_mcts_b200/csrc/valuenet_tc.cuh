@@ -1,24 +1,23 @@
-// valuenet_tc.cuh — the reference value network (model/model_vv.py:13-52) on Blackwell tensor cores (sm_100a).
+// valuenet_tc.cuh — the reference value network (model/model_vv.py:13-52) on Hopper tensor cores (sm_90a, wgmma).
 //
 // Precision: north_star asks value outputs within 1e-5 of the reference's fp32.  Plain bf16/tf32/fp16 MMAs cannot
 // reach that, so every fp32 operand x is split into two fp16 terms x = x1 + x2 (11 + 11 = 22 mantissa bits, the
-// precision class of 3xTF32) and each product a*b is accumulated in fp32 (TMEM) as a1*b2 + a2*b1 + a1*b1 (the dropped
+// precision class of 3xTF32) and each product a*b is accumulated in fp32 as a1*b2 + a2*b1 + a1*b1 (the dropped
 // a2*b2 is < 2^-22 relative).  Operands are pre-scaled by exact powers of two (activations x16, weights x64) so that the
 // low terms stay in fp16's normal range; the epilogues undo the 2^10.  Three fp16 MMAs replace one fp32 product.
 //
-//   k_tc_conv  one persistent CTA per SM, four boards in flight (software pipeline):
-//              obs key -> im2col (exact fp16) -> conv1 as one K=16 MMA per M tile -> epilogue (bias, ReLU, split) -> smem
+//   k_tc_conv  persistent CTAs of TCC_WGS warpgroups; each warpgroup carries its own boards through the whole stack:
+//              obs key -> im2col (exact fp16) -> conv1 as one K=16 wgmma per 64-row tile -> epilogue (bias, ReLU, split) -> smem
 //              conv2 / conv3 as shift-GEMMs: activations live in shared memory channel-chunk-major
 //              ([8-channel chunk][pixel row][16 B]) on an 8-wide pixel grid, so the A operand of filter row dy is the SAME
-//              array started dy*8 rows later — a canonical no-swizzle K-major UMMA layout with SBO = 128 B,
-//              LBO = rows*16 B; the three horizontal taps are stacked along N (N = 96) and summed by the epilogue with
-//              two lane shuffles.  tcgen05.mma (M=128 pixels, K=16) issued by one thread, accumulators in TMEM,
-//              completion through tcgen05.commit -> mbarrier; epilogues read TMEM with tcgen05.ld, apply bias+ReLU,
-//              re-split (fp16 x2) and write the next layer's operand (or act3 to HBM in the FC kernel's tile layout).
-//   k_tc_fc    [R,1792] x [1792,256]: 128-row tiles, operands streamed by cp.async.bulk (1-D TMA) into a 5-stage
-//              mbarrier ring — both operands are stored in HBM already in the canonical UMMA layout, so one bulk copy
-//              per operand block needs no tensor map; warp-specialised (producer / MMA issuer / 4 epilogue warps);
-//              epilogue fuses bias+ReLU+fc_out+sigmoid+affine and scatters (v, var) to the requesting tree slot.
+//              array started dy*8 rows later — a no-swizzle K-major operand layout with SBO = 128 B, LBO = rows*16 B; the
+//              three horizontal taps are stacked along N (N = 96) and summed by the epilogue with two lane shuffles.
+//              wgmma.mma_async (M=64 pixels, K=16) from shared-memory descriptors, accumulators in registers; the epilogues
+//              apply bias+ReLU, re-split (fp16 x2) and write the next layer's operand (or act3 to HBM in the FC kernel's tile layout).
+//   k_tc_fc    [R,1792] x [1792,256]: 128-row tiles, operands streamed by cp.async.bulk (1-D TMA) into an mbarrier ring —
+//              both operands are stored in HBM already in the no-swizzle K-major layout, so one bulk copy per operand block needs
+//              no tensor map; one producer warp, two consumer warpgroups (64 rows each, N = 256 accumulators in registers);
+//              the epilogue fuses bias+ReLU+fc_out+sigmoid+affine and scatters (v, var) to the requesting tree slot.
 #pragma once
 #include <cuda_fp16.h>
 #include "search_dev.cuh"
@@ -32,21 +31,7 @@ __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)_
 __device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
 }
-#ifndef B200_MBAR_SUSPEND_NS
-#define B200_MBAR_SUSPEND_NS 0   // > 0: try_wait with this suspend-time hint (fewer turns of the polling loop; see profiles/exp_variants_r2j.txt)
-#endif
 __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
-#if B200_MBAR_SUSPEND_NS > 0
-    asm volatile(
-        "{\n"
-        ".reg .pred P1;\n"
-        "LAB_WAIT:\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1, %2;\n"
-        "@P1 bra DONE;\n"
-        "bra LAB_WAIT;\n"
-        "DONE:\n"
-        "}" ::"r"(smem_u32(bar)), "r"(parity), "r"((uint32_t)B200_MBAR_SUSPEND_NS) : "memory");
-#else
     asm volatile(
         "{\n"
         ".reg .pred P1;\n"
@@ -56,688 +41,381 @@ __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
         "bra LAB_WAIT;\n"
         "DONE:\n"
         "}" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
-#endif
 }
-// whole warp waits, one lane polls (32 lanes polling the same word is shared-memory traffic the MMA operand fetch competes with)
-__device__ __forceinline__ void mbar_wait_warp(uint64_t *bar, uint32_t parity);
 __device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-#ifndef B200_MBAR_FASTPATH
-#define B200_MBAR_FASTPATH 1   // most waits of the conv pipeline find their phase already complete: one warp-wide test_wait (a broadcast read)
-#endif                         // answers that without the lane-0 poll + __syncwarp round trip
-__device__ __forceinline__ bool mbar_test(uint64_t *bar, uint32_t parity) {
-    uint32_t ok;
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n"
-        "selp.u32 %0, 1, 0, p;\n"
-        "}" : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
-    return ok != 0u;
-}
-__device__ __forceinline__ void mbar_wait_warp(uint64_t *bar, uint32_t parity) {
-#if B200_MBAR_FASTPATH
-    if (__all_sync(0xffffffffu, mbar_test(bar, parity))) return;
-#endif
-    if ((threadIdx.x & 31) == 0) mbar_wait(bar, parity);
-    __syncwarp();
 }
 __device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
-__device__ __forceinline__ void bulk_g2s(void *dst, const void *src, uint32_t bytes, uint64_t *bar) {   // 1-D TMA (UBLKCP)
+__device__ __forceinline__ void bulk_g2s(void *dst, const void *src, uint32_t bytes, uint64_t *bar) {   // 1-D TMA
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst)),
                  "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
-// the same with an L2 eviction policy (search_dev.cuh: l2_policy_stream): act3 is written once and read once
-__device__ __forceinline__ void bulk_g2s_hint(void *dst, const void *src, uint32_t bytes, uint64_t *bar, uint64_t pol) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(smem_u32(dst)),
-                 "l"(src), "r"(bytes), "r"(smem_u32(bar)), "l"(pol) : "memory");
-}
-#ifndef B200_L2_STREAM_ACT3
-#define B200_L2_STREAM_ACT3 0   // measured on B200: k_tc_fc -5 %, but the tree kernels that follow +13 % (net loss); kept as a switch
-#endif
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+// the 128 threads of warpgroup wg (named barrier 1 + wg; barrier 0 is __syncthreads)
+__device__ __forceinline__ void wg_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }
 
-template <int COLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t *dst_smem) {   // whole warp
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "n"(COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int COLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {   // whole warp
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(COLS) : "memory");
-}
-
-// K-major, no-swizzle shared-memory matrix descriptor (cute::UMMA::SmemDescriptor, version 1):
-// rows of a core matrix are 16 B apart, 8-row groups SBO apart, the two 16-byte K chunks LBO apart.
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    return (uint64_t)((saddr & 0x3ffffu) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32) | (1ull << 46);
-}
-// kind::f16 instruction descriptor: D=f32 (bits 4-5 = 1), A=B=fp16 (format 0), both K-major, N>>3 at bit 17, M>>4 at bit 24
-__host__ __device__ constexpr uint32_t umma_idesc_f16(int M, int N) {
-    return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+// K-major, no-swizzle shared-memory matrix descriptor (sm_90 GMMA): rows of a core matrix are 16 B apart, 8-row groups
+// SBO apart, the two 16-byte K chunks of a K=16 step LBO apart; layout type 0 (interleave) in bits 62-63.
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+    return (uint64_t)((saddr & 0x3ffffu) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32);
 }
 constexpr float TC_SCALE_A = 16.f, TC_SCALE_W = 64.f, TC_UNSCALE = 1.f / 1024.f;
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from touching accumulator registers across wgmma_wait (the asm above does not name them)
+template <int R>
+__device__ __forceinline__ void fence_regs(float (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, fp16 operands from shared memory (both K-major), fp32 accumulators: thread t of the
+// warpgroup holds rows 16*(t/32) + (t%32)/4 (+8) and columns 8j + 2*(t%4) (+1) in d[4j + {0,1}] (row) / d[4j + {2,3}] (row + 8).
+// accumulate == 0 overwrites D.
+__device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
     asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-        "}" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {"
+        "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+        "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31"
+        "}, %32, %33, p, 1, 1, 0, 0;\n}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-__device__ __forceinline__ void umma_commit(uint64_t *bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+__device__ __forceinline__ void wgmma_n96(float (&d)[48], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %50, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n96k16.f32.f16.f16 {"
+        "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+        "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+        "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47"
+        "}, %48, %49, p, 1, 1, 0, 0;\n}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {   // lane i of the warp <- TMEM lane (quadrant*32 + i), 16 columns
-    uint32_t r[16];
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-                   "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-                 : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+__device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {"
+        "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+        "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+        "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,"
+        "%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63"
+        "}, %64, %65, p, 1, 1, 0, 0;\n}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, float (&v)[8]) {
-    uint32_t r[8];
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]) : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[i]);
+__device__ __forceinline__ void wgmma_n256(float (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %130, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 {"
+        "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+        "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+        "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,"
+        "%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,"
+        "%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,"
+        "%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95,"
+        "%96,%97,%98,%99,%100,%101,%102,%103,%104,%105,%106,%107,%108,%109,%110,%111,"
+        "%112,%113,%114,%115,%116,%117,%118,%119,%120,%121,%122,%123,%124,%125,%126,%127"
+        "}, %128, %129, p, 1, 1, 0, 0;\n}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+          "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+          "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+          "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+          "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+          "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+          "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+          "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+          "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-__device__ __forceinline__ void tmem_ld8_sum2(uint32_t taddr, float (&v)[8]) {
-    float w1[8], w2[8];
-    tmem_ld8(taddr + 32, w2);
-    tmem_ld8(taddr, w1);
-#pragma unroll
-    for (int i = 0; i < 8; ++i) v[i] = (w2[i] + w1[i]) * TC_UNSCALE;
-}
-
-// accumulator blocks a*W1 | a*W2 sit 32 columns apart: add the small one first, undo the operand scaling
-__device__ __forceinline__ void tmem_ld16_sum2(uint32_t taddr, float (&v)[16]) {
-    float w1[16], w2[16];
-    tmem_ld16(taddr + 32, w2);
-    tmem_ld16(taddr, w1);
-#pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = (w2[i] + w1[i]) * TC_UNSCALE;
-}
-
-// x = x1 + x2 with fp16 terms (round-to-nearest each step); eight fp32 values -> two 16-byte chunks (one per split)
-__device__ __forceinline__ void split8(const float (&x)[8], uint4 &c1, uint4 &c2) {
-    uint32_t a[4], b[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        const __half2 h = __floats2half2_rn(x[2 * i], x[2 * i + 1]);                 // one packed conversion per pair
-        const float2 f = __half22float2(h);
-        const __half2 l = __floats2half2_rn(x[2 * i] - f.x, x[2 * i + 1] - f.y);
-        a[i] = *reinterpret_cast<const uint32_t *>(&h); b[i] = *reinterpret_cast<const uint32_t *>(&l);
-    }
-    c1 = make_uint4(a[0], a[1], a[2], a[3]);
-    c2 = make_uint4(b[0], b[1], b[2], b[3]);
+// x = x1 + x2 with fp16 terms (round-to-nearest each step); two fp32 values -> one 32-bit word per split
+__device__ __forceinline__ void split2(float x0, float x1, uint32_t &hi, uint32_t &lo) {
+    const __half2 h = __floats2half2_rn(x0, x1);
+    const float2 f = __half22float2(h);
+    const __half2 l = __floats2half2_rn(x0 - f.x, x1 - f.y);
+    hi = *reinterpret_cast<const uint32_t *>(&h); lo = *reinterpret_cast<const uint32_t *>(&l);
 }
 
 // ---------------------------------------------------------------------------------------------------- conv kernel
-// Measured on B200 (scripts/probe/mma_probe.cu): a tcgen05.mma costs max(44.7, ~N/2) clk however small it is, so the
-// layers are cut into FEW, WIDE instructions.  The three horizontal taps (dx) of a 3x3 filter are stacked along N:
+// The three horizontal taps (dx) of a 3x3 filter are stacked along N, so a layer is a few wide MMAs instead of many narrow ones:
 //   D'[p][dx*32 + cout] = sum_{dy, cin} act[p + dy*8][cin] * W[dy][dx][cin][cout]          (A operand shifted by dy*8 rows only)
 //   out[p][cout]        = D'[p][0*32+cout] + D'[p+1][1*32+cout] + D'[p+2][2*32+cout]        (epilogue: two lane shuffles)
-// All three layers live on an 8-wide pixel grid (p = y*8 + x), so p+dx never leaves the 32-lane warp that owns the row.
-// 18 MMAs (3 dy x 2 channel halves x 3 split products, N = 96) replace the 36 narrow ones of the tap-by-tap form, and
-// conv1 (K = 9 taps, exact {-1,0,1} inputs) runs on the tensor core too from an im2col operand the workers build.
-// (Two independent worker sets of 8 warps x 16 channels on alternating boards, one MMA issuer each, were measured on B200 at 3 204 clk per
-// board against 2 751 with one set — profiles/exp_variants_r2f.txt — and removed.)
-#ifndef B200_CONV3_PAIR
-#define B200_CONV3_PAIR 0                   // 1: conv3 on a transposed grid that holds TWO boards per M = 128 tile (9 MMAs per board instead of 18), see below.
-                                            // Built, parity-green and measured on B200 (profiles/exp_variants_r2i.txt): tensor-pipe cycles -24 %, instructions -8 %, but the
-                                            // kernel is 7-8 % SLOWER (2 750 -> 3 080 clk per board): E3 now runs every other iteration and the 18-MMA burst of a pair
-                                            // lands in front of conv2, so the workers wait longer for c2 than conv3 saves.  Off.
-#endif
-#ifndef B200_CONV3_E3FIRST
-#define B200_CONV3_E3FIRST 0                // worker order inside an iteration: E3 | E2 | E1 instead of E2 | E3 | E1
-#endif
-#ifndef B200_CONV3_XPOSE
-#define B200_CONV3_XPOSE 1                  // the conv2 epilogue re-deals its values across the warp before the store (see there); 0: padded row groups instead
-#endif
-constexpr int TCC_WORKERS = 512;            // warps 0-15: the three epilogues
-constexpr int TCC_ISSUER = TCC_WORKERS / 32; // warp 16: MMA issuer of conv1 + conv2 (one elected lane)
-constexpr int TCC_ISSUER3 = TCC_ISSUER + 1; // warp 17: MMA issuer of conv3.  A 56-clk MMA costs its issuing thread ~8 dependent instructions
-                                            // (uniform-register moves + the elect loop) and that thread shares its scheduler with four busy
-                                            // worker warps: one issuer alone cannot keep the tensor pipe fed, two (on two schedulers) can.
-constexpr int TCC_LOADER = TCC_ISSUER + 2;  // warp 18: fetches the observation keys of the CTA's boards into a shared-memory ring
-constexpr int TCC_THREADS = TCC_WORKERS + 96;
+// All three layers live on an 8-wide pixel grid (p = y*8 + x).  In the wgmma accumulator layout pixel x of a row sits in lanes 4x..4x+3,
+// so p+1 / p+2 are 4 / 8 lanes further in the same register, and p+dx never leaves the row.  A layer is 18 MMAs per 64-row tile
+// (3 dy x 2 channel halves x 3 split products, N = 96); conv1 (K = 9 taps, exact {-1,0,1} inputs) runs on the tensor core too,
+// from an im2col operand the warpgroup builds.
+constexpr int TCC_WGS = 4;                  // warpgroups per CTA; each evaluates its own boards from key to act3
+constexpr int TCC_THREADS = TCC_WGS * 128;
 constexpr int TCC_R = 144;                  // activation rows per board: 18x8 grid (act1) / 16x8 grid + the dy shifts (act2)
 constexpr int TCC_WBLOCK = 2 * 2 * 96 * 16;  // one (dy, channel half) block: [weight split 2][chunk 2][n = dx*32 + cout][16 B]
 constexpr int TCC_WBYTES = 6 * TCC_WBLOCK;   // one conv layer = 36864 B
 constexpr int TCC_W1BYTES = 2 * 64 * 16;     // conv1: [chunk 2][n = split*32 + cout][16 B], k = tap (9 of 16 used)
-constexpr int TCC_SLOTS = 4;                // boards in flight (barrier rings, im2col operands)
-constexpr int TCC_KEYS_AHEAD = 4;           // observation keys the loader warp keeps in flight (registers)
-constexpr int TCC_RUN = 4;                  // consecutive requests handed to a CTA at a time (a power of two)
-constexpr int TCC_ASLOT = 2 * 4 * TCC_R * 16;    // operand buffer of one board: act1 [split][chunk 4][144 rows][16 B]
-constexpr int TCC_IMROWS = 256;             // im2col rows per board: 144 used, two M=128 tiles
-constexpr int TCC_IMSLOT = 2 * TCC_IMROWS * 16;  // [chunk 2][256 rows][16 B] fp16
-#if B200_CONV3_PAIR
-// conv3's output is 14 x 4 pixels: on the 8-wide grid an M = 128 tile carries 56 useful rows.  TRANSPOSED (row = x, 16 columns = y) the output of
-// one board is 4 x 16 = 64 rows, so two boards share a tile:  m = x*32 + (board & 1)*16 + y.  The conv2 epilogue writes act2 in that order
-// (6 x 32 = 192 rows per pair), the A operand of filter column dx is the pair's array started dx*32 rows later, the three VERTICAL taps are
-// stacked along N and summed by the epilogue (y + dy stays inside the board's 16 lanes).  18 MMAs per PAIR of boards.
-// The 8-row groups of the pair array are 144 B apart (SBO; 128 B + 16 B of padding): the conv2 epilogue's 16-byte stores of one pixel row
-// (x = 0..5: 4 groups apart) would otherwise all hit the same banks; with the padding it is a 3-way conflict.
-constexpr int TCC_ACT1_BUFS = 2;            // act1 is no longer overwritten by act2: E1(i) follows E2(i-2) (which waited for conv2(i-2)) in program order
-constexpr int TCC_TSLOTS = 3;               // TMEM: 3 x 128 columns for conv1 / conv2 in turn (conv1(i) is issued after a1(i-1), i.e. after E2(i-3)) + 96 for the pair
-#ifndef B200_CONV3_PSBO
-#define B200_CONV3_PSBO (B200_CONV3_XPOSE ? 128 : 144)
-#endif
-constexpr int TCC_PSBO = B200_CONV3_PSBO;
-constexpr int TCC_PCHUNK = 24 * TCC_PSBO;   // one 8-channel chunk of a pair: 192 rows
-constexpr int TCC_PSLOT = 2 * 4 * TCC_PCHUNK;    // [split][chunk 4][24 row groups][144 B]
-constexpr int TCC_PAIR_BUFS = 2;
-constexpr int TCC_TMEM_PAIR = TCC_TSLOTS * 128;  // first column of the pair accumulator
-#else
-constexpr int TCC_ACT1_BUFS = TCC_SLOTS;    // act2 overwrites the slot's act1 in place (conv2 has finished reading by then)
-constexpr int TCC_TSLOTS = TCC_SLOTS;       // a slot's three accumulators reuse the same 128 columns in turn
-constexpr int TCC_PSLOT = 0;
-constexpr int TCC_PAIR_BUFS = 0;
-#endif
+constexpr int TCC_RUN = 4;                  // consecutive requests handed to a warpgroup at a time
+constexpr int TCC_ASLOT = 2 * 4 * TCC_R * 16;    // operand buffer of one board: act1 / act2 [split][chunk 4][144 rows][16 B]
+constexpr int TCC_IMROWS = 192;             // im2col rows per board: 144 used, three 64-row tiles
+constexpr int TCC_IMSLOT = 2 * TCC_IMROWS * 16;  // [chunk 2][192 rows][16 B] fp16
 constexpr int TCC_OFF_W2 = 0;
 constexpr int TCC_OFF_W3 = TCC_OFF_W2 + TCC_WBYTES;
 constexpr int TCC_OFF_W1 = TCC_OFF_W3 + TCC_WBYTES;
 constexpr int TCC_OFF_A1 = TCC_OFF_W1 + TCC_W1BYTES;
-constexpr int TCC_OFF_PAIR = TCC_OFF_A1 + TCC_ACT1_BUFS * TCC_ASLOT;
-constexpr int TCC_OFF_IM = TCC_OFF_PAIR + TCC_PAIR_BUFS * TCC_PSLOT;
-constexpr int TCC_OFF_BIAS = TCC_OFF_IM + TCC_SLOTS * TCC_IMSLOT;   // 96 floats
-constexpr int TCC_OFF_KEY = TCC_OFF_BIAS + 96 * 4;                  // TCC_SLOTS x 32 words: the front-end warp's row table (20 rows: settled | piece << 16)
-constexpr int TCC_OFF_BAR = TCC_OFF_KEY + TCC_SLOTS * 32 * 4;       // 7 x TCC_SLOTS mbarriers + tmem pointer
-constexpr int TCC_SMEM = TCC_OFF_BAR + 7 * TCC_SLOTS * 8 + 16;
-constexpr int TCC_TMEM_COLS = 512;
+constexpr int TCC_OFF_IM = TCC_OFF_A1 + TCC_WGS * TCC_ASLOT;
+constexpr int TCC_OFF_BIAS = TCC_OFF_IM + TCC_WGS * TCC_IMSLOT;    // 96 floats, pre-scaled by TC_SCALE_A
+constexpr int TCC_OFF_KEY = TCC_OFF_BIAS + 96 * 4;                  // TCC_WGS x 32 words: row table (20 rows: settled | piece << 16)
+constexpr int TCC_SMEM = TCC_OFF_KEY + TCC_WGS * 32 * 4;
 constexpr int ACT3_KCHUNKS = 224;           // 1792 / 8
 static_assert(TCC_SMEM <= 227 * 1024, "k_tc_conv shared memory");
 
 struct TcWeights {
     const uint8_t *wc1;         // TCC_W1BYTES
     const uint8_t *wc2, *wc3;   // TCC_WBYTES each, already in the shared-memory layout
-    const uint8_t *wfc;         // [split 3][k16 block 112][chunk 2][n 256][16 B]
+    const uint8_t *wfc;         // [split 2][k16 block 112][chunk 2][n 256][16 B]
 };
 
-// act3 in HBM, FC-tile layout: [split][tile of 128 rows][k chunk 224][row 128][8 bf16], k' = (y*4 + x)*32 + c
+// act3 in HBM, FC-tile layout: [split][tile of 128 rows][k chunk 224][row 128][8 fp16], k' = (y*4 + x)*32 + c
 __device__ __forceinline__ size_t act3_off(int split, int n_tiles, int ridx, int kchunk) {
     return ((((size_t)split * n_tiles + (ridx >> 7)) * ACT3_KCHUNKS + kchunk) * 128 + (ridx & 127)) * 16;
 }
 
-// three 8-column accumulator slices (32 columns apart) of this thread's TMEM lane, one wait
-__device__ __forceinline__ void tmem_ld8x3(uint32_t taddr, float (&a)[8], float (&b)[8], float (&c)[8]) {
-    uint32_t r[24];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%24];\n"
-        "tcgen05.ld.sync.aligned.32x32b.x8.b32 {%8,%9,%10,%11,%12,%13,%14,%15}, [%25];\n"
-        "tcgen05.ld.sync.aligned.32x32b.x8.b32 {%16,%17,%18,%19,%20,%21,%22,%23}, [%26];\n"
-        "tcgen05.wait::ld.sync.aligned;"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]),
-          "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-          "=r"(r[21]), "=r"(r[22]), "=r"(r[23])
-        : "r"(taddr), "r"(taddr + 32), "r"(taddr + 64)
-        : "memory");
-#pragma unroll
-    for (int i = 0; i < 8; ++i) { a[i] = __uint_as_float(r[i]); b[i] = __uint_as_float(r[8 + i]); c[i] = __uint_as_float(r[16 + i]); }
-}
-
-// two 8-column accumulator slices (32 columns apart), one wait
-__device__ __forceinline__ void tmem_ld8x2(uint32_t taddr, float (&a)[8], float (&b)[8]) {
-    uint32_t r[16];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%16];\n"
-        "tcgen05.ld.sync.aligned.32x32b.x8.b32 {%8,%9,%10,%11,%12,%13,%14,%15}, [%17];\n"
-        "tcgen05.wait::ld.sync.aligned;"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]),
-          "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr), "r"(taddr + 32)
-        : "memory");
-#pragma unroll
-    for (int i = 0; i < 8; ++i) { a[i] = __uint_as_float(r[i]); b[i] = __uint_as_float(r[8 + i]); }
-}
-
-// out[p] = D'[p][dx=0] + D'[p+1][dx=1] + D'[p+2][dx=2] for the 8 couts of this warp's chunk (see the header of this section)
-__device__ __forceinline__ void tmem_ld_conv_sum(uint32_t taddr, float (&v)[8]) {
-    float d0[8], d1[8], d2[8];
-    tmem_ld8x3(taddr, d0, d1, d2);
-#pragma unroll
-    for (int e = 0; e < 8; ++e) {
-        const float s1 = __shfl_down_sync(0xffffffffu, d1[e], 1), s2 = __shfl_down_sync(0xffffffffu, d2[e], 2);
-        v[e] = (s2 + s1) + d0[e];          // still carries the operand scaling 2^10: the callers fold TC_UNSCALE into their bias fma
-    }
-}
-
-// One 3x3 layer = 18 tcgen05.mma of N = 96: for each (dy, channel half): a1*W1, a1*W2, a2*W1 into the same 96 columns.
-__device__ __forceinline__ void issue_conv_layer(uint32_t tmem_d, uint32_t a_addr, uint32_t w_addr) {
-    const uint64_t a0 = umma_desc(a_addr, TCC_R * 16, 128), b0 = umma_desc(w_addr, 96 * 16, 128);
-    constexpr uint32_t idesc = umma_idesc_f16(128, 96);
+// One 3x3 layer on one 64-row tile = 18 wgmma of N = 96: for each (dy, channel half): a1*W1, a1*W2, a2*W1 into the same 96 columns.
+__device__ __forceinline__ void issue_conv_layer(float (&d)[48], uint32_t a_addr, uint32_t w_addr) {
+    const uint64_t a0 = gmma_desc(a_addr, TCC_R * 16, 128), b0 = gmma_desc(w_addr, 96 * 16, 128);
 #pragma unroll
     for (int dy = 0; dy < 3; ++dy) {
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             const uint32_t a_hi = 2 * h * TCC_R + dy * 8, a_lo = a_hi + 4 * TCC_R;          // 16-byte units
             const uint32_t b_hi = (dy * 2 + h) * (TCC_WBLOCK / 16), b_lo = b_hi + 2 * 96;
-            umma_f16(tmem_d, a0 + a_hi, b0 + b_hi, idesc, (dy | h) ? 1u : 0u);
-            umma_f16(tmem_d, a0 + a_hi, b0 + b_lo, idesc, 1u);
-            umma_f16(tmem_d, a0 + a_lo, b0 + b_hi, idesc, 1u);
+            wgmma_n96(d, a0 + a_hi, b0 + b_hi, (dy | h) ? 1u : 0u);
+            wgmma_n96(d, a0 + a_hi, b0 + b_lo, 1u);
+            wgmma_n96(d, a0 + a_lo, b0 + b_hi, 1u);
         }
     }
 }
 
-#if B200_CONV3_PAIR
-// conv3 of a PAIR of boards (see TCC_PSBO above): for each (dx, channel half): a1*W1, a1*W2, a2*W1; weights n = dy*32 + cout.
-__device__ __forceinline__ void issue_conv3_pair(uint32_t tmem_d, uint32_t a_addr, uint32_t w_addr) {
-    const uint64_t a0 = umma_desc(a_addr, TCC_PCHUNK, TCC_PSBO), b0 = umma_desc(w_addr, 96 * 16, 128);
-    constexpr uint32_t idesc = umma_idesc_f16(128, 96);
+// the conv1 operand of one board: row p = y*8 + x of the 18x8 output grid, k = tap = dy*3 + dx (fp16, exact {-1,0,1});
+// taps 0..7 as ONE 16-byte store, tap 8 in the second k chunk
+__device__ __forceinline__ void build_im2col3(uint8_t *im, const uint32_t *tab, int wt) {
+    for (int p = wt; p < TCC_R; p += 128) {
+        const int y = p >> 3, x = p & 7;
+        uint32_t hv[9];
 #pragma unroll
-    for (int dx = 0; dx < 3; ++dx) {
+        for (int dy = 0; dy < 3; ++dy) {
+            const uint32_t rw = tab[y + dy] >> x;
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            const uint32_t a_hi = (2 * h * TCC_PCHUNK + dx * 4 * TCC_PSBO) / 16, a_lo = a_hi + 4 * TCC_PCHUNK / 16;   // 16-byte units
-            const uint32_t b_hi = (dx * 2 + h) * (TCC_WBLOCK / 16), b_lo = b_hi + 2 * 96;
-            umma_f16(tmem_d, a0 + a_hi, b0 + b_hi, idesc, (dx | h) ? 1u : 0u);
-            umma_f16(tmem_d, a0 + a_hi, b0 + b_lo, idesc, 1u);
-            umma_f16(tmem_d, a0 + a_lo, b0 + b_hi, idesc, 1u);
+            for (int dx = 0; dx < 3; ++dx)       // 1 settled, -1 falling piece, 0 empty (model_vv.py:212)
+                hv[dy * 3 + dx] = ((rw >> dx) & 1u) * 0x3C00u | ((rw >> (16 + dx)) & 1u) * 0xBC00u;
         }
+        *reinterpret_cast<uint4 *>(im + p * 16) =
+            make_uint4(hv[0] | (hv[1] << 16), hv[2] | (hv[3] << 16), hv[4] | (hv[5] << 16), hv[6] | (hv[7] << 16));   // taps 0..7
+        *reinterpret_cast<uint32_t *>(im + TCC_IMROWS * 16 + p * 16) = hv[8];                                        // tap 8
     }
 }
-#endif
 
 __global__ void __launch_bounds__(TCC_THREADS, 1)
 k_tc_conv(NetWeights W, TcWeights TW, const uint2 *req, const int32_t *n_req_ptr, const int32_t *first_ptr, const uint32_t *keys, int M, uint8_t *act3,
           int n_tiles, unsigned long long *prof) {
-#define PROF_T(i) do { if (prof && do_prof) { long long _n = clock64(); pacc[i] += _n - ptick; ptick = _n; } } while (0)
     extern __shared__ __align__(128) uint8_t smem[];
     float *sB = reinterpret_cast<float *>(smem + TCC_OFF_BIAS);
-    uint64_t *bars = reinterpret_cast<uint64_t *>(smem + TCC_OFF_BAR);
-    constexpr int NS = TCC_SLOTS;
-    uint64_t *bar_c1 = bars, *bar_c2 = bars + NS, *bar_c3 = bars + 2 * NS;             // tensor core -> workers: layer of slot done
-    uint64_t *bar_a0 = bars + 3 * NS, *bar_a1 = bars + 4 * NS, *bar_a2 = bars + 5 * NS; // workers -> issuer: operand of slot written
-#if B200_CONV3_PAIR
-    uint64_t *bar_e3 = bars + 6 * NS;                                                   // workers -> conv3 issuer: the pair accumulator has been read
-#endif
-    uint32_t *sKey = reinterpret_cast<uint32_t *>(smem + TCC_OFF_KEY);
-    uint32_t *tmem_ptr = reinterpret_cast<uint32_t *>(smem + TCC_OFF_BAR + 7 * NS * 8);
-    const int t = threadIdx.x, warp = t >> 5, lane = t & 31;
-    // ---- one-time setup: weights into smem, zeroed operands, barriers, TMEM
+    const int t = threadIdx.x, wg = t >> 7, wt = t & 127, w = wt >> 5, lane = t & 31;
+    // ---- one-time setup: weights into smem, zeroed operands (the im2col rows past 144 stay zero)
     for (int i = t; i < TCC_WBYTES / 16; i += TCC_THREADS) {
         reinterpret_cast<uint4 *>(smem + TCC_OFF_W2)[i] = reinterpret_cast<const uint4 *>(TW.wc2)[i];
         reinterpret_cast<uint4 *>(smem + TCC_OFF_W3)[i] = reinterpret_cast<const uint4 *>(TW.wc3)[i];
     }
     for (int i = t; i < TCC_W1BYTES / 16; i += TCC_THREADS) reinterpret_cast<uint4 *>(smem + TCC_OFF_W1)[i] = reinterpret_cast<const uint4 *>(TW.wc1)[i];
     for (int i = t; i < (TCC_OFF_BIAS - TCC_OFF_A1) / 16; i += TCC_THREADS) reinterpret_cast<uint4 *>(smem + TCC_OFF_A1)[i] = make_uint4(0, 0, 0, 0);
-    if (t < 32) { sB[t] = W.b1[t]; sB[32 + t] = W.b2[t]; sB[64 + t] = W.b3[t]; }
-    if (t == 0) {
-        for (int i = 0; i < 3 * NS; ++i) mbar_init(&bars[i], 1);
-        for (int i = 3 * NS; i < 4 * NS; ++i) mbar_init(&bars[i], 1);                      // a0: the front-end warp alone builds the conv1 operand
-        for (int i = 4 * NS; i < 6 * NS; ++i) mbar_init(&bars[i], TCC_WORKERS / 32);   // a1, a2: one arrival per worker warp
-        for (int i = 6 * NS; i < 7 * NS; ++i) mbar_init(&bars[i], TCC_WORKERS / 32);          // e3 (entry 0 used): one arrival per worker warp
-        fence_barrier_init();
-    }
-    if (warp == TCC_ISSUER) tmem_alloc<TCC_TMEM_COLS>(tmem_ptr);
+    // relu(x * 2^-10 + b) * 16 == relu(fma(x, 2^-6, 16 b)) bit for bit (scaling by a power of two commutes with rounding): the biases
+    // are kept pre-scaled and an epilogue value costs one fma + one max
+    if (t < 32) { sB[t] = W.b1[t] * TC_SCALE_A; sB[32 + t] = W.b2[t] * TC_SCALE_A; sB[64 + t] = W.b3[t] * TC_SCALE_A; }
     fence_async_smem();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
     const int first = first_ptr ? *first_ptr : 0;      // this launch evaluates the requests [first, *n_req_ptr) (the deep lane's: see k_merge_requests)
     const int n_req = *n_req_ptr - first;
-    // Boards are handed out in runs of TCC_RUN consecutive requests (neighbouring act3 rows get written close in time; short runs keep
-    // the CTAs' board counts within TCC_RUN of each other: with runs of 8 the last CTAs had 4 % more work); board i of
-    // this CTA's sequence lives in slot i % 4.  Four boards are in flight at different stages (software pipeline):
-    //   workers, iteration i :  S0(i) im2col | E2(i-2) conv2 epilogue | E3(i-3) conv3 epilogue | E1(i) conv1 epilogue
-    //   issuer,  iteration i :  conv2(i-1) | conv1(i) | conv3(i-2), each as soon as the workers have written its operand
-    // The order is chosen so that the tensor pipe never runs dry: conv2(i-1)'s operand was finished at the end of the
-    // previous iteration (E1 comes last), conv1(i) is short and queued behind it, conv3(i-2)'s operand (E2) is ready long
-    // before conv2 retires; the workers drain older boards (E2, E3) while conv2 runs and reach E1(i) after conv1(i) is done.
+    // boards are handed out in runs of TCC_RUN consecutive requests (neighbouring act3 rows get written close in time)
+    const int n_workers = (int)gridDim.x * TCC_WGS, wid = (int)blockIdx.x * TCC_WGS + wg;
     const int n_runs = (n_req + TCC_RUN - 1) / TCC_RUN;
     int n_local = 0;
-    for (int run = blockIdx.x; run < n_runs; run += gridDim.x) n_local += min(TCC_RUN, n_req - run * TCC_RUN);
-    auto board_of = [&](int i) -> int { return first + ((i / TCC_RUN) * (int)gridDim.x + (int)blockIdx.x) * TCC_RUN + (i % TCC_RUN); };
-    if (warp == TCC_ISSUER) {
-        // ===================================================== MMA issuer
-        if (lane == 0) {
-            const uint32_t s_w1 = smem_u32(smem + TCC_OFF_W1), s_w2 = smem_u32(smem + TCC_OFF_W2), s_w3 = smem_u32(smem + TCC_OFF_W3);
-            const uint32_t s_act = smem_u32(smem + TCC_OFF_A1), s_im = smem_u32(smem + TCC_OFF_IM);
-            const bool do_prof = blockIdx.x == 0;
-            long long pacc[16] = {0}, ptick = clock64();
-            for (int i = 0; i < n_local + 1; ++i) {
-                // conv1(i) goes FIRST: its operand comes from the front-end warp (boards ahead), its accumulator columns were last read by
-                // E3(i-4), and E1(i-1) — the last phase of the workers' previous iteration, a1(i-1) — implies that E3(i-4) is done.  With
-                // conv1 queued behind the 18 MMAs of conv2 (round 1: the workers built the operand, so it could not be ready earlier) the
-                // workers stood at E1(i) for ~1 k clk per board waiting for it.
-                if (i >= 1) {
-                    const int j = i - 1, slot = j % NS;
-                    mbar_wait(&bar_a1[slot], (uint32_t)(j / NS) & 1u);
-                    PROF_T(10);
-                }
-                if (i < n_local) {                               // conv1 (model_vv.py:32): im2col [256 x 16] x W1 [16 x 64], two M tiles
-                    const int slot = i % NS;
-                    mbar_wait(&bar_a0[slot], (uint32_t)(i / NS) & 1u);
-                    PROF_T(8);
-                    tc_fence_after();
-                    const uint64_t a0 = umma_desc(s_im + slot * TCC_IMSLOT, TCC_IMROWS * 16, 128), b0 = umma_desc(s_w1, 64 * 16, 128);
-                    umma_f16(tmem_base + (i % TCC_TSLOTS) * 128, a0, b0, umma_idesc_f16(128, 64), 0u);
-                    umma_f16(tmem_base + (i % TCC_TSLOTS) * 128 + 64, a0 + 128, b0, umma_idesc_f16(128, 64), 0u);
-                    umma_commit(&bar_c1[slot]);
-                    PROF_T(9);
-                }
-                if (i >= 1) {                                    // conv2 (model_vv.py:34): act1 on the 18x8 grid
-                    const int j = i - 1, slot = j % NS;
-                    tc_fence_after();
-                    issue_conv_layer(tmem_base + (j % TCC_TSLOTS) * 128, s_act + (j % TCC_ACT1_BUFS) * TCC_ASLOT, s_w2);
-                    umma_commit(&bar_c2[slot]);
-                    PROF_T(11);
-                }
+    for (int run = wid; run < n_runs; run += n_workers) n_local += min(TCC_RUN, n_req - run * TCC_RUN);
+    auto board_of = [&](int i) -> int { return first + ((i / TCC_RUN) * n_workers + wid) * TCC_RUN + (i % TCC_RUN); };
+    uint8_t *act = smem + TCC_OFF_A1 + wg * TCC_ASLOT, *im = smem + TCC_OFF_IM + wg * TCC_IMSLOT;
+    uint32_t *sKey = reinterpret_cast<uint32_t *>(smem + TCC_OFF_KEY) + wg * 32;
+    const uint32_t s_act = smem_u32(act), s_im = smem_u32(im);
+    const uint32_t s_w1 = smem_u32(smem + TCC_OFF_W1), s_w2 = smem_u32(smem + TCC_OFF_W2), s_w3 = smem_u32(smem + TCC_OFF_W3);
+    const int qd = lane & 3, rl = lane >> 2;             // accumulator rows 16w + rl (+8), columns 8j + 2qd (+1)
+    constexpr float K23 = TC_UNSCALE * TC_SCALE_A, K1 = TC_SCALE_A / TC_SCALE_W;
+    constexpr int SPLIT = 4 * TCC_R * 16;                // act1 / act2: second fp16 term
+    const bool do_prof = prof && blockIdx.x == 0 && t == 0;
+    long long pacc[4] = {0, 0, 0, 0}, ptick = clock64();
+    auto prof_t = [&](int k) { if (do_prof) { const long long n = clock64(); pacc[k] += n - ptick; ptick = n; } };
+    // A key is a random 48-byte read from an arena of tens of GB: lanes 0..11 of warp 0 fetch the NEXT board's key while this one is evaluated
+    auto fetch = [&](int i) -> uint32_t {
+        if (i >= n_local || lane >= 12) return 0u;
+        const uint2 rq = req[board_of(i)];
+        return keys[((size_t)rq.x * M + (rq.y & 0x0fffffffu)) * KEY_WORDS + lane];
+    };
+    uint32_t kw = w == 0 ? fetch(0) : 0u;
+    for (int i = 0; i < n_local; ++i) {
+        const int ridx = board_of(i);
+        if (w == 0) {
+            // row table: lane r < 20 holds board row r: settled cells in bits 0..9, the falling piece's cells in bits 16..25
+            const uint32_t rowpair = __shfl_sync(0xffffffffu, kw, (lane >> 1) & 15), pcs = __shfl_sync(0xffffffffu, kw, 10);
+            uint32_t tab = (rowpair >> ((lane & 1) * 16)) & 0x3ffu;
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {                        // the falling piece's cells (sorted bytes of key word 10)
+                const uint32_t cell = (pcs >> (8 * k)) & 0xffu, pr = (cell * 205u) >> 11, pcol = cell - pr * 10u;
+                tab |= (pr == (uint32_t)lane ? 1u : 0u) << (16 + pcol);
             }
-            if (prof && do_prof) for (int i = 8; i < 12; ++i) atomicAdd(&prof[i], (unsigned long long)pacc[i]);
+            kw = fetch(i + 1);
+            if (lane < 20) sKey[lane] = tab;
         }
-    } else if (warp == TCC_ISSUER3) {
-        // ===================================================== second MMA issuer: conv3 (model_vv.py:36)
-        if (lane == 0) {
-            const uint32_t s_w3 = smem_u32(smem + TCC_OFF_W3);
-            const bool do_prof = blockIdx.x == 0;
-            long long pacc[16] = {0}, ptick = clock64();
-#if B200_CONV3_PAIR
-            // pair k = boards 2k, 2k+1 of this CTA.  a2 of the pair's LAST board implies (program order of every worker warp) that the other
-            // board's act2 is written and that E3(k-2) (which waited for conv3(k-2)) is done with the pair buffer.  The ONE pair accumulator
-            // is handed back explicitly (e3): a last pair of one board is ready (a2(2k), first phase of iteration 2k+2) before E3(k-1) of
-            // that same iteration has read it.
-            const uint32_t s_pair = smem_u32(smem + TCC_OFF_PAIR);
-            for (int k = 0; 2 * k < n_local; ++k) {
-                const int jl = min(2 * k + 1, n_local - 1);
-                mbar_wait(&bar_a2[jl % NS], (uint32_t)(jl / NS) & 1u);
-                if (k >= 1) mbar_wait(&bar_e3[0], (uint32_t)(k - 1) & 1u);
-                PROF_T(12);
-                tc_fence_after();
-                issue_conv3_pair(tmem_base + TCC_TMEM_PAIR, s_pair + (k % TCC_PAIR_BUFS) * TCC_PSLOT, s_w3);
-                umma_commit(&bar_c3[k & 1]);
-                PROF_T(13);
-            }
-#else
-            const uint32_t s_act = smem_u32(smem + TCC_OFF_A1);
-            for (int j = 0; j < n_local; ++j) {                  // act2 on the 16x8 grid
-                const int slot = j % NS;
-                mbar_wait(&bar_a2[slot], (uint32_t)(j / NS) & 1u);
-                PROF_T(12);
-                tc_fence_after();
-                issue_conv_layer(tmem_base + slot * 128, s_act + slot * TCC_ASLOT, s_w3);
-                umma_commit(&bar_c3[slot]);
-                PROF_T(13);
-            }
-#endif
-            if (prof && do_prof) for (int i = 12; i < 14; ++i) atomicAdd(&prof[i], (unsigned long long)pacc[i]);
-        }
-    } else if (warp == TCC_LOADER) {
-        // ===================================================== front end (one warp): observation key -> conv1 operand.
-        // A key is a random 48-byte read from an arena of tens of GB (~2.4 k clk); TCC_KEYS_AHEAD of them are kept in flight.  The same
-        // warp then builds the im2col operand of conv1 (fp16, exact {-1,0,1}): row p = y*8 + x of the 18x8 output grid, k = tap = dy*3 + dx,
-        // taps 0..7 as ONE 16-byte store, tap 8 in the second k chunk.  (Round 1 had all 16 worker warps build it, 27 % of their cycle;
-        // one warp running up to TCC_SLOTS boards ahead of the epilogues does it off the workers' critical path.)
-        uint2 rqs = make_uint2(0, 0);
-        uint32_t kq[TCC_KEYS_AHEAD];
-        auto fetch = [&](int i) -> uint32_t {                       // whole warp; board i of this CTA (i < n_local)
-            if ((i & 31) == 0 && i + lane < n_local) rqs = req[board_of(i + lane)];
-            const uint32_t gx = __shfl_sync(0xffffffffu, rqs.x, i & 31), gy = __shfl_sync(0xffffffffu, rqs.y, i & 31);
-            return lane < 12 ? keys[((size_t)gx * M + (gy & 0x0fffffffu)) * KEY_WORDS + lane] : 0u;
-        };
+        wg_sync(wg);                                             // also: every warp has waited for the previous board's last MMAs
+        build_im2col3(im, sKey, wt);
+        fence_async_smem();
+        wg_sync(wg);
+        prof_t(0);
+        // ---- conv1 (model_vv.py:32): im2col [192 x 16] x W1 [16 x 64] in three 64-row tiles; epilogue: bias + ReLU + split -> act1
+#pragma unroll 1
+        for (int mt = 0; mt < 3; ++mt) {
+            float d[32];
 #pragma unroll
-        for (int j = 0; j < TCC_KEYS_AHEAD; ++j) kq[j] = j < n_local ? fetch(j) : 0u;
-        for (int i0 = 0; i0 < n_local; i0 += TCC_KEYS_AHEAD) {
+            for (int k = 0; k < 32; ++k) d[k] = 0.f;
+            wgmma_fence();
+            wgmma_n64(d, gmma_desc(s_im + mt * 1024, TCC_IMROWS * 16, 128), gmma_desc(s_w1, 64 * 16, 128), 0u);
+            wgmma_commit();
+            wgmma_wait<0>();
+            fence_regs(d);
 #pragma unroll
-            for (int j = 0; j < TCC_KEYS_AHEAD; ++j) {
-                const int i = i0 + j;
-                if (i >= n_local) break;
-                const int slot = i % NS;
-                // row table: lane r < 20 holds board row r: settled cells in bits 0..9, the falling piece's cells in bits 16..25
-                const uint32_t kw = kq[j];
-                const uint32_t rowpair = __shfl_sync(0xffffffffu, kw, (lane >> 1) & 15), pcs = __shfl_sync(0xffffffffu, kw, 10);
-                uint32_t tab = (rowpair >> ((lane & 1) * 16)) & 0x3ffu;
+            for (int h = 0; h < 2; ++h) {
+                const int r = mt * 64 + 16 * w + 8 * h + rl;
+                if (r < TCC_R) {
 #pragma unroll
-                for (int k = 0; k < 4; ++k) {                    // the falling piece's cells (sorted bytes of key word 10)
-                    const uint32_t cell = (pcs >> (8 * k)) & 0xffu, pr = (cell * 205u) >> 11, pcol = cell - pr * 10u;
-                    tab |= (pr == (uint32_t)lane ? 1u : 0u) << (16 + pcol);
+                    for (int j = 0; j < 4; ++j) {                // cout 8j + 2qd + e: weight split 1 sits 32 columns (4 blocks) further
+                        const int c = 8 * j + 2 * qd;
+                        const float o0 = fmaxf(fmaf(d[4 * (j + 4) + 2 * h] + d[4 * j + 2 * h], K1, sB[c]), 0.f);
+                        const float o1 = fmaxf(fmaf(d[4 * (j + 4) + 2 * h + 1] + d[4 * j + 2 * h + 1], K1, sB[c + 1]), 0.f);
+                        uint32_t hi, lo;
+                        split2(o0, o1, hi, lo);
+                        uint8_t *dst = act + (j * TCC_R + r) * 16 + qd * 4;
+                        *reinterpret_cast<uint32_t *>(dst) = hi;
+                        *reinterpret_cast<uint32_t *>(dst + SPLIT) = lo;
+                    }
                 }
-                if (i + TCC_KEYS_AHEAD < n_local) kq[j] = fetch(i + TCC_KEYS_AHEAD);            // next key of this register, in flight while the operand is built
-                if (i >= NS) mbar_wait_warp(&bar_c1[slot], (uint32_t)((i - NS) / NS) & 1u);     // conv1 of the slot's previous board has read its operand
-                if (lane < 20) sKey[slot * 32 + lane] = tab;
-                __syncwarp();
-                uint8_t *im = smem + TCC_OFF_IM + slot * TCC_IMSLOT;
+            }
+        }
+        fence_async_smem();
+        wg_sync(wg);
+        prof_t(1);
+        // ---- conv2 (model_vv.py:34) on act1 (18x8 grid) and conv3 (:36) on act2 (16x8 grid).  act2 overwrites act1 in place: the epilogue
+        // of tile 0 writes rows 0..63, tile 1 reads rows 64..143 only.  Rows of act2 that no valid conv3 output reads keep act1 values.
+#pragma unroll 1
+        for (int layer = 0; layer < 2; ++layer) {
+            const float *bias = sB + 32 * (layer + 1);
+#pragma unroll 1
+            for (int mt = 0; mt < 2; ++mt) {
+                float d[48];
 #pragma unroll
-                for (int pp = 0; pp < 5; ++pp) {                 // 144 pixels over 32 lanes
-                    const int p = pp * 32 + lane;
-                    if (p < 144) {
-                        const int y = p >> 3, x = p & 7;
-                        uint32_t hv[9];
+                for (int k = 0; k < 48; ++k) d[k] = 0.f;
+                wgmma_fence();
+                issue_conv_layer(d, s_act + mt * 1024, layer ? s_w3 : s_w2);
+                wgmma_commit();
+                wgmma_wait<0>();
+                fence_regs(d);
 #pragma unroll
-                        for (int dy = 0; dy < 3; ++dy) {
-                            const uint32_t rw = sKey[slot * 32 + y + dy] >> x;
+                for (int h = 0; h < 2; ++h) {
+                    const int y = mt * 8 + 2 * w + h, x = rl;
 #pragma unroll
-                            for (int dx = 0; dx < 3; ++dx)       // 1 settled, -1 falling piece, 0 empty (model_vv.py:212)
-                                hv[dy * 3 + dx] = ((rw >> dx) & 1u) * 0x3C00u | ((rw >> (16 + dx)) & 1u) * 0xBC00u;
+                    for (int j = 0; j < 4; ++j) {
+                        float o[2];
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {            // out[p] = D'[p][dx=0] + D'[p+1][dx=1] + D'[p+2][dx=2]
+                            const int k = 4 * j + 2 * h + e;
+                            const float s1 = __shfl_down_sync(0xffffffffu, d[16 + k], 4), s2 = __shfl_down_sync(0xffffffffu, d[32 + k], 8);
+                            o[e] = fmaxf(fmaf((s2 + s1) + d[k], K23, bias[8 * j + 2 * qd + e]), 0.f);
                         }
-                        *reinterpret_cast<uint4 *>(im + p * 16) =
-                            make_uint4(hv[0] | (hv[1] << 16), hv[2] | (hv[3] << 16), hv[4] | (hv[5] << 16), hv[6] | (hv[7] << 16));   // taps 0..7
-                        *reinterpret_cast<uint32_t *>(im + TCC_IMROWS * 16 + p * 16) = hv[8];                                        // tap 8
+                        uint32_t hi, lo;
+                        split2(o[0], o[1], hi, lo);
+                        if (layer == 0) {
+                            if (x < 6) {                         // act2: 16x6 valid pixels on the 8-wide grid
+                                uint8_t *dst = act + (j * TCC_R + y * 8 + x) * 16 + qd * 4;
+                                *reinterpret_cast<uint32_t *>(dst) = hi;
+                                *reinterpret_cast<uint32_t *>(dst + SPLIT) = lo;
+                            }
+                        } else if (y < 14 && x < 4) {            // act3 -> HBM
+                            const int kc = (y * 4 + x) * 4 + j;
+                            *reinterpret_cast<uint32_t *>(act3 + act3_off(0, n_tiles, ridx, kc) + qd * 4) = hi;
+                            *reinterpret_cast<uint32_t *>(act3 + act3_off(1, n_tiles, ridx, kc) + qd * 4) = lo;
+                        }
                     }
                 }
-                fence_async_smem();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&bar_a0[slot]);
             }
+            fence_async_smem();
+            wg_sync(wg);
+            prof_t(2 + layer);
         }
-    } else {
-        // ===================================================== workers (512 threads)
-        const bool do_prof = blockIdx.x == 0 && t == 0;
-        long long pacc[16] = {0}, ptick = clock64();
-        const int q = warp & 3, cq = warp >> 2, m = q * 32 + lane;       // TMEM lane quadrant, 8-cout chunk, pixel row
-        const uint32_t t_lane = tmem_base + ((uint32_t)(q * 32) << 16) + cq * 8;
-        // this warp's 8 couts, all three layers.  relu(x * 2^-10 + b) * 16 == relu(fma(x, 2^-6, 16 b)) bit for bit (scaling by a power of two commutes
-        // with rounding): the biases are kept pre-scaled and an epilogue value costs one fma + one max instead of mul, add, max, mul
-        float bias1[8], bias2[8], bias3[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) { bias1[e] = sB[cq * 8 + e] * TC_SCALE_A; bias2[e] = sB[32 + cq * 8 + e] * TC_SCALE_A; bias3[e] = sB[64 + cq * 8 + e] * TC_SCALE_A; }
-        constexpr float K23 = TC_UNSCALE * TC_SCALE_A, K1 = TC_SCALE_A / TC_SCALE_W;
-#if B200_CONV3_PAIR
-        const int n_iter = 2 * ((n_local + 1) / 2) + 3;                   // the last pair's E3 runs at iteration 2k+4
-#else
-        const int n_iter = n_local + 3;
-#endif
-        auto phase_e2 = [&](int i) {
-            // ---- E2(i-2): conv2 epilogue: dx sum + bias + ReLU + split -> act2
-            if (i >= 2 && i - 2 < n_local) {
-                const int j = i - 2, slot = j % NS;
-                mbar_wait_warp(&bar_c2[slot], (uint32_t)(j / NS) & 1u);
-                PROF_T(3);
-                tc_fence_after();
-                float v[8];
-                tmem_ld_conv_sum(t_lane + (j % TCC_TSLOTS) * 128, v);
-                {
-                    float o[8];
-#pragma unroll
-                    for (int e = 0; e < 8; ++e) o[e] = fmaxf(fmaf(v[e], K23, bias2[e]), 0.f);
-                    uint4 c1, c2;
-                    split8(o, c1, c2);
-#if !B200_CONV3_PAIR
-                    if ((m & 7) < 6) {                           // 16x8 grid, in place of the slot's act1
-                        uint8_t *base = smem + TCC_OFF_A1 + slot * TCC_ASLOT + (cq * TCC_R + m) * 16;
-                        *reinterpret_cast<uint4 *>(base) = c1;
-                        *reinterpret_cast<uint4 *>(base + 4 * TCC_R * 16) = c2;
-                    }
-#else
-#if B200_CONV3_XPOSE
-                    // The 8 lanes of a store phase hold ONE y and x = 0..7: on the pair grid their rows are 4 groups (512 B) apart, an 8-way bank
-                    // conflict.  Re-deal the warp's 4 y x 8 x values x-major first (lane' = x*4 + yy takes lane yy*8 + x): a phase then holds
-                    // two x and four y (four different 16-byte bank groups), a 2-way conflict, and the row groups stay 128-byte aligned.
-                    const int src = (lane & 3) * 8 + (lane >> 2), xs = lane >> 2, ys = (q << 2) + (lane & 3);
-                    c1.x = __shfl_sync(0xffffffffu, c1.x, src); c1.y = __shfl_sync(0xffffffffu, c1.y, src);
-                    c1.z = __shfl_sync(0xffffffffu, c1.z, src); c1.w = __shfl_sync(0xffffffffu, c1.w, src);
-                    c2.x = __shfl_sync(0xffffffffu, c2.x, src); c2.y = __shfl_sync(0xffffffffu, c2.y, src);
-                    c2.z = __shfl_sync(0xffffffffu, c2.z, src); c2.w = __shfl_sync(0xffffffffu, c2.w, src);
-#else
-                    const int xs = m & 7, ys = m >> 3;           // padded row groups (TCC_PSBO = 144): a 3-way conflict, but the MMA's 128-byte rows straddle lines
-#endif
-                    if (xs < 6) {
-                        const int prow = xs * 32 + (j & 1) * 16 + ys;   // transposed pair grid: x*32 + board*16 + y
-                        uint8_t *base = smem + TCC_OFF_PAIR + ((j >> 1) % TCC_PAIR_BUFS) * TCC_PSLOT + cq * TCC_PCHUNK + (prow >> 3) * TCC_PSBO + (prow & 7) * 16;
-                        *reinterpret_cast<uint4 *>(base) = c1;
-                        *reinterpret_cast<uint4 *>(base + 4 * TCC_PCHUNK) = c2;
-                    }
-#endif
-                }
-                tc_fence_before();
-                fence_async_smem();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&bar_a2[slot]);     // 32 same-address arrivals would serialise in the shared-memory pipe the MMAs read through
-                PROF_T(4);
-            }
-        };
-        auto phase_e3 = [&](int i) {
-            // ---- E3: conv3 epilogue: tap sum + bias + ReLU + split -> act3 in HBM (FC tile layout)
-#if B200_CONV3_PAIR
-            if (i >= 4 && !(i & 1) && i - 4 < n_local) {         // pair k = boards 2k, 2k+1, one iteration after E2(2k+1)
-                const int k = (i - 4) >> 1, j = 2 * k + (lane >> 4);
-                mbar_wait_warp(&bar_c3[k & 1], (uint32_t)(k >> 1) & 1u);
-                PROF_T(5);
-                tc_fence_after();
-                const int y = lane & 15, x = q;                  // TMEM lane m = x*32 + board*16 + y
-                float v[8];
-                tmem_ld_conv_sum(t_lane + TCC_TMEM_PAIR, v);     // the taps stacked along N are the vertical ones here: y + dy = lane + dy
-                if (y < 14 && j < n_local) {
-                    const int ridx = board_of(j);
-#else
-            if (i >= 3) {
-                const int j = i - 3, slot = j % NS, ridx = board_of(j);
-                mbar_wait_warp(&bar_c3[slot], (uint32_t)(j / NS) & 1u);
-                PROF_T(5);
-                tc_fence_after();
-                const int y = m >> 3, x = m & 7;
-                float v[8];
-                tmem_ld_conv_sum(t_lane + slot * 128, v);
-                if (y < 14 && x < 4) {
-#endif
-                    float o[8];
-#pragma unroll
-                    for (int e = 0; e < 8; ++e) o[e] = fmaxf(fmaf(v[e], K23, bias3[e]), 0.f);
-                    uint4 c1, c2;
-                    split8(o, c1, c2);
-                    const int kc = (y * 4 + x) * 4 + cq;
-#if B200_L2_STREAM_ACT3
-                    const uint64_t pol = l2_policy_stream();
-                    stg_hint(reinterpret_cast<int4 *>(act3 + act3_off(0, n_tiles, ridx, kc)), make_int4((int)c1.x, (int)c1.y, (int)c1.z, (int)c1.w), pol);
-                    stg_hint(reinterpret_cast<int4 *>(act3 + act3_off(1, n_tiles, ridx, kc)), make_int4((int)c2.x, (int)c2.y, (int)c2.z, (int)c2.w), pol);
-#else
-                    *reinterpret_cast<uint4 *>(act3 + act3_off(0, n_tiles, ridx, kc)) = c1;
-                    *reinterpret_cast<uint4 *>(act3 + act3_off(1, n_tiles, ridx, kc)) = c2;
-#endif
-                }
-                tc_fence_before();
-#if B200_CONV3_PAIR
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&bar_e3[0]);
-#endif
-                PROF_T(6);
-            }
-        };
-        auto phase_e1 = [&](int i) {
-            // ---- E1(i): conv1 epilogue: bias + ReLU + split -> act1 (18x8 grid)
-            if (i < n_local) {
-                const int j = i, slot = j % NS;
-                mbar_wait_warp(&bar_c1[slot], (uint32_t)(j / NS) & 1u);
-                PROF_T(1);
-                tc_fence_after();
-                uint8_t *abase = smem + TCC_OFF_A1 + (j % TCC_ACT1_BUFS) * TCC_ASLOT + cq * TCC_R * 16;
-                const uint32_t t_c1 = t_lane + (j % TCC_TSLOTS) * 128;
-                {
-                    float w1[8], w2[8], o[8];
-                    tmem_ld8x2(t_c1, w1, w2);
-#pragma unroll
-                    for (int e = 0; e < 8; ++e) o[e] = fmaxf(fmaf(w2[e] + w1[e], K1, bias1[e]), 0.f);
-                    uint4 c1, c2;
-                    split8(o, c1, c2);
-                    *reinterpret_cast<uint4 *>(abase + m * 16) = c1;
-                    *reinterpret_cast<uint4 *>(abase + 4 * TCC_R * 16 + m * 16) = c2;
-                }
-                if (q == 0) {                                    // rows 128..143 sit in lanes 0..15 of the second M tile
-                    float w1[8], w2[8], o[8];
-                    tmem_ld8x2(t_c1 + 64, w1, w2);
-                    if (lane < 16) {
-#pragma unroll
-                        for (int e = 0; e < 8; ++e) o[e] = fmaxf(fmaf(w2[e] + w1[e], K1, bias1[e]), 0.f);
-                        uint4 c1, c2;
-                        split8(o, c1, c2);
-                        *reinterpret_cast<uint4 *>(abase + (128 + lane) * 16) = c1;
-                        *reinterpret_cast<uint4 *>(abase + 4 * TCC_R * 16 + (128 + lane) * 16) = c2;
-                    }
-                }
-                tc_fence_before();
-                fence_async_smem();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&bar_a1[slot]);     // 32 same-address arrivals would serialise in the shared-memory pipe the MMAs read through
-                PROF_T(2);
-            }
-        };
-        for (int i = 0; i < n_iter; ++i) {
-#if B200_CONV3_PAIR && B200_CONV3_E3FIRST
-            phase_e3(i); phase_e2(i); phase_e1(i);
-#else
-            phase_e2(i); phase_e3(i); phase_e1(i);
-#endif
-        }
-        if (prof && do_prof) for (int i = 0; i < 16; ++i) if (i < 8 || i > 13) atomicAdd(&prof[i], (unsigned long long)pacc[i]);
     }
-#undef PROF_T
-    tc_fence_before();
-    __syncthreads();
-    if (warp == TCC_ISSUER) tmem_dealloc<TCC_TMEM_COLS>(tmem_base);
+    if (do_prof) for (int k = 0; k < 4; ++k) atomicAdd(&prof[k], (unsigned long long)pacc[k]);
 }
 
 // ---------------------------------------------------------------------------------------------------- fc kernel
-constexpr int TCF_THREADS = 192;            // warp 0 producer, warp 1 MMA issuer, warps 2-5 epilogue
+constexpr int TCF_CONSUMERS = 2;            // warpgroups 0-1: MMA + epilogue, 64 rows of the 128-row tile each
+constexpr int TCF_PRODUCER = TCF_CONSUMERS * 4;   // warp 8: bulk copies
+constexpr int TCF_THREADS = TCF_CONSUMERS * 128 + 32;
 constexpr int TCF_STAGES = 8;
 constexpr int TCF_A_BYTES = 2 * 128 * 16;   // one split of one k16 block of the A tile
 constexpr int TCF_B_BYTES = 2 * 256 * 16;
 constexpr int TCF_STAGE = 2 * TCF_A_BYTES + 2 * TCF_B_BYTES;   // 24576
 constexpr int TCF_KBLOCKS = 112;            // 1792 / 16
 constexpr int TCF_OFF_BAR = TCF_STAGES * TCF_STAGE;
-constexpr int TCF_OFF_EPI = TCF_OFF_BAR + 256;                 // (2*stages + 2 mbarriers + tmem ptr fit in 256 B) bias[256] | wout[2][256] | bout/ub/lb
-static_assert((2 * TCF_STAGES + 2) * 8 + 4 <= 256, "barrier block overflows into the epilogue constants");
+constexpr int TCF_OFF_EPI = TCF_OFF_BAR + 256;                 // bias[256] | wout[2][256] | bout/ub/lb
+static_assert(2 * TCF_STAGES * 8 <= 256, "barrier block overflows into the epilogue constants");
 constexpr int TCF_SMEM = TCF_OFF_EPI + (256 * 3 + 8) * 4;
-constexpr int TCF_TMEM_COLS = 256;
+static_assert(TCF_SMEM <= 227 * 1024, "k_tc_fc shared memory");
 
 __global__ void __launch_bounds__(TCF_THREADS, 1)
 k_tc_fc(NetWeights W, TcWeights TW, const uint8_t *act3, int n_tiles_alloc, const uint2 *req, const int32_t *n_req_ptr, float2 *eval_out) {
     extern __shared__ __align__(128) uint8_t smem[];
     uint64_t *full = reinterpret_cast<uint64_t *>(smem + TCF_OFF_BAR);     // [stage] operands landed
-    uint64_t *empty = full + TCF_STAGES;                                    // [stage] operands consumed
-    uint64_t *acc_full = empty + TCF_STAGES;                                // accumulator complete
-    uint64_t *acc_empty = acc_full + 1;                                     // accumulator drained by the epilogue
-    uint32_t *tmem_ptr = reinterpret_cast<uint32_t *>(acc_empty + 1);
+    uint64_t *empty = full + TCF_STAGES;                                    // [stage] operands consumed (one arrival per consumer warpgroup)
     float *sBias = reinterpret_cast<float *>(smem + TCF_OFF_EPI), *sWo = sBias + 256, *sTail = sWo + 512;
     const int t = threadIdx.x, warp = t >> 5, lane = t & 31;
     for (int i = t; i < 256; i += TCF_THREADS) { sBias[i] = W.bfc1[i]; sWo[i] = W.wout[i]; sWo[256 + i] = W.wout[256 + i]; }
     if (t < 2) { sTail[t] = W.bout[t]; sTail[2 + t] = W.ub[t]; sTail[4 + t] = W.lb[t]; }
     if (t == 0) {
-        for (int i = 0; i < TCF_STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-        mbar_init(acc_full, 1);
-        mbar_init(acc_empty, 128);
+        for (int i = 0; i < TCF_STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], TCF_CONSUMERS); }
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc<TCF_TMEM_COLS>(tmem_ptr);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
     const int n_req = *n_req_ptr;
     const int n_tiles = (n_req + 127) >> 7;
-    if (warp == 0) {
+    if (warp == TCF_PRODUCER) {
         if (lane == 0) {   // ===== producer: bulk copies of the pre-laid-out operand blocks
             int stage = 0; uint32_t ph = 0;
             for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
@@ -747,77 +425,67 @@ k_tc_fc(NetWeights W, TcWeights TW, const uint8_t *act3, int n_tiles_alloc, cons
                     uint8_t *dst = smem + stage * TCF_STAGE;
 #pragma unroll
                     for (int s = 0; s < 2; ++s) {
-#if B200_L2_STREAM_ACT3
-                        bulk_g2s_hint(dst + s * TCF_A_BYTES, act3 + (((size_t)s * n_tiles_alloc + tile) * ACT3_KCHUNKS + 2 * j) * 2048, TCF_A_BYTES, &full[stage], l2_policy_stream());
-#else
                         bulk_g2s(dst + s * TCF_A_BYTES, act3 + (((size_t)s * n_tiles_alloc + tile) * ACT3_KCHUNKS + 2 * j) * 2048, TCF_A_BYTES, &full[stage]);
-#endif
                         bulk_g2s(dst + 2 * TCF_A_BYTES + s * TCF_B_BYTES, TW.wfc + ((size_t)s * TCF_KBLOCKS + j) * TCF_B_BYTES, TCF_B_BYTES, &full[stage]);
                     }
                     if (++stage == TCF_STAGES) { stage = 0; ph ^= 1; }
                 }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {   // ===== MMA issuer: D[128 x 256] += A[128 x 16] * B[256 x 16]^T, six split terms per k block
-            const uint32_t idesc = umma_idesc_f16(128, 256);
-            int stage = 0; uint32_t ph = 0, aph = 0;
-            for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-                mbar_wait(acc_empty, aph ^ 1);
-                tc_fence_after();
-                uint32_t acc = 0;
-                for (int j = 0; j < TCF_KBLOCKS; ++j) {
-                    mbar_wait(&full[stage], ph);
-                    tc_fence_after();
-                    const uint32_t sbase = smem_u32(smem + stage * TCF_STAGE);
-#pragma unroll
-                    for (int term = 0; term < 3; ++term) {   // a1*b2, a2*b1, a1*b1 (small terms first)
-                        const int sa = term == 1 ? 1 : 0, sb = term == 0 ? 1 : 0;
-                        uint64_t ad = umma_desc(sbase + sa * TCF_A_BYTES, 128 * 16, 128);
-                        uint64_t bd = umma_desc(sbase + 2 * TCF_A_BYTES + sb * TCF_B_BYTES, 256 * 16, 128);
-                        umma_f16(tmem_base, ad, bd, idesc, acc);
-                        acc = 1;
-                    }
-                    umma_commit(&empty[stage]);
-                    if (++stage == TCF_STAGES) { stage = 0; ph ^= 1; }
-                }
-                umma_commit(acc_full);
-                aph ^= 1;
-            }
-        }
-    } else {   // ===== epilogue warps 2..5: TMEM quadrant = warp % 4, one row per thread
-        const int q = warp & 3, row = q * 32 + lane;
-        uint32_t aph = 0;
+    } else {   // ===== consumers: D[64 x 256] += A[64 x 16] * B[256 x 16]^T per warpgroup, three split terms per k block
+        const int wg = t >> 7, w = warp & 3, qd = lane & 3, rl = lane >> 2;
+        int stage = 0; uint32_t ph = 0;
         for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-            mbar_wait(acc_full, aph);
-            tc_fence_after();
-            float p0 = 0.f, p1 = 0.f;
-#pragma unroll 1
-            for (int c0 = 0; c0 < 256; c0 += 16) {
-                float v[16];
-                tmem_ld16(tmem_base + ((uint32_t)(q * 32) << 16) + c0, v);
+            float d[128];
 #pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                    float h = fmaxf(v[j] * TC_UNSCALE + sBias[c0 + j], 0.f);   // model_vv.py:39-40
-                    p0 = fmaf(h, sWo[c0 + j], p0); p1 = fmaf(h, sWo[256 + c0 + j], p1);   // :41
+            for (int k = 0; k < 128; ++k) d[k] = 0.f;
+            int prev = -1;
+            for (int j = 0; j < TCF_KBLOCKS; ++j) {
+                mbar_wait(&full[stage], ph);
+                const uint32_t sbase = smem_u32(smem + stage * TCF_STAGE);
+                wgmma_fence();
+#pragma unroll
+                for (int term = 0; term < 3; ++term) {   // a1*b2, a2*b1, a1*b1 (small terms first)
+                    const int sa = term == 1 ? 1 : 0, sb = term == 0 ? 1 : 0;
+                    const uint64_t ad = gmma_desc(sbase + sa * TCF_A_BYTES + wg * 1024, 128 * 16, 128);
+                    const uint64_t bd = gmma_desc(sbase + 2 * TCF_A_BYTES + sb * TCF_B_BYTES, 256 * 16, 128);
+                    wgmma_n256(d, ad, bd, (j | term) ? 1u : 0u);
+                }
+                wgmma_commit();
+                wgmma_wait<1>();                         // the previous k block's MMAs are done with their stage
+                if (prev >= 0 && (t & 127) == 0) mbar_arrive(&empty[prev]);
+                prev = stage;
+                if (++stage == TCF_STAGES) { stage = 0; ph ^= 1; }
+            }
+            wgmma_wait<0>();
+            fence_regs(d);
+            if ((t & 127) == 0) mbar_arrive(&empty[prev]);
+            float p0[2] = {0.f, 0.f}, p1[2] = {0.f, 0.f};
+#pragma unroll
+            for (int j = 0; j < 32; ++j)
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const int c = 8 * j + 2 * qd + e;
+                        const float hv = fmaxf(d[4 * j + 2 * h + e] * TC_UNSCALE + sBias[c], 0.f);   // model_vv.py:39-40
+                        p0[h] = fmaf(hv, sWo[c], p0[h]); p1[h] = fmaf(hv, sWo[256 + c], p1[h]);      // :41
+                    }
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {                // the four lanes of a row hold interleaved column quarters
+                p0[h] += __shfl_xor_sync(0xffffffffu, p0[h], 1); p1[h] += __shfl_xor_sync(0xffffffffu, p1[h], 1);
+                p0[h] += __shfl_xor_sync(0xffffffffu, p0[h], 2); p1[h] += __shfl_xor_sync(0xffffffffu, p1[h], 2);
+                const int ridx = tile * 128 + wg * 64 + 16 * w + 8 * h + rl;
+                if (qd == 0 && ridx < n_req) {
+                    const float x0 = p0[h] + sTail[0], x1 = p1[h] + sTail[1];
+                    const float s0 = 1.f / (1.f + expf(-x0)), s1 = 1.f / (1.f + expf(-x1));      // :42
+                    const uint2 rq = req[ridx];
+                    eval_out[(size_t)rq.x * 8 + (rq.y >> 28)] =
+                        make_float2(__fadd_rn(__fmul_rn(s0, sTail[2]), sTail[4]), __fadd_rn(__fmul_rn(s1, sTail[3]), sTail[5]));   // :51
                 }
             }
-            tc_fence_before();
-            mbar_arrive(acc_empty);
-            const int ridx = tile * 128 + row;
-            if (ridx < n_req) {
-                float x0 = p0 + sTail[0], x1 = p1 + sTail[1];
-                float s0 = 1.f / (1.f + expf(-x0)), s1 = 1.f / (1.f + expf(-x1));      // :42
-                uint2 rq = req[ridx];
-                eval_out[(size_t)rq.x * 8 + (rq.y >> 28)] =
-                    make_float2(__fadd_rn(__fmul_rn(s0, sTail[2]), sTail[4]), __fadd_rn(__fmul_rn(s1, sTail[3]), sTail[5]));   // :51
-            }
-            aph ^= 1;
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc<TCF_TMEM_COLS>(tmem_base);
 }
 
 // ---------------------------------------------------------------------------------------------------- host side
@@ -834,7 +502,7 @@ static inline void host_split2(float x, uint16_t *o) {   // x*scale = h1 + h2 in
 }
 static inline float host_half_f(uint16_t h) { __half x; memcpy(&x, &h, 2); return __half2float(x); }
 
-// w = the state_dict-order weight vector of include/b200_tetris_mcts.h.  Pure re-layout + bf16 splitting.
+// w = the state_dict-order weight vector of include/b200_tetris_mcts.h.  Pure re-layout + fp16 splitting.
 static int tc_prepare(void **state, const float *w, cudaStream_t stream) {
     TcState *st = (TcState *)*state;
     if (!st) { st = new TcState(); *state = st; }
@@ -864,10 +532,9 @@ static int tc_prepare(void **state, const float *w, cudaStream_t stream) {
                                 int ci = 16 * hh + 8 * c2 + e;
                                 uint16_t s2[2];
                                 host_split2(cw[(n * 32 + ci) * 9 + dy * 3 + dx] * TC_SCALE_W, s2);
-                                // the tap that shifts the A operand selects the block, the other one is stacked along N (conv3 in pair mode: transposed)
-                                const int shift_tap = (layer && B200_CONV3_PAIR) ? dx : dy, n_tap = (layer && B200_CONV3_PAIR) ? dy : dx;
+                                // the tap that shifts the A operand (dy) selects the block, the other one (dx) is stacked along N
                                 for (int s = 0; s < 2; ++s)
-                                    dst[(((((size_t)(shift_tap * 2 + hh)) * 2 + s) * 2 + c2) * 96 + n_tap * 32 + n) * 8 + e] = s2[s];
+                                    dst[(((((size_t)(dy * 2 + hh)) * 2 + s) * 2 + c2) * 96 + dx * 32 + n) * 8 + e] = s2[s];
                             }
     }
     for (int j = 0; j < TCF_KBLOCKS; ++j)

@@ -1,7 +1,7 @@
 """Multi-GPU plumbing: one process per GPU (torch.distributed, NCCL over NVLink), games sharded embarrassingly.
 
 The reference has no distributed backend at all (SURVEY §2b: workers are `play.py &` processes exchanging HDF5 files,
-cycle.sh:53-74).  The only exchange step of the B200 build is the all-gather of fixed-size replay-sample blocks
+cycle.sh:53-74).  The only exchange step of this build is the all-gather of fixed-size replay-sample blocks
 (212-byte rows {int8 state[200], f32 value, f32 variance, f32 visit}; schema = ValueSim.memory, agents/ValueSim.py:25-30)
 plus small counter reductions for reporting.  No data-path collective exists inside the search."""
 import os
