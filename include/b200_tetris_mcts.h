@@ -204,8 +204,9 @@ int b200_replay_append(b200_engine *e, const uint8_t *rows_host, int n_rows);   
 /* --- value-network training step (SURVEY 8f.2): Model_VV._loss / Model.train / Yogi.step / Model_VV.train_data of the reference
  *     (model/model_vv.py:94-153,227-231, model/model.py:52-119, model/yogi.py:39-90) on the device.  weights = the state_dict vector of
  *     b200_load_weights (PyTorch layouts); a batch is {states int8[n][200], value f32[n], variance f32[n], weight f32[n]} (the four arrays
- *     of ValueSim.memory, agents/ValueSim.py:25-30).  Host logic that stays on the host (validation split, batch sampling, early stopping,
- *     checkpoint files): tetris_mcts_b200/model/model_vv.py Model_VV.train_data. */
+ *     of ValueSim.memory, agents/ValueSim.py:25-30).  Host logic that stays on the host (validation split, early stopping, checkpoint files):
+ *     tetris_mcts_b200/model/model_vv.py Model_VV.train_data (host arrays) and Model_VV.train_rows (device replay rows, batches drawn on the
+ *     device by b200_trainer_train_rows_dev). */
 typedef struct b200_trainer b200_trainer;
 const char *b200_trainer_last_error(void);
 int b200_trainer_create(int device, const float *weights, int max_batch, b200_trainer **out);     /* Model_VV._init_model (model_vv.py:125-134) */
@@ -227,6 +228,21 @@ int b200_trainer_step(b200_trainer *t, const int8_t *states, const float *value,
  * indices (np.random.choice, model/model.py:207), weight = visit * weight_scale (weights / weights.mean(), model/model.py:186-187) */
 int b200_trainer_step_rows_dev(b200_trainer *t, const void *rows_dev, int n_rows, const int32_t *idx, int n, float weight_scale,
                                int weighted, double grad_clip, double *loss, double *loss_std, double *grad_norm);
+/* Model.train_data's inner loop on device rows: `iters` steps of b200_trainer_step_rows_dev with batches of `batch` rows drawn ON THE DEVICE,
+ * uniformly with replacement from rows [0, n_train_rows) (np.random.choice(n_train_rows, batch), model/model.py:207), and one host
+ * synchronisation at the end.  Row i of step it (iteration number j = first_iter + it) is
+ *     idx = splitmix64(splitmix64(splitmix64(seed) + j) + i) mod n_train_rows        (uint64 arithmetic, wrapping)
+ *     splitmix64(x): z = x + 0x9E3779B97F4A7C15; z = (z ^ z >> 30) * 0xBF58476D1CE4E5B9; z = (z ^ z >> 27) * 0x94D049BB133111EB; z ^ z >> 31
+ * Gradient norm, clipping and Yogi are step_rows_dev's arithmetic: each step is bit-identical to b200_trainer_step_rows_dev fed those indices.
+ * log_out (host): [iters][3] = {loss, loss_std, grad_norm} of each step. */
+int b200_trainer_train_rows_dev(b200_trainer *t, const void *rows_dev, int n_train_rows, int batch, int iters, uint64_t seed, int64_t first_iter,
+                                float weight_scale, int weighted, double grad_clip, double *log_out);
+/* Model_VV._loss under no_grad on device rows [first, first + n) (a chunk of Model.compute_loss); *weight_sum = fp64 sum of visit * weight_scale */
+int b200_trainer_loss_rows_dev(b200_trainer *t, const void *rows_dev, int first, int n, float weight_scale, int weighted,
+                               double *loss, double *loss_std, double *weight_sum);
+/* max(value), max(variance) and the fp64 sum of visits of device rows [0, n) (out_ubound, model_vv.py:227-231; the weight mean,
+ * model/model.py:186-187), reduced in a fixed order on the trainer's stream */
+int b200_rows_stats_dev(b200_trainer *t, const void *rows_dev, int n, float *max_value, float *max_variance, double *visit_sum);
 
 #ifdef __cplusplus
 }

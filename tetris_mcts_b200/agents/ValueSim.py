@@ -23,54 +23,71 @@ class ValueSim(TreeAgent):
         super().__init__(max_nodes=100000, gamma=gamma, low=1, weights=weights, **kwargs)   # ValueSim.py:16
         self.online, self.min_visits_to_store = online, min_visits_to_store
         self.memory_size, self.memory_growth_rate, self.n_trains = memory_size, memory_growth_rate, 0   # ValueSim.py:21-37
-        self._weights, self._rows, self.model = np.asarray(weights, np.float32), None, None
+        self._weights, self._online = np.asarray(weights, np.float32), None
         if online and not self.benchmark:                         # ValueSim.py:21-37: the replay memory lives on the device (k_gc fills it)
+            from ..online import OnlineTrainer
             self._eng.replay_enable(min_visits=min_visits_to_store, capacity=memory_size)
-            print('online: freed observations are stored on the device as in ValueSim.store_nodes (ValueSim.py:122-159); train_nodes() '
-                  'trains on them (Model_VV.train_data on the device trainer)', **perr)
+            # accumulation policy 3 is train_nodes' rule: train once memory_index >= min(n_trains * memory_growth_rate, memory_size)
+            self._eng.replay_policy(3, memory_growth_rate=memory_growth_rate)
+            self._online = OnlineTrainer(self._eng, self._weights, memory_size, batch_size=1024, iters_per_val=100, max_iters=50000)   # ValueSim.py:180
+            self._gcs = 0
+            print('online: freed observations are stored on the device as in ValueSim.store_nodes (ValueSim.py:122-159) and the value network '
+                  'is trained on them after the collections that fill the memory (train_nodes, ValueSim.py:161-185)', **perr)
 
-    def train_nodes(self, dump_data=True, path='./data/dump', **train_kwargs):    # ValueSim.py:161-185
-        """Drain the device replay memory (rows k_gc stored: ValueSim.store_nodes, ValueSim.py:122-159) into ValueSim.memory; when
-        memory_index >= min(n_trains * memory_growth_rate, memory_size) dump it (np.savez('./data/dump', ...), ValueSim.py:176-177), run
-        Model_VV.train_data on the device trainer (ValueSim.py:180: iters_per_val=100, batch_size=1024, max_iters=50000) and hot-swap the
-        search network.  Returns the memory arrays used for training, or None while still collecting (ValueSim.py:170-172)."""
-        import torch
+    @property
+    def model(self):
+        return self._online.model if self._online else None
+
+    def _after_collections(self):
+        """remove_nodes' store_nodes + train_nodes (ValueSim.py:101-115) after a call in which the engine collected (gcs counter moved)"""
+        if self._online is None:
+            return
+        gcs = self._eng.counters()["gcs"]
+        if gcs != self._gcs:
+            self._gcs = gcs
+            self.train_nodes()
+
+    def play(self):
+        action = super().play()
+        self._after_collections()
+        return action
+
+    def update_root(self, game):
+        super().update_root(game)
+        self._after_collections()
+
+    def remove_nodes(self):
+        super().remove_nodes()
+        self._after_collections()
+
+    def train_nodes(self, dump_data=True, path='./data/dump'):    # ValueSim.py:161-185
+        """When memory_index >= min(n_trains * memory_growth_rate, memory_size): dump the memory (np.savez('./data/dump', ...),
+        ValueSim.py:176-177), run Model_VV.train_rows on the device rows (ValueSim.py:180: iters_per_val=100, batch_size=1024,
+        max_iters=50000) and hot-swap the search network.  Returns the memory arrays used for training, or None while still collecting
+        (ValueSim.py:170-172)."""
         from .. import replay
-        if not (self.online and not self.benchmark):
+        if self._online is None:
             return None
         print('Training...', **perr)
-        cap = self.memory_size
-        dev = torch.device("cuda", int(self._eng.cfg.device))      # the engine's device, not torch's current one
-        buf = torch.empty((cap, replay.SAMPLE_BYTES), dtype=torch.uint8, device=dev)
-        torch.cuda.synchronize(dev)                                # the engine copies on its own stream: nothing of torch's may be pending on buf
-        n = self._eng.replay_drain_into(buf.data_ptr(), cap)
-        rows = buf[:n].cpu().numpy()
-        self._rows = rows if self._rows is None else np.concatenate([self._rows, rows])[:cap]
-        d_size = len(self._rows)
+        train_now, d_size = self._eng.replay_policy_step(self.episode)
         m_size = min(self.n_trains * self.memory_growth_rate, self.memory_size)
-        if d_size >= m_size and d_size > 0:
-            print('Enough training data ({} >= {}), proceed to training.'.format(d_size, m_size), **perr)
-        else:
+        if not train_now:
             print('Not enough training data ({} < {}), collecting more data.'.format(d_size, m_size), **perr)
             return None
-        if dump_data:
-            replay.dump(path, self._rows)
-        memory = replay.rows_to_memory(self._rows)
+        print('Enough training data ({} >= {}), proceed to training.'.format(d_size, m_size), **perr)
+        if not self._online.train(d_size, self.episode, dump_path=path if dump_data else None):
+            return None
+        if not dump_data:
+            self._online.last_rows = self._online.buf[:d_size].cpu().numpy()
         self.n_trains += 1
-        if self.model is None:
-            from ..model.model_vv import Model_VV
-            self.model = Model_VV(device=int(self._eng.cfg.device), eval_kind="net")
-            self.model.weights = self._weights
-            self.model._eng.load_weights(self._weights)
-        kw = dict(iters_per_val=100, batch_size=1024, max_iters=50000)                    # ValueSim.py:180
-        kw.update(train_kwargs)
-        self.model.train_data(memory, **kw)
-        self.model.training(False)
-        self._weights = self.model.weights
-        self._eng.load_weights(self._weights)                      # the search now evaluates with the trained network
-        self._rows = None                                          # memory_index = 0 (ValueSim.py:183)
+        self._weights = self._online.weights
         print('Training complete.', **perr)
-        return memory
+        return replay.rows_to_memory(self._online.last_rows)
+
+    def close(self):
+        if self._online is not None:
+            self._online.close()
+        super().close()
 
     def evaluate_state(self, state):                              # ValueSim.py:46-50
         v, var = self._eng.valuenet(state[None])

@@ -8,6 +8,8 @@
 //   Model.train                    model/model.py:95-119       zero_grad, loss.backward(), gradient norm, optional clip, optimizer.step()
 //   Yogi.step                      model/yogi.py:39-90         (lr=1e-3, eps=1e-3, weight_decay=1e-3: model_vv.py:132)
 //   Model_VV.train_data            model/model_vv.py:227-231   out_ubound <- [max(value), max(variance)] of the training data
+//   Model.train_data               model/model.py:176-249      b200_trainer_train_rows_dev: a validation interval of steps on device rows, batches
+//                                                              drawn on the device, one host synchronisation; _loss_rows_dev / b200_rows_stats_dev
 //
 // Arithmetic: fp32 storage as in the reference; every contraction (forward GEMMs, weight / bias / input gradients) accumulates in fp64 and
 // rounds once to fp32, so the result does not depend on a blocking order and sits within the reference's own fp32 rounding noise
@@ -287,6 +289,77 @@ __global__ void k_yogi(float *__restrict__ p, const float *__restrict__ grad, fl
     }
 }
 
+// ------------------------------------------------------------------------------------------------ device-side training loop (b200_trainer_train_rows_dev)
+// batch indices: idx[i] = splitmix64(splitmix64(splitmix64(seed) + iteration) + i) mod n_rows (include/b200_tetris_mcts.h)
+__host__ __device__ inline uint64_t splitmix64(uint64_t x) {
+    uint64_t z = x + 0x9E3779B97F4A7C15ull;
+    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+    return z ^ (z >> 31);
+}
+__global__ void k_sample_idx(int32_t *idx, int n, int n_rows, uint64_t seed, uint64_t iteration) {
+    const uint64_t base = splitmix64(splitmix64(seed) + iteration);
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) idx[i] = (int32_t)(splitmix64(base + (uint64_t)i) % (uint64_t)n_rows);
+}
+__global__ void k_seq_idx(int32_t *idx, int n, int first) {
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) idx[i] = first + i;
+}
+// step_common's host arithmetic on the device, operation for operation (no contraction into FMAs): gn = sqrt(sum_i sqrt(ss_i)^2) in tensor order,
+// coef = clip / (gn + 1e-6); out_gn <- gn; coef_out <- (float)coef when clipping applies (coef < 1), else -1 (k_scale_dev then leaves the gradient)
+__global__ void k_grad_norm(const double *__restrict__ ss, double grad_clip, double *__restrict__ out_gn, float *__restrict__ coef_out) {
+    double tot = 0.0;
+    for (int i = 0; i < N_TENSORS; ++i) { const double nrm = __dsqrt_rn(ss[i]); tot = __dadd_rn(tot, __dmul_rn(nrm, nrm)); }
+    const double gn = __dsqrt_rn(tot);
+    *out_gn = gn;
+    float c = -1.f;
+    if (grad_clip > 0.0) { const double coef = __ddiv_rn(grad_clip, __dadd_rn(gn, 1e-6)); if (coef < 1.0) c = (float)coef; }
+    *coef_out = c;
+}
+__global__ void k_scale_dev(float *g, int n, const float *__restrict__ coef) {
+    const float c = *coef;
+    if (c < 0.f) return;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) g[i] *= c;
+}
+// sum of the batch weights in fp64 (the chunk size Model.compute_loss weighs a weighted chunk with, model/model.py:69-70), one CTA, fixed order
+__global__ void __launch_bounds__(256) k_sum(const float *__restrict__ x, int n, double *out) {
+    __shared__ double s[256];
+    double a = 0.0;
+    for (int i = threadIdx.x; i < n; i += 256) a += (double)x[i];
+    s[threadIdx.x] = a;
+    __syncthreads();
+    for (int d = 128; d > 0; d >>= 1) { if (threadIdx.x < d) s[threadIdx.x] += s[threadIdx.x + d]; __syncthreads(); }
+    if (threadIdx.x == 0) *out = s[0];
+}
+// max(value), max(variance), sum(visit) (fp64) of rows [0, n): per-CTA partials over a fixed grid-stride, then one CTA adds them in CTA order
+constexpr int STATS_CTAS = 132;
+__global__ void __launch_bounds__(256) k_rows_stats_part(const uint8_t *__restrict__ rows, int n, float *__restrict__ pmax, double *__restrict__ psum) {
+    __shared__ float s_v[256], s_var[256];
+    __shared__ double s_w[256];
+    float mv = -INFINITY, mvar = -INFINITY;
+    double w = 0.0;
+    for (int i = blockIdx.x * 256 + threadIdx.x; i < n; i += STATS_CTAS * 256) {
+        float f[3];
+        memcpy(f, rows + (size_t)i * 212 + 200, 12);
+        mv = fmaxf(mv, f[0]); mvar = fmaxf(mvar, f[1]); w += (double)f[2];
+    }
+    s_v[threadIdx.x] = mv; s_var[threadIdx.x] = mvar; s_w[threadIdx.x] = w;
+    __syncthreads();
+    for (int d = 128; d > 0; d >>= 1) {
+        if (threadIdx.x < d) {
+            s_v[threadIdx.x] = fmaxf(s_v[threadIdx.x], s_v[threadIdx.x + d]); s_var[threadIdx.x] = fmaxf(s_var[threadIdx.x], s_var[threadIdx.x + d]);
+            s_w[threadIdx.x] += s_w[threadIdx.x + d];
+        }
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) { pmax[2 * blockIdx.x] = s_v[0]; pmax[2 * blockIdx.x + 1] = s_var[0]; psum[blockIdx.x] = s_w[0]; }
+}
+__global__ void k_rows_stats_final(const float *__restrict__ pmax, const double *__restrict__ psum, float *__restrict__ out_max, double *__restrict__ out_sum) {
+    float mv = -INFINITY, mvar = -INFINITY;
+    double w = 0.0;
+    for (int b = 0; b < STATS_CTAS; ++b) { mv = fmaxf(mv, pmax[2 * b]); mvar = fmaxf(mvar, pmax[2 * b + 1]); w += psum[b]; }
+    out_max[0] = mv; out_max[1] = mvar; *out_sum = w;
+}
+
 inline int nblk(size_t n, int t = 256) { size_t b = (n + t - 1) / t; return (int)(b < 1 ? 1 : (b > 132 * 16 ? 132 * 16 : b)); }
 
 }  // namespace
@@ -305,6 +378,9 @@ struct b200_trainer {
     float *col1, *a1, *col2, *a2, *col3, *a3, *flat, *h, *pred, *lossv, *dz;
     float *dh, *dflat, *dc3, *dcol3, *da2, *dcol2, *da1;
     double *part; size_t part_elems = 0;
+    // b200_trainer_train_rows_dev / _loss_rows_dev / b200_rows_stats_dev
+    float *d_coef = nullptr, *d_pmax = nullptr, *d_max2 = nullptr; double *d_psum = nullptr, *d_dsum = nullptr;
+    double *d_log = nullptr; size_t log_cap = 0;                         // [iters][3] step log, grown on demand (not in allocs)
 };
 
 namespace {
@@ -409,6 +485,7 @@ extern "C" int b200_trainer_destroy(b200_trainer *t) {
     if (!t) return B200_OK;
     if (t->stream) cudaStreamSynchronize(t->stream);
     for (void *p : t->allocs) cudaFree(p);
+    if (t->d_log) cudaFree(t->d_log);
     if (t->stream) cudaStreamDestroy(t->stream);
     delete t;
     return B200_OK;
@@ -437,6 +514,8 @@ extern "C" int b200_trainer_create(int device, const float *weights, int max_bat
     // split-k partial sums (fp64): only the weight-gradient products are split; the largest is fc1 (256 x 1792) with <= 8 k ranges
     t->part_elems = (size_t)8 * 256 * 1792;
     rc |= talloc(t, &t->part, t->part_elems);
+    rc |= talloc(t, &t->d_coef, 1); rc |= talloc(t, &t->d_pmax, 2 * STATS_CTAS); rc |= talloc(t, &t->d_psum, STATS_CTAS);
+    rc |= talloc(t, &t->d_max2, 2); rc |= talloc(t, &t->d_dsum, 1);
     if (rc) return B200_ERR_CUDA;
     TCK(cudaMemcpyAsync(t->w, weights, N_ALL * sizeof(float), cudaMemcpyHostToDevice, t->stream));
     TCK(cudaMemcpyAsync(t->d_toff, T_OFF, sizeof(T_OFF), cudaMemcpyHostToDevice, t->stream));
@@ -581,4 +660,87 @@ extern "C" int b200_trainer_step_rows_dev(b200_trainer *t, const void *rows_dev,
     TCK(cudaMemcpyAsync(t->d_idx, idx, (size_t)n * 4, cudaMemcpyHostToDevice, t->stream));
     k_gather_rows<<<nblk((size_t)n * 203), 256, 0, t->stream>>>((const uint8_t *)rows_dev, t->d_idx, n, weight_scale, t->x0, t->value, t->variance, t->weight);
     return step_common(t, n, weighted, grad_clip, loss, loss_std, grad_norm);
+}
+
+// Model.train_data's inner loop (model/model.py:205-212) for `iters` steps on device rows, with one host synchronisation at the end: each step
+// draws its batch on the device (k_sample_idx: uniform with replacement over rows [0, n_train_rows), iteration number first_iter + it), then
+// runs exactly step_common's kernels; the gradient norm and the clip coefficient are computed on the device with step_common's host arithmetic,
+// so every step is bit-identical to b200_trainer_step_rows_dev fed the same indices.  log_out (host) gets [iters][3] = {loss, loss_std, grad_norm}.
+extern "C" int b200_trainer_train_rows_dev(b200_trainer *t, const void *rows_dev, int n_train_rows, int batch, int iters, uint64_t seed, int64_t first_iter,
+                                           float weight_scale, int weighted, double grad_clip, double *log_out) {
+    if (!t || !rows_dev || !log_out || batch < 1 || batch > t->max_batch || n_train_rows < 1 || iters < 0 || first_iter < 0)
+        return tfail(B200_ERR_BAD_ARG, "trainer: bad argument");
+    TCK(cudaSetDevice(t->device));
+    if (iters == 0) return B200_OK;
+    if ((size_t)iters * 3 > t->log_cap) {
+        TCK(cudaStreamSynchronize(t->stream));
+        if (t->d_log) { cudaFree(t->d_log); t->d_log = nullptr; t->log_cap = 0; }
+        TCK(cudaMalloc(&t->d_log, (size_t)iters * 3 * sizeof(double)));
+        t->log_cap = (size_t)iters * 3;
+    }
+    float *W = t->w;
+    for (int it = 0; it < iters; ++it) {
+        double *lg = t->d_log + (size_t)it * 3;
+        k_sample_idx<<<nblk(batch), 256, 0, t->stream>>>(t->d_idx, batch, n_train_rows, seed, (uint64_t)(first_iter + it));
+        k_gather_rows<<<nblk((size_t)batch * 203), 256, 0, t->stream>>>((const uint8_t *)rows_dev, t->d_idx, batch, weight_scale, t->x0, t->value, t->variance, t->weight);
+        int rc = forward(t, batch);
+        if (rc) return rc;
+        k_head<<<(batch + 127) / 128, 128, 0, t->stream>>>(t->h, W + O_FOW, W + O_FOB, W + O_UB, W + O_LB, t->value, t->variance, t->weight, batch, weighted,
+                                                           t->pred, t->lossv, t->dz);
+        k_std_mean<<<1, 256, 0, t->stream>>>(t->lossv, batch, lg);
+        rc = backward(t, batch);
+        if (rc) return rc;
+        k_sumsq<<<N_TENSORS, 256, 0, t->stream>>>(t->grad, t->d_toff, t->d_sumsq);
+        k_grad_norm<<<1, 1, 0, t->stream>>>(t->d_sumsq, grad_clip, lg + 2, t->d_coef);
+        if (grad_clip > 0.0) k_scale_dev<<<nblk(N_TRAIN), 256, 0, t->stream>>>(t->grad, N_TRAIN, t->d_coef);
+        // Yogi constants from the step counter alone (step_common)
+        const bool first = !t->have_state;
+        if (first) { t->step = 0; t->have_state = true; }
+        t->step += 1;
+        const double bc1 = 1.0 - pow(t->beta1, (double)t->step), bc2 = 1.0 - pow(t->beta2, (double)t->step);
+        YogiConst c;
+        c.beta1 = (float)t->beta1; c.one_minus_beta1 = (float)(1.0 - t->beta1); c.neg_one_minus_beta2 = (float)(-(1.0 - t->beta2));
+        c.wd = (float)t->wd; c.eps = (float)t->eps; c.sqrt_bc2 = (float)sqrt(bc2); c.step_size = (float)(t->lr / bc1); c.first = first ? 1 : 0;
+        k_yogi<<<nblk(N_TRAIN), 256, 0, t->stream>>>(t->w, t->grad, t->m, t->v, N_TRAIN, c);
+    }
+    TCK(cudaGetLastError());
+    TCK(cudaMemcpyAsync(log_out, t->d_log, (size_t)iters * 3 * sizeof(double), cudaMemcpyDeviceToHost, t->stream));
+    TCK(cudaStreamSynchronize(t->stream));
+    return B200_OK;
+}
+
+// Model_VV._loss under no_grad on device rows [first, first + n) (one chunk of Model.compute_loss, model/model.py:52-83), weight = visit *
+// weight_scale; *weight_sum = the fp64 sum of those weights (the chunk's size in a weighted combination)
+extern "C" int b200_trainer_loss_rows_dev(b200_trainer *t, const void *rows_dev, int first, int n, float weight_scale, int weighted,
+                                          double *loss, double *loss_std, double *weight_sum) {
+    if (!t || !rows_dev || first < 0 || n < 1 || n > t->max_batch) return tfail(B200_ERR_BAD_ARG, "trainer: bad argument (1 <= n <= max_batch)");
+    TCK(cudaSetDevice(t->device));
+    k_seq_idx<<<nblk(n), 256, 0, t->stream>>>(t->d_idx, n, first);
+    k_gather_rows<<<nblk((size_t)n * 203), 256, 0, t->stream>>>((const uint8_t *)rows_dev, t->d_idx, n, weight_scale, t->x0, t->value, t->variance, t->weight);
+    k_sum<<<1, 256, 0, t->stream>>>(t->weight, n, t->d_dsum);
+    double wsum = 0.0;
+    TCK(cudaMemcpyAsync(&wsum, t->d_dsum, sizeof(double), cudaMemcpyDeviceToHost, t->stream));
+    int rc = forward(t, n);
+    if (rc) return rc;
+    rc = loss_and_head(t, n, weighted, false, loss, loss_std);      // synchronises the stream
+    if (rc) return rc;
+    TCK(cudaGetLastError());
+    if (weight_sum) *weight_sum = wsum;
+    return B200_OK;
+}
+
+// max(value), max(variance) and the fp64 sum of visits over rows [0, n) (Model_VV.train_data's out_ubound, model_vv.py:227-231, and the mean of
+// Model.train_data's weight normalisation, model/model.py:186-187) without copying the rows to the host; fixed reduction order
+extern "C" int b200_rows_stats_dev(b200_trainer *t, const void *rows_dev, int n, float *max_value, float *max_variance, double *visit_sum) {
+    if (!t || !rows_dev || n < 1 || !max_value || !max_variance || !visit_sum) return tfail(B200_ERR_BAD_ARG, "trainer: bad argument");
+    TCK(cudaSetDevice(t->device));
+    k_rows_stats_part<<<STATS_CTAS, 256, 0, t->stream>>>((const uint8_t *)rows_dev, n, t->d_pmax, t->d_psum);
+    k_rows_stats_final<<<1, 1, 0, t->stream>>>(t->d_pmax, t->d_psum, t->d_max2, t->d_dsum);
+    TCK(cudaGetLastError());
+    float mx[2]; double sum = 0.0;
+    TCK(cudaMemcpyAsync(mx, t->d_max2, sizeof(mx), cudaMemcpyDeviceToHost, t->stream));
+    TCK(cudaMemcpyAsync(&sum, t->d_dsum, sizeof(double), cudaMemcpyDeviceToHost, t->stream));
+    TCK(cudaStreamSynchronize(t->stream));
+    *max_value = mx[0]; *max_variance = mx[1]; *visit_sum = sum;
+    return B200_OK;
 }

@@ -99,6 +99,20 @@ def load_checkpoint_weights(filename=EXP_PATH + "model_checkpoint"):
     return None
 
 
+def _combine_chunks(loss, std, bsize):
+    """Model.compute_loss's combination of per-chunk (mean, std, size) into one (model/model.py:67-83)"""
+    loss, std, bsize = np.array(loss), np.nan_to_num(np.array(std)), np.array(bsize)
+    d_size = bsize.sum()
+    combined = float(np.sum(loss * bsize) / d_size)
+    std_combined = float(np.sqrt(np.sum(bsize * std ** 2 + bsize * (loss ** 2 - combined ** 2)) / d_size))
+    return {"loss": combined, "loss_std": std_combined}
+
+
+# Model.train_data's options as its callers pass them (ValueSim.py:180); train_rows implements these values only
+_TRAIN_ROWS_FIXED = dict(validation_fraction=0.1, sample_replacement=True, oversampling=False, weighted=True, early_stopping=True,
+                         early_stopping_patience=10, early_stopping_threshold=1., shuffle=False)
+
+
 class Model_VV:
     """Model_VV().load(); .training(flag); .inference(batch); .train(batch); .train_data(data); .save()  (model/model_vv.py:104-231 on
     model/model.py:39-255).  Inference runs through the engine's network kernels, training through the device trainer."""
@@ -180,11 +194,7 @@ class Model_VV:
             mean, sd = t.loss(b, weighted=weighted)
             loss.append(mean); std.append(sd)
             bsize.append(float(np.sum(b[-1])) if weighted else float(len(b[0])))
-        loss, std, bsize = np.array(loss), np.nan_to_num(np.array(std)), np.array(bsize)
-        d_size = bsize.sum()
-        combined = float(np.sum(loss * bsize) / d_size)
-        std_combined = float(np.sqrt(np.sum(bsize * std ** 2 + bsize * (loss ** 2 - combined ** 2)) / d_size))
-        return {"loss": combined, "loss_std": std_combined}
+        return _combine_chunks(loss, std, bsize)
 
     def train(self, batch, grad_clip=0., g_norm_warn=1e3, weighted=False):   # model/model.py:95-119
         r = self._trainer_obj().step(batch, weighted=weighted, grad_clip=grad_clip)
@@ -245,6 +255,70 @@ class Model_VV:
             self.save(checkpoint)
         self._publish()
         self.training(False)
+
+    def train_rows(self, rows_dev_ptr, n_rows, batch_size=128, iters_per_val=500, max_iters=100000, checkpoint=EXP_PATH + "model_checkpoint",
+                   seed=0, chunksize=1024, **options):
+        """train_data on 212-byte replay rows that stay on the device (the engine's memory, b200_replay_peek_dev): out_ubound and the weight
+        mean come from b200_rows_stats_dev, batches are drawn on the device (Trainer.train_rows_dev, seeded by `seed`; the reference's draw is
+        np.random.choice), a validation interval runs with one synchronisation, and the validation loss is computed chunk by chunk on the device
+        and combined as compute_loss combines it.  Same split (the last 10 % of the rows, no shuffle), early stopping, checkpoint and log lines
+        as train_data.  Returns False without training when the split leaves no validation rows (the reference fails on d[:-0])."""
+        bad = {k: v for k, v in options.items() if k not in _TRAIN_ROWS_FIXED or v != _TRAIN_ROWS_FIXED[k]}
+        if bad:
+            raise ValueError("train_rows implements train_data with %s only; got %s" % (_TRAIN_ROWS_FIXED, bad))
+        n_rows = int(n_rows)
+        validation_size = int(n_rows * _TRAIN_ROWS_FIXED["validation_fraction"])
+        if validation_size == 0:
+            print("Not enough training data ({} < {}), collecting more data.".format(n_rows, int(np.ceil(1 / _TRAIN_ROWS_FIXED["validation_fraction"]))), **perr)
+            return False
+        t = self._trainer_obj()
+        max_value, max_variance, visit_sum = t.rows_stats(rows_dev_ptr, n_rows)
+        t.set_out_ubound(max_value, max_variance)                                             # model_vv.py:228-229
+        scale = float(n_rows / visit_sum)                                                     # weights / weights.mean(), model/model.py:186-187
+        n_train = n_rows - validation_size
+        print("Training data size: {}    Validation data size: {}".format(n_train, validation_size), **perr)
+        patience, threshold = _TRAIN_ROWS_FIXED["early_stopping_patience"], _TRAIN_ROWS_FIXED["early_stopping_threshold"]
+        fails, loss_val_min = 0, float("inf")
+        self.training(True)
+        for it0 in range(0, int(max_iters), int(iters_per_val)):
+            k = min(int(iters_per_val), int(max_iters) - it0)
+            log = t.train_rows_dev(rows_dev_ptr, n_train, batch_size, k, seed, it0, scale, weighted=True)
+            loss_avg = g_norm_avg = 0
+            for loss, _std, g_norm in log:
+                if g_norm > 1e3:
+                    print("Large gradient ({}) detected".format(g_norm), **perr)             # Model.train's g_norm_warn (model/model.py:103-105)
+                loss_avg += loss
+                g_norm_avg += g_norm
+            if k < iters_per_val:
+                break                                                                         # no validation after a partial interval
+            loss_val = self._loss_rows(rows_dev_ptr, n_train, n_rows, scale, chunksize)
+            loss_val_mean, loss_val_std = loss_val["loss"], loss_val["loss_std"] / validation_size ** 0.5
+            suffix = ""
+            if loss_val_mean - loss_val_min < loss_val_std * threshold:
+                fails = 0
+                if loss_val_mean < loss_val_min:
+                    suffix = "*"
+                    self.save(checkpoint, verbose=False)
+                    loss_val_min = loss_val_mean
+            else:
+                fails += 1
+                if fails >= patience:
+                    break
+            print("Iteration:{:7d}  training loss:{:6.4f}  validation loss:{:6.4f}±{:6.4f}  gradient norm:{:6.3f}    {}"
+                  .format(it0 + k, loss_avg / iters_per_val, loss_val_mean, loss_val_std, g_norm_avg / iters_per_val, suffix), **perr)
+        self.load(checkpoint)                                                                 # model/model.py:240-241: back to the best model
+        self._publish()
+        self.training(False)
+        return True
+
+    def _loss_rows(self, rows_dev_ptr, first, end, weight_scale, chunksize=1024):
+        """compute_loss(weighted=True) on device rows [first, end)"""
+        t = self._trainer_obj()
+        loss, std, bsize = [], [], []
+        for c in range(first, end, chunksize):
+            mean, sd, wsum = t.loss_rows_dev(rows_dev_ptr, c, min(chunksize, end - c), weight_scale, weighted=True)
+            loss.append(mean); std.append(sd); bsize.append(wsum)
+        return _combine_chunks(loss, std, bsize)
 
     def close(self):
         if self._trainer is not None:

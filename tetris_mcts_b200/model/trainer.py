@@ -29,8 +29,32 @@ def _lib():
         lib.b200_trainer_loss.argtypes = [P, P, P, P, P, C.c_int, C.c_int, P, P, P]
         lib.b200_trainer_step.argtypes = [P, P, P, P, P, C.c_int, C.c_int, C.c_double, P, P, P]
         lib.b200_trainer_step_rows_dev.argtypes = [P, P, C.c_int, P, C.c_int, C.c_float, C.c_int, C.c_double, P, P, P]
+        lib.b200_trainer_train_rows_dev.argtypes = [P, P, C.c_int, C.c_int, C.c_int, C.c_uint64, C.c_int64, C.c_float, C.c_int, C.c_double, P]
+        lib.b200_trainer_loss_rows_dev.argtypes = [P, P, C.c_int, C.c_int, C.c_float, C.c_int, P, P, P]
+        lib.b200_rows_stats_dev.argtypes = [P, P, C.c_int, P, P, P]
         _sig_done = True
     return lib
+
+
+_M64 = np.uint64(0xFFFFFFFFFFFFFFFF)
+
+
+def _splitmix64(x):
+    with np.errstate(over="ignore"):
+        z = (x + np.uint64(0x9E3779B97F4A7C15)) & _M64
+        z = (z ^ (z >> np.uint64(30))) * np.uint64(0xBF58476D1CE4E5B9)
+        z = (z ^ (z >> np.uint64(27))) * np.uint64(0x94D049BB133111EB)
+        return z ^ (z >> np.uint64(31))
+
+
+def sample_indices(seed, iteration, batch, n_rows):
+    """The batch Trainer.train_rows_dev draws on the device for one iteration (include/b200_tetris_mcts.h b200_trainer_train_rows_dev),
+    restated in numpy: idx[i] = splitmix64(splitmix64(splitmix64(seed) + iteration) + i) mod n_rows."""
+    base = _splitmix64(np.array([seed], np.uint64))[0]
+    with np.errstate(over="ignore"):
+        base = _splitmix64(np.array([base + np.uint64(iteration)], np.uint64))[0]
+        keys = _splitmix64(base + np.arange(batch, dtype=np.uint64))
+    return (keys % np.uint64(n_rows)).astype(np.int32)
 
 
 def _check(rc):
@@ -124,3 +148,24 @@ class Trainer:
                                                  int(bool(weighted)), float(grad_clip), out[0:1].ctypes.data_as(P), out[1:2].ctypes.data_as(P),
                                                  out[2:3].ctypes.data_as(P)))
         return {"loss": float(out[0]), "loss_std": float(out[1]), "grad_norm": float(out[2])}
+
+    def train_rows_dev(self, rows_dev_ptr, n_train_rows, batch, iters, seed, first_iter, weight_scale, weighted=True, grad_clip=0.0):
+        """`iters` steps of step_rows_dev on batches drawn on the device (sample_indices(seed, first_iter + it, batch, n_train_rows)), one host
+        synchronisation in all -> float64 [iters, 3] = per-step (loss, loss_std, grad_norm)."""
+        log = np.zeros((int(iters), 3), np.float64)
+        _check(_lib().b200_trainer_train_rows_dev(self.h, P(int(rows_dev_ptr)), int(n_train_rows), int(batch), int(iters), int(seed) & 0xFFFFFFFFFFFFFFFF,
+                                                  int(first_iter), float(weight_scale), int(bool(weighted)), float(grad_clip), L.ptr(log)))
+        return log
+
+    def loss_rows_dev(self, rows_dev_ptr, first, n, weight_scale, weighted=True):
+        """Model_VV._loss under no_grad on device rows [first, first + n) -> (mean, population std, sum of the weights)"""
+        out = np.zeros(3, np.float64)
+        _check(_lib().b200_trainer_loss_rows_dev(self.h, P(int(rows_dev_ptr)), int(first), int(n), float(weight_scale), int(bool(weighted)),
+                                                 out[0:1].ctypes.data_as(P), out[1:2].ctypes.data_as(P), out[2:3].ctypes.data_as(P)))
+        return float(out[0]), float(out[1]), float(out[2])
+
+    def rows_stats(self, rows_dev_ptr, n):
+        """(max value, max variance, fp64 sum of visits) of device rows [0, n)"""
+        mx, s = np.zeros(2, np.float32), np.zeros(1, np.float64)
+        _check(_lib().b200_rows_stats_dev(self.h, P(int(rows_dev_ptr)), int(n), mx[0:1].ctypes.data_as(P), mx[1:2].ctypes.data_as(P), L.ptr(s)))
+        return float(mx[0]), float(mx[1]), float(s[0])
