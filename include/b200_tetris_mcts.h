@@ -76,7 +76,9 @@ int b200_engine_destroy(b200_engine *e);
 int b200_engine_set_stream(b200_engine *e, void *cuda_stream);
 int b200_engine_get_stream(b200_engine *e, void **cuda_stream_out);
 
-/* --- Model.load (model/model.py:163-174): weights = the state_dict tensors concatenated (B200_N_WEIGHTS floats) */
+/* --- Model.load (model/model.py:163-174): weights = the state_dict tensors concatenated (B200_N_WEIGHTS floats).
+ *     A B200_EVAL_NET_TC engine returns B200_ERR_BAD_ARG, keeping its previous weights, when a conv or fc1 weight is non-finite or has
+ *     |w| * 64 > 65504 (fp16 overflow in the tensor cores' operand split); the same holds for b200_load_dist_weights. */
 int b200_load_weights(b200_engine *e, const float *weights);
 
 /* --- TreeAgent.update_root (agents/agent.py:296-301) for all games: recs[n_games][20] */

@@ -298,6 +298,11 @@ extern "C" int b200_engine_get_stream(b200_engine *e, void **cuda_stream_out) {
 // ---------------------------------------------------------------------------------------------------- weights
 extern "C" int b200_load_weights(b200_engine *e, const float *w) {
     if (!e || !w) return fail(B200_ERR_BAD_ARG, "null argument");
+#ifdef B200_WITH_TC
+    if (e->cfg.eval_kind == B200_EVAL_NET_TC && !tc_weights_fit(w))
+        return fail(B200_ERR_BAD_ARG, "net_tc: a conv or fc1 weight is non-finite or has |w| * 64 > 65504, which overflows the tensor cores' "
+                                      "fp16 x 2 operand split (eval_kind net takes finite weights of any size)");
+#endif
     CK(cudaSetDevice(e->cfg.device));
     const float *c1w = w, *c1b = c1w + 288, *c2w = c1b + 32, *c2b = c2w + 9216, *c3w = c2b + 32, *c3b = c3w + 9216;
     const float *f1w = c3b + 32, *f1b = f1w + 458752, *fow = f1b + 256, *fob = fow + 512, *ub = fob + 2, *lb = ub + 2;
@@ -402,6 +407,11 @@ extern "C" int b200_load_dist_weights(b200_engine *e, const float *w, int atoms)
     if (!e || !w || atoms < 2 || atoms > 64) return fail(B200_ERR_BAD_ARG, "bad argument");
     CK(cudaSetDevice(e->cfg.device));
     if (e->A.mode == MODE_DIST && atoms != e->A.dist_bins) return fail(B200_ERR_BAD_ARG, "atoms must equal dist_bins");
+#ifdef B200_WITH_TC
+    if (e->cfg.eval_kind == B200_EVAL_NET_TC && !dn_tc_weights_fit(w))
+        return fail(B200_ERR_BAD_ARG, "net_tc: a conv or fc1 weight is non-finite or has |w| * 64 > 65504, which overflows the tensor cores' "
+                                      "fp16 x 2 operand split (eval_kind net takes finite weights of any size)");
+#endif
     std::vector<float> h;
     dn_relayout(w, atoms, h);
     if (!e->d_dnw) { if (dalloc(e, &e->d_dnw, h.size(), false)) return B200_ERR_CUDA; }

@@ -323,6 +323,12 @@ struct DnTcState {
     uint8_t *d_act2 = nullptr; size_t tiles = 0;
 };
 
+// conv1, conv2 and fc1 go through the fp16 x 2 split (see tc_weights_fit); fc_v stays fp32
+static bool dn_tc_weights_fit(const float *w) {
+    const float *c1w = w, *c2w = c1w + 512 + 32, *f1w = c2w + 16384 + 32;
+    return tc_split_fits(c1w, 512) && tc_split_fits(c2w, 16384) && tc_split_fits(f1w, (size_t)128 * 2048);
+}
+
 // w = the state_dict-order weight vector of model_distributional.py (see dn_relayout).  Pure re-layout + fp16 splitting.
 static int dn_tc_prepare(void **state, const float *w, int atoms, cudaStream_t stream) {
     DnTcState *st = (DnTcState *)*state;

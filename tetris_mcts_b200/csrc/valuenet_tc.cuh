@@ -502,6 +502,18 @@ static inline void host_split2(float x, uint16_t *o) {   // x*scale = h1 + h2 in
 }
 static inline float host_half_f(uint16_t h) { __half x; memcpy(&x, &h, 2); return __half2float(x); }
 
+// The split scales a weight by TC_SCALE_W before rounding it to fp16: |w| * 64 above fp16's largest finite value (65504, |w| >= ~1023.5)
+// would become an infinity and poison every output.  True when every weight the split carries (conv1-3, fc1) is in range (NaN is not).
+static inline bool tc_split_fits(const float *x, size_t n) {
+    for (size_t i = 0; i < n; ++i)
+        if (!(fabsf(x[i]) * TC_SCALE_W <= 65504.f)) return false;
+    return true;
+}
+static bool tc_weights_fit(const float *w) {
+    const float *c1w = w, *c2w = w + 288 + 32, *c3w = c2w + 9216 + 32, *f1w = c3w + 9216 + 32;
+    return tc_split_fits(c1w, 288) && tc_split_fits(c2w, 9216) && tc_split_fits(c3w, 9216) && tc_split_fits(f1w, (size_t)256 * 1792);
+}
+
 // w = the state_dict-order weight vector of include/b200_tetris_mcts.h.  Pure re-layout + fp16 splitting.
 static int tc_prepare(void **state, const float *w, cudaStream_t stream) {
     TcState *st = (TcState *)*state;
