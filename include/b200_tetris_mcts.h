@@ -164,12 +164,12 @@ int b200_get_all_childs(int index, const int32_t *child, int M, uint8_t *mark);
 
 /* --- distributional cores (agents/core_distributional.py, BASELINE config 5), operator level, reference array layout:
  *     node_stats f32[M][5] = {visit, mean, reward, variance, M2}, node_dist f32[M][bins], child int32[M][7] */
-int b200_dist_shift_distribution(const float *dist, int bins, double x, double vmin, double vmax, float *out);     /* :12-36 */
+int b200_dist_shift_distribution(const float *dist, int bins, double x, double vmin, double vmax, float *out);     /* :12-36, x >= 0 */
 int b200_dist_mean_variance(const float *dist, int bins, double vmin, double vmax, double *mean, double *var);     /* :48-63 */
 int b200_dist_select_trace(int index, const int32_t *child, const float *node_stats, int M, int low, uint32_t *rng_state,
                            int32_t *trace_out, int max_trace, int32_t *trace_len);                                 /* :82-106 */
 int b200_dist_backup_trace(const int32_t *trace, int D, float *node_stats, float *node_dist, int M, int bins, double r,
-                           const float *dist, double vmin, double vmax);                                           /* :109-124 */
+                           const float *dist, double vmin, double vmax);                          /* :109-124, bins <= 64 */
 
 /* --- distributional engine (B200_MODE_DIST): Model.load / Model.inference of model/model_distributional.py:18-57 and the
  *     node-indexed arrays of one game.  weights: seq.conv1.w[32,1,4,4] b[32] seq.conv2.w[32,32,4,4] b[32] seq.fc1.w[128,2048]

@@ -673,7 +673,8 @@ int mo_agent_mcts(mo_agent *a, int sims) {
                     for (int r = 0; r < 20; ++r)
                         for (int c = 0; c < 10; ++c) st[r * 10 + c] = (int8_t)((key[r >> 1] >> ((r & 1) * 16 + c)) & 1);
                     for (int j = 0; j < 4; ++j) st[(key[10] >> (8 * j)) & 0xff] = -1;
-                    dn_forward(cf->weights, st, 1, cf->dist_bins, dist);
+                    if (cf->eval_mode == MO_EVAL_CALLBACK) cf->eval_cb(cf->eval_ctx, st, 1, dist, NULL);   /* dist_bins probabilities into v */
+                    else dn_forward(cf->weights, st, 1, cf->dist_bins, dist);
                 }
                 if (expand(a, leaf) < 0) continue;       /* tree dropped: this simulation is abandoned */
                 if (a->overflow) return -1;

@@ -53,7 +53,7 @@ typedef struct {
     double rollout_variance; /* Vanilla.py:54 1e3 */
     int eval_mode;      /* MO_EVAL_* */
     const float *weights;  /* MO_EVAL_NET: packed as valuenet_oracle.c expects */
-    mo_eval_fn eval_cb; void *eval_ctx;
+    mo_eval_fn eval_cb; void *eval_ctx;   /* MO_MODE_DIST: called with k = 1 and var = NULL, writes dist_bins probabilities to v */
     uint32_t search_seed;  /* per-agent xorshift stream replacing rand()/random.randint (SURVEY H4) */
     int stale_pop;         /* agent.py:229-232 erases by the freed slot's STALE game; 1 = reproduce */
     int dist_bins;         /* MO_MODE_DIST: atoms (DistValueSimOnline.py:13: 50) */

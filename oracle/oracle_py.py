@@ -252,6 +252,11 @@ class Agent:
         if eval_cb is not None:
             def tramp(ctx, states, k, v, var):
                 st = np.ctypeslib.as_array(states, shape=(k * 200,)).reshape(k, 1, 20, 10)
+                if mode == 3:                                         # distributional: eval_cb(states) -> f32[k, dist_bins]
+                    p = np.ravel(np.asarray(eval_cb(st), np.float32))
+                    for i in range(k * dist_bins):
+                        v[i] = float(p[i])
+                    return
                 rv, rvar = eval_cb(st)
                 for i in range(k):
                     v[i] = float(np.ravel(rv)[i])

@@ -3,6 +3,7 @@
   core_live_golden.npz  the same core.cpp's select_trace_obs / backup_trace_obs on the seeded arenas of test_cpu_oracle_pins.py
   valuenet_golden.npz outputs of the reference's own model/model_vv.py Model_VV (torch CPU) with seeded weights
   dist_golden.npz     outputs of the reference's own numba cores agents/core_distributional.py (fastmath: pinned to 1e-5)
+  dist_edges_golden.npz  the same numba cores on the edge cases of arena_gen (atoms 2-64, five ranges, bin-truncation shifts)
   agent_golden.npz    per-move statistics of the reference's own agents/ValueSimLP.py + agents/agent.py driving
                       the oracle env (the only non-reference part: pyTetris is absent upstream) with the synthetic
                       evaluator patched onto the agent instance (no reference file is modified)
@@ -571,6 +572,44 @@ def gen_dist():
     print("dist_golden: %d cases" % n)
 
 
+def gen_dist_edges():
+    """dist_edges_golden.npz: the reference's own numba shift_distribution, mean_variance and backup_trace_distributional on the edge
+    cases of arena_gen (atoms 2-64, five value ranges, x at 0, at multiples of delta, where int(b + x / delta) truncates one bin
+    further than b + int(x / delta), at and beyond the range; histograms random, one-hot at either end, one bin only)."""
+    import agents.core_distributional as R
+    from arena_gen import dist_edge_configs, edge_dists, edge_shifts, edge_backup_cases
+    cfgs = dist_edge_configs()
+    out = dict(cfg=np.array(cfgs, np.float64))
+    sh_idx, sh_x, sh_out, mv_idx, mv_out = [], [], [], [], []
+    tr = dict(idx=[], r=[], trace=[], ns=[], nd=[], bk_ns=[], bk_nd=[])
+    n_trunc = 0
+    for c, (bins, vmin, vmax) in enumerate(cfgs):
+        dists = edge_dists(bins, bins)
+        out["dists_%d" % c] = dists
+        xs, near = edge_shifts(bins, vmin, vmax, 1000 + c)
+        n_trunc += len(near)
+        for k, d in enumerate(dists):
+            for x in xs:
+                sh_idx.append((c, k)); sh_x.append(x)
+                sh_out.append(np.asarray(R.shift_distribution(d, float(x), vmin, vmax), np.float32))
+            mv_idx.append((c, k)); mv_out.append(np.array(R.mean_variance(d, vmin, vmax), np.float64))
+        for case in edge_backup_cases(bins, vmin, vmax, 2000 + c):
+            ns, nd = case["node_stats"].copy(), case["node_dist"].copy()
+            R.backup_trace_distributional(case["trace"], ns, nd, case["r"], case["dist"], vmin, vmax)
+            for key, v in (("idx", (c, case["dist_k"])), ("r", case["r"]), ("trace", case["trace"]), ("ns", case["node_stats"]),
+                           ("nd", case["node_dist"].ravel()), ("bk_ns", ns), ("bk_nd", nd.ravel())):
+                tr[key].append(v)
+    off = lambda parts: np.cumsum([0] + [len(p) for p in parts]).astype(np.int64)     # noqa: E731
+    out.update(sh_idx=np.array(sh_idx, np.int32), sh_x=np.array(sh_x, np.float64), sh_off=off(sh_out), sh_out=np.concatenate(sh_out),
+               mv_idx=np.array(mv_idx, np.int32), mv_out=np.stack(mv_out),
+               tr_idx=np.array(tr["idx"], np.int32), tr_r=np.array(tr["r"], np.float64), tr_off=off(tr["trace"]),
+               tr_trace=np.concatenate(tr["trace"]), tr_node_off=off(tr["ns"]), tr_ns=np.concatenate(tr["ns"]), tr_bk_ns=np.concatenate(tr["bk_ns"]),
+               tr_nd_off=off(tr["nd"]), tr_nd=np.concatenate(tr["nd"]), tr_bk_nd=np.concatenate(tr["bk_nd"]))
+    np.savez_compressed(os.path.join(HERE, "dist_edges_golden.npz"), **out)
+    print("dist_edges_golden: %d configurations, %d shifts (%d truncation x values), %d mean_variance, %d traces"
+          % (len(cfgs), len(sh_x), n_trunc, len(mv_out), len(tr["r"])))
+
+
 if __name__ == "__main__":
     O.build(ref=True)
     shim_path = os.path.join(ROOT, "oracle", "_ref", "librandshim.so")
@@ -582,6 +621,8 @@ if __name__ == "__main__":
     pt, core = O.mount_reference()
     if "--dist" in sys.argv:
         gen_dist()
+    elif "--dist-edges" in sys.argv:
+        gen_dist_edges()
     elif "--train" in sys.argv:
         gen_train()
     elif "--agent-online" in sys.argv:
@@ -614,6 +655,7 @@ if __name__ == "__main__":
         gen_agent_explicit_gc(pt)
         gen_agent_cpp(pt)
         gen_dist()
+        gen_dist_edges()
         gen_train()
         import subprocess
         subprocess.run([sys.executable, os.path.abspath(__file__), "--agent-online-all"], check=True)

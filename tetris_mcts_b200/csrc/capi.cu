@@ -1220,7 +1220,7 @@ extern "C" int b200_get_all_childs(int index, const int32_t *child, int M, uint8
 
 // ---------------------------------------------------------------------------------------------------- distributional cores (a16)
 extern "C" int b200_dist_shift_distribution(const float *dist, int bins, double x, double vmin, double vmax, float *out) {
-    if (!dist || !out || bins < 1 || bins > 4096) return fail(B200_ERR_BAD_ARG, "bad argument");
+    if (!dist || !out || bins < 1 || bins > 4096 || !(x >= 0)) return fail(B200_ERR_BAD_ARG, "bad argument");   // x < 0 would index below bin 0
     if (b200_device_count() == 0) return fail(B200_ERR_CUDA, "no CUDA device: this library has no CPU path");
     TwinBufs b; float *d_in = nullptr, *d_out = nullptr;
     TW(b.up(&d_in, dist, (size_t)bins)); TW(b.up(&d_out, (const float *)nullptr, (size_t)bins));
@@ -1264,12 +1264,14 @@ extern "C" int b200_dist_select_trace(int index, const int32_t *child, const flo
 
 extern "C" int b200_dist_backup_trace(const int32_t *trace, int D, float *node_stats, float *node_dist, int M, int bins, double r,
                                       const float *dist, double vmin, double vmax) {
-    if (!trace || D < 1 || !node_stats || !node_dist || !dist || bins < 1) return fail(B200_ERR_BAD_ARG, "bad argument");
+    if (!trace || D < 1 || !node_stats || !node_dist || !dist || bins < 1 || bins > 64) return fail(B200_ERR_BAD_ARG, "bad argument");
+    for (int t = 0; t < D; ++t)
+        if (trace[t] < 0 || trace[t] >= M) return fail(B200_ERR_BAD_ARG, "trace index out of range");
     if (b200_device_count() == 0) return fail(B200_ERR_CUDA, "no CUDA device: this library has no CPU path");
-    TwinBufs b; float *d_ns = nullptr, *d_nd = nullptr, *d_dist = nullptr, *d_scr = nullptr;
+    TwinBufs b; float *d_ns = nullptr, *d_nd = nullptr, *d_dist = nullptr;
     TW(b.up(&b.trace, trace, (size_t)D)); TW(b.up(&d_ns, (const float *)node_stats, (size_t)M * 5)); TW(b.up(&d_nd, (const float *)node_dist, (size_t)M * bins));
-    TW(b.up(&d_dist, dist, (size_t)bins)); TW(b.up(&d_scr, (const float *)nullptr, (size_t)bins));
-    k_dist_backup<<<1, 1>>>(b.trace, D, d_ns, d_nd, bins, r, d_dist, vmin, vmax, d_scr);
+    TW(b.up(&d_dist, dist, (size_t)bins));
+    k_dist_backup_trace<<<1, 32>>>(b.trace, D, d_ns, d_nd, bins, r, d_dist, vmin, vmax);   // the engine's backup (dist_backup_trace_warp)
     CK(cudaGetLastError());
     CK(cudaMemcpy(node_stats, d_ns, (size_t)M * 5 * 4, cudaMemcpyDeviceToHost));
     CK(cudaMemcpy(node_dist, d_nd, (size_t)M * bins * 4, cudaMemcpyDeviceToHost));

@@ -99,38 +99,91 @@ __device__ inline int dist_select_trace(int index, const int32_t *child, const f
     return D;
 }
 
-// core_distributional.py:109-124; scratch = bins floats
-__device__ inline void dist_backup_trace(const int32_t *trace, int D, float *node_stats, float *node_dist, int bins, double r,
-                                         const float *dist, double vmin, double vmax, float *scratch) {
-    const double mean = dist_mean(dist, bins, vmin, vmax);
-    for (int t = 0; t < D; ++t) {
-        const int idx = trace[t];
-        float *ns = node_stats + (size_t)idx * 5, *nd = node_dist + (size_t)idx * bins;
-        const double _r = r - (double)ns[2];
-        dist_shift(dist, bins, _r, vmin, vmax, scratch);
-        for (int b = 0; b < bins; ++b) {
-            float num = __fadd_rn(__fmul_rn(nd[b], ns[0]), scratch[b]);
-            nd[b] = (float)((double)num / ((double)ns[0] + 1.0));
+// One level of backup_trace_distributional (core_distributional.py:112-124), one warp, lanes over the bins (bins <= 64): shift the
+// leaf histogram d by x = r - reward (shift_distribution, :12-36), fold it into the node's running average nd, then lane 0 updates the
+// node's Welford statistics ns = {visit, mean, reward, variance, M2}.  mean = dist_mean(d).
+// shift_distribution is taken as a gather with the reference's bin mapping: source b goes to lb = min(int(b + bin_shift), T) with weight
+// 1 - frac and to ub = min(lb + 1, T) with frac, int() truncating the DOUBLE sum.  That sum is b + s or b + s + 1 (s = int(bin_shift)):
+// the second when bin_shift lies just below an integer and adding b rounds it up to that integer (DESIGN §3).  So the sources reaching
+// a target tb < T lie in tb - s - 2 .. tb - s, and T also collects every source clamped onto it.  Each target adds its sources' terms
+// in ascending source order, (1 - frac) before frac, each rounded to float as the scalar loop does.
+__device__ inline void dist_backup_level(const float *d, int bins, double delta, double mean, double r, float *ns, float *nd, int lane) {
+    const int T = bins - 1;
+    // only lane 0 touches ns in memory (it rewrites it below); the others get visit and reward from its registers.  Each lane reads and
+    // writes only its own bins of nd, so the levels need no other synchronisation, even when a node repeats in the trace.
+    float ns0 = 0.f, ns1 = 0.f, ns2 = 0.f, ns4 = 0.f;
+    if (lane == 0) { ns0 = ns[0]; ns1 = ns[1]; ns2 = ns[2]; ns4 = ns[4]; }
+    ns0 = __shfl_sync(0xffffffffu, ns0, 0);
+    ns2 = __shfl_sync(0xffffffffu, ns2, 0);
+    const double _r = r - (double)ns2;
+    const double bin_shift = _r / delta, frac = bin_shift - floor(bin_shift);
+    const int s = bin_shift < (double)bins ? (int)bin_shift : bins;
+    // b + bin_shift < 128 has an ulp of at most 2^-46, so it can only round up to the next integer when 1 - frac is below that: otherwise
+    // every source maps to b + s: a target tb < T takes exactly tb - s - 1 (its frac) and tb - s (its 1 - frac), T takes T - s - 1 (its
+    // frac) and both terms of every source from T - s on
+    const bool plain = frac < 1.0 - 0x1p-40;
+    for (int tb = lane; tb < bins; tb += 32) {
+        float acc = 0.f;
+        if (plain) {
+            const int b1 = tb - s - 1, b2 = tb - s;
+            if (b1 >= 0 && b1 < bins) acc = (float)__dadd_rn((double)acc, __dmul_rn((double)d[b1], frac));
+            if (tb < T) {
+                if (b2 >= 0 && b2 < bins) acc = (float)__dadd_rn((double)acc, __dmul_rn((double)d[b2], 1.0 - frac));
+            } else {
+                for (int b = max(b2, 0); b < bins; ++b) {
+                    acc = (float)__dadd_rn((double)acc, __dmul_rn((double)d[b], 1.0 - frac));
+                    acc = (float)__dadd_rn((double)acc, __dmul_rn((double)d[b], frac));
+                }
+            }
+        } else {
+            const int hi = tb < T ? min(tb - s, T) : T;
+            for (int b = max(tb - s - 2, 0); b <= hi; ++b) {
+                const double sb = __dadd_rn((double)b, bin_shift);
+                const int lb = sb >= (double)T ? T : (int)sb, ub = lb + 1 >= T ? T : lb + 1;
+                if (lb == tb) acc = (float)__dadd_rn((double)acc, __dmul_rn((double)d[b], 1.0 - frac));
+                if (ub == tb) acc = (float)__dadd_rn((double)acc, __dmul_rn((double)d[b], frac));
+            }
         }
+        const float num = __fadd_rn(__fmul_rn(nd[tb], ns0), acc);
+        nd[tb] = (float)((double)num / ((double)ns0 + 1.0));
+    }
+    if (lane == 0) {
         const double x = mean + _r;
-        ns[0] = __fadd_rn(ns[0], 1.f);
-        const double delta = x - (double)ns[1];
-        ns[1] = (float)((double)ns[1] + delta / (double)ns[0]);
-        const double delta2 = x - (double)ns[1];
-        ns[4] = (float)((double)ns[4] + delta * delta2);
-        if (ns[0] > 1.f) ns[3] = (float)((double)ns[4] / ((double)ns[0] - 1.0));
+        const float n1 = __fadd_rn(ns0, 1.f);
+        const double dl = x - (double)ns1;
+        const float m1 = (float)((double)ns1 + dl / (double)n1);
+        const double dl2 = x - (double)m1;
+        const float m2 = (float)((double)ns4 + dl * dl2);
+        ns[0] = n1; ns[1] = m1; ns[4] = m2;
+        if (n1 > 1.f) ns[3] = (float)((double)m2 / ((double)n1 - 1.0));
     }
 }
 
-// ---- single-call twins (one thread; these are operator-level parity entry points, not the throughput path)
+// backup_trace_distributional (core_distributional.py:109-124) for one trace, one full warp.  d: the leaf histogram in shared memory;
+// node rows ns_stride floats apart in node_stats (5 in the reference layout, NSTAT_WORDS in the arena).  The engine's k_dist_backup and
+// the operator b200_dist_backup_trace both run this.
+__device__ inline void dist_backup_trace_warp(const float *d, int bins, double vmin, double vmax, double r, const int32_t *trace, int D,
+                                              float *node_stats, int ns_stride, float *node_dist, int lane) {
+    const double delta = (vmax - vmin) / bins;
+    const double mean = dist_mean(d, bins, vmin, vmax);
+    for (int t = 0; t < D; ++t) {
+        const int idx = trace[t];
+        dist_backup_level(d, bins, delta, mean, r, node_stats + (size_t)idx * ns_stride, node_dist + (size_t)idx * bins, lane);
+    }
+}
+
+// ---- single-call twins (operator-level parity entry points, not the throughput path)
 __global__ void k_dist_shift(const float *dist, int bins, double x, double vmin, double vmax, float *out) { dist_shift(dist, bins, x, vmin, vmax, out); }
 __global__ void k_dist_mean_variance(const float *dist, int bins, double vmin, double vmax, double *out) { dist_mean_variance(dist, bins, vmin, vmax, out[0], out[1]); }
 __global__ void k_dist_select(int index, const int32_t *child, const float *node_stats, int low, int32_t *trace, int max_trace, uint32_t *rng, int32_t *len) {
     *len = dist_select_trace(index, child, node_stats, low, trace, max_trace, rng);
 }
-__global__ void k_dist_backup(const int32_t *trace, int D, float *node_stats, float *node_dist, int bins, double r, const float *dist, double vmin,
-                              double vmax, float *scratch) {
-    dist_backup_trace(trace, D, node_stats, node_dist, bins, r, dist, vmin, vmax, scratch);
+__global__ void __launch_bounds__(32) k_dist_backup_trace(const int32_t *trace, int D, float *node_stats, float *node_dist, int bins, double r,
+                                                           const float *dist, double vmin, double vmax) {   // one warp, bins <= 64
+    __shared__ float d[64];
+    for (int b = threadIdx.x; b < bins; b += 32) d[b] = dist[b];
+    __syncwarp();
+    dist_backup_trace_warp(d, bins, vmin, vmax, r, trace, D, node_stats, 5, node_dist, threadIdx.x);
 }
 
 }  // namespace b200

@@ -3,6 +3,7 @@
 // per SM on 132 SMs.  The tree walk is pointer chasing (latency bound); occupancy, not ILP, hides HBM latency here.
 #pragma once
 #include "search_dev.cuh"
+#include "dist_dev.cuh"
 
 namespace b200 {
 
@@ -858,10 +859,8 @@ __global__ void k_eval_synthetic_dist(Arena A) {
     }
 }
 
-// backup_trace_distributional (core_distributional.py:109-124), one warp per game, lanes over the histogram bins.
-// The trace levels are independent of each other (dist and r are fixed), so each level is: shift the evaluator's
-// histogram by (r - reward[idx]) (closed-form gather of shift_distribution, same add order per bin; the clamped top bin is
-// summed sequentially), fold it into the node's running average, update the node's Welford statistics.
+// backup_trace_distributional (core_distributional.py:109-124), one warp per game, lanes over the histogram bins
+// (dist_backup_trace_warp, dist_dev.cuh: the same code the operator b200_dist_backup_trace runs).
 __global__ void __launch_bounds__(128) k_dist_backup(Arena A) {
     __shared__ float s_dist[4][64];
     const int wid = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -869,54 +868,16 @@ __global__ void __launch_bounds__(128) k_dist_backup(Arena A) {
     if (g >= A.G || A.status[g] != ST_OK) return;
     const int D = A.trace_len[g], kind = A.leaf_kind[g];
     if (kind == LEAF_SUSPENDED || D <= 0) return;
-    const int bins = A.dist_bins, T = bins - 1;
+    const int bins = A.dist_bins;
     const int32_t *trace = A.trace + (size_t)g * A.trace_max;
     const int leaf = trace[D - 1];
-    float *nsb = A.nstat + (size_t)g * A.M * NSTAT_WORDS, *ndb = A.ndist + (size_t)g * A.M * bins;
     const double r = (double)__int_as_float(A.row[node_at(A, g, leaf) * ROW_WORDS + 23]);   // leaf_game.getScore(), DistValueSimOnline.py:64
     float *d = s_dist[wid];
     for (int b = lane; b < bins; b += 32)
         d[b] = kind == LEAF_EXPANDED ? A.dist_eval[(size_t)g * bins + b] : (b == 0 ? 1.f : 0.f);   // v_dummy, DistValueSimOnline.py:26-27
     __syncwarp();
-    const double delta = (A.dist_vmax - A.dist_vmin) / bins;
-    double mean = 0.0;                                               // mean_dist, core_distributional.py:39-45 (sequential order)
-    for (int b = 0; b < bins; ++b) mean = __dadd_rn(mean, __dmul_rn((double)d[b], (b + 0.5) * delta));
-    for (int t = 0; t < D; ++t) {
-        const int idx = trace[t];
-        float *ns = nsb + (size_t)idx * NSTAT_WORDS, *nd = ndb + (size_t)idx * bins;
-        const float ns0 = ns[0], ns1 = ns[1], ns2 = ns[2], ns4 = ns[4];
-        const double _r = r - (double)ns2;
-        const double bin_shift = _r / delta, frac = bin_shift - floor(bin_shift);
-        const int s = (int)bin_shift;                                // (int)(b + bin_shift) = b + s for bin_shift >= 0
-        for (int tb = lane; tb < bins; tb += 32) {
-            float acc = 0.f;
-            if (tb < T) {
-                int b1 = tb - s - 1, b2 = tb - s;
-                if (b1 >= 0 && b1 < bins) acc = (float)__dadd_rn((double)acc, __dmul_rn((double)d[b1], frac));          // its upper target
-                if (b2 >= 0 && b2 < bins) acc = (float)__dadd_rn((double)acc, __dmul_rn((double)d[b2], 1.0 - frac));    // its lower target
-            } else {
-                int b0 = T - s - 1;
-                if (b0 >= 0 && b0 < bins) acc = (float)__dadd_rn((double)acc, __dmul_rn((double)d[b0], frac));
-                for (int b = (T - s < 0 ? 0 : T - s); b < bins; ++b) {                                                   // clamped bins
-                    acc = (float)__dadd_rn((double)acc, __dmul_rn((double)d[b], 1.0 - frac));
-                    acc = (float)__dadd_rn((double)acc, __dmul_rn((double)d[b], frac));
-                }
-            }
-            float num = __fadd_rn(__fmul_rn(nd[tb], ns0), acc);
-            nd[tb] = (float)((double)num / ((double)ns0 + 1.0));
-        }
-        if (lane == 0) {
-            const double x = mean + _r;
-            const float n1 = __fadd_rn(ns0, 1.f);
-            const double dl = x - (double)ns1;
-            const float m1 = (float)((double)ns1 + dl / (double)n1);
-            const double dl2 = x - (double)m1;
-            const float m2 = (float)((double)ns4 + dl * dl2);
-            ns[0] = n1; ns[1] = m1; ns[4] = m2;
-            if (n1 > 1.f) ns[3] = (float)((double)m2 / ((double)n1 - 1.0));
-        }
-        __syncwarp();
-    }
+    dist_backup_trace_warp(d, bins, A.dist_vmin, A.dist_vmax, r, trace, D, A.nstat + (size_t)g * A.M * NSTAT_WORDS, NSTAT_WORDS,
+                           A.ndist + (size_t)g * A.M * bins, lane);
 }
 
 // ---------------------------------------------------------------- compute_stats / get_action (agent.py:153-185)
