@@ -212,6 +212,19 @@ int b200_replay_append(b200_engine *e, const uint8_t *rows_host, int n_rows);   
 typedef struct b200_trainer b200_trainer;
 const char *b200_trainer_last_error(void);
 int b200_trainer_create(int device, const float *weights, int max_batch, b200_trainer **out);     /* Model_VV._init_model (model_vv.py:125-134) */
+/* Trainer kinds: which GEMMs a training step's contractions run on.  Every b200_trainer_* entry point below works on either kind with the
+ * same contract; b200_trainer_create is b200_trainer_create_kind(..., B200_TRAIN_FP64, ...).
+ *   B200_TRAIN_FP64  CUDA-core GEMMs accumulating in fp64, rounded once to fp32.
+ *   B200_TRAIN_TC    the conv / fc1 forward, input-gradient and weight-gradient GEMMs on Hopper tensor cores (3xTF32: each fp32 operand
+ *                    split into two tf32 terms, three wgmma products accumulated in fp32, fp32 chains capped at 2048 k with fp64 partials
+ *                    summed in a fixed order).  Loss, gradient norm and each gradient tensor stay within 1e-5 (relative, resp. of the
+ *                    tensor's norm) of float64 arithmetic; fp32's exponent range is kept, so small gradients do not flush.  Bit-
+ *                    reproducible run to run, and train_rows_dev stays bit-identical to step_rows_dev fed the same indices, as for fp64.
+ * Weights and Yogi state mean the same in both kinds, so a checkpoint of one kind loads into the other.
+ * b200_trainer_create_kind returns B200_ERR_BAD_ARG for an unknown kind. */
+#define B200_TRAIN_FP64 0
+#define B200_TRAIN_TC 1
+int b200_trainer_create_kind(int device, const float *weights, int max_batch, int kind, b200_trainer **out);
 int b200_trainer_destroy(b200_trainer *t);
 int b200_trainer_set_hyper(b200_trainer *t, double lr, double beta1, double beta2, double eps, double weight_decay);   /* Yogi(...) model_vv.py:132 */
 int b200_trainer_set_out_ubound(b200_trainer *t, float ub_value, float ub_variance);             /* model_vv.py:227-231 */

@@ -12,7 +12,8 @@ perr = dict(file=stderr, flush=True)
 class ValueSim(TreeAgent):
     _mode = "single"
 
-    def __init__(self, online=True, memory_size=500000, min_visits_to_store=10, gamma=0.999, memory_growth_rate=5000, weights=None, **kwargs):
+    def __init__(self, online=True, memory_size=500000, min_visits_to_store=10, gamma=0.999, memory_growth_rate=5000, weights=None,
+                 train_kind="fp64", **kwargs):
         kwargs.pop("max_nodes", None)
         if weights is None:
             # ValueSim.py:42-44: self.model = Model(); self.model.load(); self.model.training(False).  Model.load (model/model.py:163-174)
@@ -29,7 +30,8 @@ class ValueSim(TreeAgent):
             self._eng.replay_enable(min_visits=min_visits_to_store, capacity=memory_size)
             # accumulation policy 3 is train_nodes' rule: train once memory_index >= min(n_trains * memory_growth_rate, memory_size)
             self._eng.replay_policy(3, memory_growth_rate=memory_growth_rate)
-            self._online = OnlineTrainer(self._eng, self._weights, memory_size, batch_size=1024, iters_per_val=100, max_iters=50000)   # ValueSim.py:180
+            self._online = OnlineTrainer(self._eng, self._weights, memory_size, batch_size=1024, iters_per_val=100, max_iters=50000,
+                                         train_kind=train_kind)   # ValueSim.py:180
             self._gcs = 0
             print('online: freed observations are stored on the device as in ValueSim.store_nodes (ValueSim.py:122-159) and the value network '
                   'is trained on them after the collections that fill the memory (train_nodes, ValueSim.py:161-185)', **perr)

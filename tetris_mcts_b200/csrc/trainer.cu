@@ -16,14 +16,43 @@
 // (tests: rtol 1e-5 against goldens recorded from the reference's own Model_VV.train on torch CPU).  Convolutions are lowered to
 // GEMMs through explicit im2col buffers in HBM (the PyTorch [co][ci][ky][kx] weight layout is used as it lies: k = ci*9 + ky*3 + kx).
 // No atomics: every reduction has a fixed order, training is bit-reproducible run to run.
+//
+// Trainer kinds (b200_trainer_create_kind).  B200_TRAIN_FP64 runs every contraction through k_gemm (CUDA cores, fp64 accumulation, above).
+// B200_TRAIN_TC runs the forward, input-gradient and conv / fc1 weight-gradient GEMMs through k_gemm_tc on Hopper tensor cores (wgmma
+// m64nNk8 .f32.tf32.tf32); fc_out's 2 x 256 weight gradient, the bias sums and everything around the GEMMs are shared by both kinds.
+// Precision of the tc kind (3xTF32):
+//   - split: every fp32 operand x is stored as big = rna_tf32(x), small = rna_tf32(x - big) (x - big is exact in fp32).  tf32 keeps 10 + 1
+//     mantissa bits and fp32's exponent range, so |x - big| <= 2^-11 |x|, |x - big - small| <= 2^-22 |x| down to fp32's subnormal floor:
+//     nothing is pre-scaled and nothing underflows that fp32 itself would hold (gradients of 1e-30 keep 22 bits).  Below 2^-126 the terms
+//     are subnormal and the split's error becomes absolute, <= 2^-137; above (2 - 2^-11) 2^127 (0.02 % below fp32's largest) big rounds
+//     to infinity.
+//   - products: a*b is accumulated as a_small*b_big + a_big*b_small + a_big*b_big (small products first, fp32 accumulators); the dropped
+//     a_small*b_small and the two split residuals leave <= 3 * 2^-22 |a b| per product.
+//   - reductions: the tensor core's fp32 accumulation does not round to nearest (measured on an H100: a 2048-k wgmma chain was biased by
+//     ~1e-4 of the result on same-sign sums, consistent with truncating each addition), so a wgmma chain covers one 32-wide k tile only
+//     (12 MMAs, scale-d = 0 at the tile's first): its sum goes into a separate fp32 register accumulator by an IEEE round-to-nearest FADD.
+//     Truncation over 32 terms is <= 32 * 2^-23 = 4e-6 of the tile's |terms| worst case and ~2^-24 sqrt(32) typical; the FADD chain of
+//     one chunk covers at most TG_KCHUNK = 2048 consecutive k (64 tiles): statistically ~sqrt(64) * 2^-24 = 5e-7 of the sum of |terms|
+//     (worst case 64 * 2^-24 = 4e-6).  Longer reductions (the weight gradients reduce
+//     over B * 56 .. B * 144 pixels, 590 k terms at B = 4096) are cut into chunks of <= 2048 k; each chunk writes its tile as an fp64
+//     partial and k_finish adds the partials in ascending chunk order in fp64, so the error does not grow with the batch.  The chunk
+//     length rests on the worst case: one FADD chain over all 590 k terms (18 k tile sums) is bounded only by 18k * 2^-24 = 1.1e-3 of
+//     the |terms|, 2048 k by 4e-6, under the 1e-5 the trainer is held to (typical errors grow like sqrt(n) and stay below 1e-5 either
+//     way on the tests' data, so no test separates the two).
+//   - together: every GEMM output is within ~1e-6 of the sum of its |terms| (split, tile truncation and chunk sum; ~1e-5 worst case), the same class as the
+//     inference split (valuenet_tc.cuh); tests hold loss, gradient norm and each gradient tensor to 1e-5 of float64 autograd.
+//   - determinism: the chunking depends on the shapes alone and no reduction uses atomics: the tc kind is bit-reproducible run to run and
+//     b200_trainer_train_rows_dev stays bit-identical to b200_trainer_step_rows_dev fed the same indices.
 #include <cuda_runtime.h>
 #include <cmath>
 #include <cstdio>
 #include <cstring>
+#include <algorithm>
 #include <string>
 #include <vector>
 
 #include "../../include/b200_tetris_mcts.h"
+#include "gmma.cuh"
 
 namespace {
 
@@ -110,6 +139,139 @@ __global__ void __launch_bounds__(256) k_gemm(const float *__restrict__ A, const
             const int m = m0 + ty * 4 + i, n = n0 + tx * 4 + j;
             if (m < M && n < N) C[(size_t)m * N + n] = acc[i][j];
         }
+}
+
+// ------------------------------------------------------------------------------------------------ GEMM on tensor cores (3xTF32, the tc kind)
+// C[M,N] (+)= op(A)[M,K] * op(B)[K,N] with k_gemm's TA / TB storage conventions; ct: C is stored transposed ([N][M]), which lets a
+// 32-row weight gradient run as a 32-column product.  One warpgroup per CTA, a 64 x BN output tile, 32-wide k tiles.  The staging
+// loads read the tile (transposed or not) into registers, split each value into two tf32 terms and store both K-major in shared
+// memory in the no-swizzle core-matrix layout [k chunk of 4][row][16 B]: a k8 step is two chunks ROWS * 16 B apart (LBO), 8-row groups
+// are 128 B apart (SBO).  The next tile's loads are in flight while the wgmmas of this one run.  blockIdx.z covers k range z; more than
+// one range: each writes its fp32 tile as an fp64 partial to Cpart + z*M*N and k_finish sums them (see the file header).
+constexpr int TG_BM = 64, TG_BK = 32, TG_KCHUNK = 2048;
+static_assert(TG_KCHUNK % TG_BK == 0, "chunks are whole k tiles");
+
+__device__ __forceinline__ float tf32_rna(float x) {
+    uint32_t r;
+    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
+    return __uint_as_float(r);
+}
+// D[64 x N] (+)= A[64 x 8] * B[N x 8]^T, tf32 operands from shared memory (K-major), fp32 accumulators in valuenet_tc.cuh's layout:
+// thread t holds rows 16*(t/32) + (t%32)/4 (+8) and columns 8j + 2*(t%4) (+1) in d[4j + {0,1}] (row) / d[4j + {2,3}] (row + 8).
+// accumulate == 0 overwrites D.
+__device__ __forceinline__ void wgmma_tf32(float (&d)[16], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {"
+        "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15"
+        "}, %16, %17, p, 1, 1;\n}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+__device__ __forceinline__ void wgmma_tf32(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {"
+        "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+        "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31"
+        "}, %32, %33, p, 1, 1;\n}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+
+template <bool TA, bool TB, int BN>
+__global__ void __launch_bounds__(128) k_gemm_tc(const float *__restrict__ A, const float *__restrict__ B, double *__restrict__ Cpart,
+                                                 int M, int N, int K, int k_per_split, float *__restrict__ Cdirect, const float *__restrict__ bias,
+                                                 int relu, int ct) {
+    static_assert(BN == 32 || BN == 64, "wgmma_tf32 covers N = 32 and 64");
+    constexpr int NA = TG_BM * TG_BK / 128, NB = BN * TG_BK / 128, KC = TG_BK / 4;
+    __shared__ __align__(128) float sA[2][KC][TG_BM][4];     // [big / small][k chunk][row][4 k]
+    __shared__ __align__(128) float sB[2][KC][BN][4];
+    const int tid = threadIdx.x;
+    const int m0 = blockIdx.y * TG_BM, n0 = blockIdx.x * BN;
+    const int kb = blockIdx.z * k_per_split, ke = min(K, kb + k_per_split);
+    // element i of a thread's share of the A / B tile: (row, k) chosen so that a warp reads along the stored fast index
+    auto a_at = [&](int i, int &mm, int &kk) { const int e = i * 128 + tid; if (TA) { mm = e & 63; kk = e >> 6; } else { kk = e & 31; mm = e >> 5; } };
+    auto b_at = [&](int i, int &nn, int &kk) { const int e = i * 128 + tid; if (TB) { kk = e & 31; nn = e >> 5; } else { nn = e % BN; kk = e / BN; } };
+    float ra[NA], rb[NB];
+    auto load = [&](int k0) {
+#pragma unroll
+        for (int i = 0; i < NA; ++i) {
+            int mm, kk; a_at(i, mm, kk);
+            const int k = k0 + kk, m = m0 + mm;
+            ra[i] = (k < ke && m < M) ? (TA ? A[(size_t)k * M + m] : A[(size_t)m * K + k]) : 0.f;
+        }
+#pragma unroll
+        for (int i = 0; i < NB; ++i) {
+            int nn, kk; b_at(i, nn, kk);
+            const int k = k0 + kk, n = n0 + nn;
+            rb[i] = (k < ke && n < N) ? (TB ? B[(size_t)n * K + k] : B[(size_t)k * N + n]) : 0.f;
+        }
+    };
+    float d[BN / 2], acc[BN / 2];                          // d: this k tile's sum (tensor core), acc: the chunk's sum (FADD, round to nearest)
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) { d[i] = 0.f; acc[i] = 0.f; }
+    const uint32_t sa = b200::smem_u32(&sA[0][0][0][0]), sb = b200::smem_u32(&sB[0][0][0][0]);
+    constexpr uint32_t A_TERM = KC * TG_BM * 16, B_TERM = KC * BN * 16;     // bytes of one split term
+    load(kb);
+    for (int k0 = kb; k0 < ke; k0 += TG_BK) {
+        __syncthreads();                                   // the previous tile's wgmmas are complete (every thread waited on them)
+#pragma unroll
+        for (int i = 0; i < NA; ++i) {
+            int mm, kk; a_at(i, mm, kk);
+            const float big = tf32_rna(ra[i]);
+            sA[0][kk >> 2][mm][kk & 3] = big;
+            sA[1][kk >> 2][mm][kk & 3] = tf32_rna(ra[i] - big);
+        }
+#pragma unroll
+        for (int i = 0; i < NB; ++i) {
+            int nn, kk; b_at(i, nn, kk);
+            const float big = tf32_rna(rb[i]);
+            sB[0][kk >> 2][nn][kk & 3] = big;
+            sB[1][kk >> 2][nn][kk & 3] = tf32_rna(rb[i] - big);
+        }
+        b200::fence_async_smem();
+        __syncthreads();
+        b200::wgmma_fence();
+#pragma unroll
+        for (int s = 0; s < TG_BK / 8; ++s) {              // a_small*b_big, a_big*b_small, a_big*b_big (small products first)
+            const uint32_t ao = s * 2 * TG_BM * 16, bo = s * 2 * BN * 16;
+            wgmma_tf32(d, b200::gmma_desc(sa + A_TERM + ao, TG_BM * 16, 128), b200::gmma_desc(sb + bo, BN * 16, 128), s ? 1u : 0u);
+            wgmma_tf32(d, b200::gmma_desc(sa + ao, TG_BM * 16, 128), b200::gmma_desc(sb + B_TERM + bo, BN * 16, 128), 1u);
+            wgmma_tf32(d, b200::gmma_desc(sa + ao, TG_BM * 16, 128), b200::gmma_desc(sb + bo, BN * 16, 128), 1u);
+        }
+        b200::wgmma_commit();
+        if (k0 + TG_BK < ke) load(k0 + TG_BK);            // next tile's global loads overlap this tile's MMAs
+        b200::wgmma_wait<0>();
+        b200::fence_regs(d);
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[i] += d[i];
+    }
+    const int w = tid >> 5, lane = tid & 31, qd = lane & 3, rl = lane >> 2;
+    double *Cp = Cdirect ? nullptr : Cpart + (size_t)blockIdx.z * M * N;
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int m = m0 + 16 * w + 8 * h + rl, n = n0 + 8 * j + 2 * qd + e;
+                if (m >= M || n >= N) continue;
+                const size_t o = ct ? (size_t)n * M + m : (size_t)m * N + n;
+                const float a = acc[4 * j + 2 * h + e];
+                if (Cdirect) {                             // one k range: bias / ReLU here (no partial-sum buffer)
+                    float v = a;
+                    if (bias) v = v + bias[n];
+                    if (relu) v = fmaxf(v, 0.f);
+                    Cdirect[o] = v;
+                } else {
+                    Cp[o] = (double)a;
+                }
+            }
 }
 
 // out[i] = float(sum_z part[z][i] (+ bias[i % N] when bias)), optional ReLU; also used to finish single-split GEMMs
@@ -365,7 +527,7 @@ inline int nblk(size_t n, int t = 256) { size_t b = (n + t - 1) / t; return (int
 }  // namespace
 
 struct b200_trainer {
-    int device = 0, max_batch = 0;
+    int device = 0, max_batch = 0, kind = B200_TRAIN_FP64;
     cudaStream_t stream = nullptr;
     std::vector<void *> allocs;
     float *w = nullptr, *grad = nullptr, *m = nullptr, *v = nullptr;     // [N_ALL] / [N_TRAIN]
@@ -377,7 +539,7 @@ struct b200_trainer {
     float *x0, *value, *variance, *weight;
     float *col1, *a1, *col2, *a2, *col3, *a3, *flat, *h, *pred, *lossv, *dz;
     float *dh, *dflat, *dc3, *dcol3, *da2, *dcol2, *da1;
-    double *part; size_t part_elems = 0;
+    double *part; size_t part_elems = 0;                                // split-k / chunk partial sums (fp64)
     // b200_trainer_train_rows_dev / _loss_rows_dev / b200_rows_stats_dev
     float *d_coef = nullptr, *d_pmax = nullptr, *d_max2 = nullptr; double *d_psum = nullptr, *d_dsum = nullptr;
     double *d_log = nullptr; size_t log_cap = 0;                         // [iters][3] step log, grown on demand (not in allocs)
@@ -412,17 +574,66 @@ int gemm(b200_trainer *t, const float *A, const float *B, float *C, int M, int N
     return 0;
 }
 
+// k ranges of a tc GEMM, from the shapes alone: chunks of <= TG_KCHUNK (the fp32 chain cap), and when the output has too few tiles to fill
+// the GPU (< 2 x 132 CTAs), more ranges of >= 256 k.  In that second case splits <= ceil(264 / tiles) and M*N <= tiles * 64 * 64, so the
+// partials take <= (264 + tiles) * 4096 < 528 * 4096 doubles (tc_part_elems).
+inline int tc_k_per_split(int M, int N, int K, int BN) {
+    const int tiles = ((M + TG_BM - 1) / TG_BM) * ((N + BN - 1) / BN);
+    int splits = (K + TG_KCHUNK - 1) / TG_KCHUNK;
+    if (K >= 512 && tiles * splits < 132 * 2) splits = std::max(splits, std::min((132 * 2 + tiles - 1) / tiles, K / 256));
+    return ((K + splits - 1) / splits + TG_BK - 1) / TG_BK * TG_BK;
+}
+
+// C = op(A) op(B) on tensor cores (k_gemm_tc), optional bias / ReLU; ct: C stored transposed
+template <bool TA, bool TB, int BN>
+int gemm_tc(b200_trainer *t, const float *A, const float *B, float *C, int M, int N, int K, const float *bias, int relu, int ct = 0) {
+    const int kps = tc_k_per_split(M, N, K, BN), splits = (K + kps - 1) / kps;
+    dim3 grid((N + BN - 1) / BN, (M + TG_BM - 1) / TG_BM, splits);
+    if (splits == 1) {
+        k_gemm_tc<TA, TB, BN><<<grid, 128, 0, t->stream>>>(A, B, nullptr, M, N, K, kps, C, bias, relu, ct);
+        return 0;
+    }
+    if ((size_t)splits * M * N > t->part_elems) return tfail(B200_ERR_BAD_ARG, "trainer: partial-sum buffer too small");
+    k_gemm_tc<TA, TB, BN><<<grid, 128, 0, t->stream>>>(A, B, t->part, M, N, K, kps, nullptr, nullptr, 0, ct);
+    k_finish<<<nblk((size_t)M * N), 256, 0, t->stream>>>(t->part, splits, (size_t)M * N, ct ? M : N, bias, relu, C);
+    return 0;
+}
+
+// the partial-sum buffer of the tc kind at max_batch: the conv / fc1 weight gradients in TG_KCHUNK chunks, or the small-grid bound above
+size_t tc_part_elems(int max_batch) {
+    const size_t B = (size_t)max_batch;
+    auto chunks = [](size_t K) { return (K + TG_KCHUNK - 1) / TG_KCHUNK; };
+    size_t n = (size_t)528 * 4096;
+    n = std::max(n, chunks(B) * 256 * 1792);                 // fc1
+    n = std::max(n, chunks(B * 144) * 9 * 32);               // conv1
+    n = std::max(n, chunks(B * 96) * 288 * 32);              // conv2 (conv3 reduces over fewer pixels)
+    return n;
+}
+
+// C = op(A) op(B) (+ bias, ReLU) in the trainer's kind; BN is the tc kernel's tile width for this shape
+template <bool TA, bool TB, int BN>
+int mm(b200_trainer *t, const float *A, const float *B, float *C, int M, int N, int K, const float *bias, int relu) {
+    if (t->kind == B200_TRAIN_TC) return gemm_tc<TA, TB, BN>(t, A, B, C, M, N, K, bias, relu);
+    return gemm<TA, TB>(t, A, B, C, M, N, K, bias, relu);
+}
+// conv weight gradient dW[32][Kc] = dout^T [32 x P] . col [P x Kc]; the tc kind computes dW^T = col^T dout (32 output columns) and stores
+// it transposed
+int conv_wgrad(b200_trainer *t, const float *dout, const float *col, float *dW, int Kc, int P) {
+    if (t->kind == B200_TRAIN_TC) return gemm_tc<true, false, 32>(t, col, dout, dW, Kc, 32, P, nullptr, 0, 1);
+    return gemm<true, false>(t, dout, col, dW, 32, Kc, P, nullptr, 0);
+}
+
 int forward(b200_trainer *t, int B) {
     float *W = t->w;
     int rc = 0;
     k_im2col<<<nblk((size_t)B * 144 * 9), 256, 0, t->stream>>>(t->x0, B, 20, 10, 1, t->col1);
-    rc |= gemm<false, true>(t, t->col1, W + O_C1W, t->a1, B * 144, 32, 9, W + O_C1B, 1);          // model_vv.py:32-33
+    rc |= mm<false, true, 32>(t, t->col1, W + O_C1W, t->a1, B * 144, 32, 9, W + O_C1B, 1);        // model_vv.py:32-33
     k_im2col<<<nblk((size_t)B * 96 * 288), 256, 0, t->stream>>>(t->a1, B, 18, 8, 32, t->col2);
-    rc |= gemm<false, true>(t, t->col2, W + O_C2W, t->a2, B * 96, 32, 288, W + O_C2B, 1);          // :34-35
+    rc |= mm<false, true, 32>(t, t->col2, W + O_C2W, t->a2, B * 96, 32, 288, W + O_C2B, 1);        // :34-35
     k_im2col<<<nblk((size_t)B * 56 * 288), 256, 0, t->stream>>>(t->a2, B, 16, 6, 32, t->col3);
-    rc |= gemm<false, true>(t, t->col3, W + O_C3W, t->a3, B * 56, 32, 288, W + O_C3B, 1);          // :36-37
+    rc |= mm<false, true, 32>(t, t->col3, W + O_C3W, t->a3, B * 56, 32, 288, W + O_C3B, 1);        // :36-37
     k_nhwc_to_flat<<<nblk((size_t)B * 1792), 256, 0, t->stream>>>(t->a3, B, t->flat);              // :38 nn.Flatten on NCHW
-    rc |= gemm<false, true>(t, t->flat, W + O_F1W, t->h, B, 256, 1792, W + O_F1B, 1);              // :39-40
+    rc |= mm<false, true, 64>(t, t->flat, W + O_F1W, t->h, B, 256, 1792, W + O_F1B, 1);            // :39-40
     return rc;
 }
 
@@ -452,27 +663,27 @@ int loss_and_head(b200_trainer *t, int B, int weighted, bool want_grad, double *
 int backward(b200_trainer *t, int B) {
     float *W = t->w, *G = t->grad;
     int rc = 0;
-    // fc_out: dWo[j][k] = sum_b dz[b][j] h[b][k]; dbo[j] = sum_b dz[b][j]
+    // fc_out: dWo[j][k] = sum_b dz[b][j] h[b][k]; dbo[j] = sum_b dz[b][j]  (k_gemm in both kinds: 2 x 256 outputs)
     rc |= gemm<true, false>(t, t->dz, t->h, G + O_FOW, 2, 256, B, nullptr, 0);
     k_colsum<<<1, 256, 0, t->stream>>>(t->dz, B, 2, G + O_FOB);
     k_dh<<<nblk((size_t)B * 256), 256, 0, t->stream>>>(t->dz, W + O_FOW, t->h, B, t->dh);
     // fc1: dW1[n][k] = sum_b dh[b][n] flat[b][k]; db1; dflat = dh . W1
-    rc |= gemm<true, false>(t, t->dh, t->flat, G + O_F1W, 256, 1792, B, nullptr, 0);
+    rc |= mm<true, false, 64>(t, t->dh, t->flat, G + O_F1W, 256, 1792, B, nullptr, 0);
     k_colsum<<<8, 256, 0, t->stream>>>(t->dh, B, 256, G + O_F1B);
-    rc |= gemm<false, false>(t, t->dh, W + O_F1W, t->dflat, B, 1792, 256, nullptr, 0);
+    rc |= mm<false, false, 64>(t, t->dh, W + O_F1W, t->dflat, B, 1792, 256, nullptr, 0);
     k_flat_to_nhwc_relu<<<nblk((size_t)B * 1792), 256, 0, t->stream>>>(t->dflat, t->flat, B, t->dc3);   // ReLU after conv3 (act3)
     // conv3
-    rc |= gemm<true, false>(t, t->dc3, t->col3, G + O_C3W, 32, 288, B * 56, nullptr, 0);
+    rc |= conv_wgrad(t, t->dc3, t->col3, G + O_C3W, 288, B * 56);
     k_colsum<<<1, 256, 0, t->stream>>>(t->dc3, B * 56, 32, G + O_C3B);
-    rc |= gemm<false, false>(t, t->dc3, W + O_C3W, t->dcol3, B * 56, 288, 32, nullptr, 0);
+    rc |= mm<false, false, 64>(t, t->dc3, W + O_C3W, t->dcol3, B * 56, 288, 32, nullptr, 0);
     k_col2im_relu<<<nblk((size_t)B * 96 * 32), 256, 0, t->stream>>>(t->dcol3, t->a2, B, 16, 6, 32, t->da2);
     // conv2
-    rc |= gemm<true, false>(t, t->da2, t->col2, G + O_C2W, 32, 288, B * 96, nullptr, 0);
+    rc |= conv_wgrad(t, t->da2, t->col2, G + O_C2W, 288, B * 96);
     k_colsum<<<1, 256, 0, t->stream>>>(t->da2, B * 96, 32, G + O_C2B);
-    rc |= gemm<false, false>(t, t->da2, W + O_C2W, t->dcol2, B * 96, 288, 32, nullptr, 0);
+    rc |= mm<false, false, 64>(t, t->da2, W + O_C2W, t->dcol2, B * 96, 288, 32, nullptr, 0);
     k_col2im_relu<<<nblk((size_t)B * 144 * 32), 256, 0, t->stream>>>(t->dcol2, t->a1, B, 18, 8, 32, t->da1);
     // conv1 (no input gradient needed)
-    rc |= gemm<true, false>(t, t->da1, t->col1, G + O_C1W, 32, 9, B * 144, nullptr, 0);
+    rc |= conv_wgrad(t, t->da1, t->col1, G + O_C1W, 9, B * 144);
     k_colsum<<<1, 256, 0, t->stream>>>(t->da1, B * 144, 32, G + O_C1B);
     return rc;
 }
@@ -492,13 +703,18 @@ extern "C" int b200_trainer_destroy(b200_trainer *t) {
 }
 
 extern "C" int b200_trainer_create(int device, const float *weights, int max_batch, b200_trainer **out) {
+    return b200_trainer_create_kind(device, weights, max_batch, B200_TRAIN_FP64, out);
+}
+
+extern "C" int b200_trainer_create_kind(int device, const float *weights, int max_batch, int kind, b200_trainer **out) {
     if (!weights || !out || max_batch < 1 || max_batch > 65536) return tfail(B200_ERR_BAD_ARG, "trainer: bad argument (1 <= max_batch <= 65536)");
+    if (kind != B200_TRAIN_FP64 && kind != B200_TRAIN_TC) return tfail(B200_ERR_BAD_ARG, "trainer: unknown kind (B200_TRAIN_FP64 or B200_TRAIN_TC)");
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return tfail(B200_ERR_CUDA, "no CUDA device: this library has no CPU path");
     TCK(cudaSetDevice(device));
     b200_trainer *t = new b200_trainer();
     struct Guard { b200_trainer *t; ~Guard() { if (t) b200_trainer_destroy(t); } } guard{t};
-    t->device = device; t->max_batch = max_batch;
+    t->device = device; t->max_batch = max_batch; t->kind = kind;
     TCK(cudaStreamCreateWithFlags(&t->stream, cudaStreamNonBlocking));
     const size_t B = (size_t)max_batch;
     int rc = 0;
@@ -511,8 +727,9 @@ extern "C" int b200_trainer_create(int device, const float *weights, int max_bat
     rc |= talloc(t, &t->pred, B * 2); rc |= talloc(t, &t->lossv, B); rc |= talloc(t, &t->dz, B * 2);
     rc |= talloc(t, &t->dh, B * 256); rc |= talloc(t, &t->dflat, B * 1792); rc |= talloc(t, &t->dc3, B * 56 * 32); rc |= talloc(t, &t->dcol3, B * 56 * 288);
     rc |= talloc(t, &t->da2, B * 96 * 32); rc |= talloc(t, &t->dcol2, B * 96 * 288); rc |= talloc(t, &t->da1, B * 144 * 32);
-    // split-k partial sums (fp64): only the weight-gradient products are split; the largest is fc1 (256 x 1792) with <= 8 k ranges
-    t->part_elems = (size_t)8 * 256 * 1792;
+    // split-k partial sums (fp64): fp64 kind: only the weight-gradient products are split; the largest is fc1 (256 x 1792) with <= 8 k
+    // ranges.  tc kind: tc_part_elems.
+    t->part_elems = kind == B200_TRAIN_TC ? tc_part_elems(max_batch) : (size_t)8 * 256 * 1792;
     rc |= talloc(t, &t->part, t->part_elems);
     rc |= talloc(t, &t->d_coef, 1); rc |= talloc(t, &t->d_pmax, 2 * STATS_CTAS); rc |= talloc(t, &t->d_psum, STATS_CTAS);
     rc |= talloc(t, &t->d_max2, 2); rc |= talloc(t, &t->d_dsum, 1);

@@ -117,10 +117,13 @@ class Model_VV:
     """Model_VV().load(); .training(flag); .inference(batch); .train(batch); .train_data(data); .save()  (model/model_vv.py:104-231 on
     model/model.py:39-255).  Inference runs through the engine's network kernels, training through the device trainer."""
 
-    def __init__(self, device=0, seed=0, **kwargs):
+    def __init__(self, device=0, seed=0, train_kind="fp64", **kwargs):
         from ..engine import BatchedEngine
+        from .trainer import KINDS
+        if train_kind not in KINDS:
+            raise ValueError("train_kind must be one of %s, not %r" % (sorted(KINDS), train_kind))
         self.weights = init_weights(seed)
-        self.device = device
+        self.device, self.train_kind = device, train_kind
         self._eng = BatchedEngine(1, max_nodes=64, eval_kind=kwargs.get("eval_kind", "net"), device=device)
         self._eng.load_weights(self.weights)
         self._trainer = None
@@ -131,7 +134,7 @@ class Model_VV:
     def _trainer_obj(self):
         if self._trainer is None:
             from .trainer import Trainer
-            self._trainer = Trainer(self.weights, max_batch=4096, device=self.device)    # Yogi(lr=1e-3, eps=1e-3, weight_decay=1e-3), model_vv.py:132
+            self._trainer = Trainer(self.weights, max_batch=4096, device=self.device, kind=self.train_kind)    # Yogi(lr=1e-3, eps=1e-3, weight_decay=1e-3), model_vv.py:132
             if self._opt_state is not None:
                 self._trainer.set_state(*self._opt_state)
         return self._trainer

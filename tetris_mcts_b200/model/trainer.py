@@ -1,6 +1,9 @@
 """ctypes face of the device trainer (tetris_mcts_b200/csrc/trainer.cu, include/b200_tetris_mcts.h b200_trainer_*): one optimiser step of the
 reference's value network — Model_VV._loss (model/model_vv.py:136-153, GaussianLL :94-101), Model.train (model/model.py:95-119), Yogi.step
-(model/yogi.py:39-90) — entirely on the GPU.  No CPU path: without the library / a device the calls raise."""
+(model/yogi.py:39-90) — entirely on the GPU.  No CPU path: without the library / a device the calls raise.
+
+kind: "fp64" runs the contractions on CUDA cores with fp64 accumulation (the reference kind); "tc" runs them on Hopper tensor cores with
+the 3xTF32 split (trainer.cu header, include/b200_tetris_mcts.h B200_TRAIN_TC).  Weights and optimiser state are the same in both kinds."""
 import ctypes as C
 
 import numpy as np
@@ -8,6 +11,7 @@ import numpy as np
 from .. import _lib as L
 
 N_TRAIN = 478338            # trainable floats (state_dict order without out_ubound / out_lbound)
+KINDS = {"fp64": 0, "tc": 1}  # B200_TRAIN_FP64, B200_TRAIN_TC
 P = C.c_void_p
 _sig_done = False
 
@@ -18,6 +22,7 @@ def _lib():
     if not _sig_done:
         lib.b200_trainer_last_error.restype = C.c_char_p
         lib.b200_trainer_create.argtypes = [C.c_int, P, C.c_int, C.POINTER(P)]
+        lib.b200_trainer_create_kind.argtypes = [C.c_int, P, C.c_int, C.c_int, C.POINTER(P)]
         lib.b200_trainer_destroy.argtypes = [P]
         lib.b200_trainer_set_hyper.argtypes = [P] + [C.c_double] * 5
         lib.b200_trainer_set_out_ubound.argtypes = [P, C.c_float, C.c_float]
@@ -75,12 +80,15 @@ def _batch(batch):
 
 
 class Trainer:
-    def __init__(self, weights, max_batch=4096, device=0, lr=1e-3, betas=(0.9, 0.999), eps=1e-3, weight_decay=1e-3):
+    def __init__(self, weights, max_batch=4096, device=0, lr=1e-3, betas=(0.9, 0.999), eps=1e-3, weight_decay=1e-3, kind="fp64"):
+        if kind not in KINDS:
+            raise ValueError("trainer kind must be one of %s, not %r" % (sorted(KINDS), kind))
+        self.kind = kind
         w = np.ascontiguousarray(weights, np.float32).ravel()
         if w.size != L.N_WEIGHTS:
             raise ValueError("expected %d floats (state_dict order)" % L.N_WEIGHTS)
         self.h, self.max_batch, self.device = P(), int(max_batch), int(device)
-        _check(_lib().b200_trainer_create(int(device), L.ptr(w), int(max_batch), C.byref(self.h)))
+        _check(_lib().b200_trainer_create_kind(int(device), L.ptr(w), int(max_batch), KINDS[kind], C.byref(self.h)))
         _check(_lib().b200_trainer_set_hyper(self.h, lr, betas[0], betas[1], eps, weight_decay))     # Yogi(lr=1e-3, eps=1e-3, weight_decay=1e-3), model_vv.py:132
 
     def close(self):

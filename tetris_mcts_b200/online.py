@@ -10,8 +10,13 @@ from .model.model_vv import EXP_PATH
 
 
 class OnlineTrainer:
-    def __init__(self, eng, weights, capacity, batch_size=1024, iters_per_val=100, max_iters=50000, checkpoint=EXP_PATH + "model_checkpoint"):
+    def __init__(self, eng, weights, capacity, batch_size=1024, iters_per_val=100, max_iters=50000, checkpoint=EXP_PATH + "model_checkpoint",
+                 train_kind="fp64"):
         import torch
+        from .model.trainer import KINDS
+        if train_kind not in KINDS:
+            raise ValueError("train_kind must be one of %s, not %r" % (sorted(KINDS), train_kind))
+        self.train_kind = train_kind
         dev = torch.device("cuda", int(eng.cfg.device))            # the engine's device, not torch's current one
         self.buf = torch.empty((int(capacity), replay.SAMPLE_BYTES), dtype=torch.uint8, device=dev)
         torch.cuda.synchronize(dev)                                # the engine copies on its own stream: nothing of torch's may be pending on buf
@@ -22,7 +27,7 @@ class OnlineTrainer:
     def _model(self):
         if self.model is None:
             from .model.model_vv import Model_VV
-            self.model = Model_VV(device=int(self.eng.cfg.device), eval_kind="net")
+            self.model = Model_VV(device=int(self.eng.cfg.device), eval_kind="net", train_kind=self.train_kind)
             self.model.weights = self.weights
             self.model._eng.load_weights(self.weights)
         return self.model

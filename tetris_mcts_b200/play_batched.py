@@ -89,7 +89,8 @@ def run(args, out=sys.stdout, timing=None):
         from .online import OnlineTrainer
         eng.replay_enable(min_visits=25 if mode == "lp" else 10, capacity=args.memory_size)
         eng.replay_policy(args.accumulation_policy, episodes_per_train=args.episodes_per_train, memory_growth_rate=args.memory_growth_rate)
-        trainer = OnlineTrainer(eng, weights, args.memory_size, batch_size=args.train_batch_size, max_iters=args.train_max_iters)   # ValueSim.py:180
+        trainer = OnlineTrainer(eng, weights, args.memory_size, batch_size=args.train_batch_size, max_iters=args.train_max_iters,
+                                train_kind=args.train_kind)   # ValueSim.py:180
     status = RealtimeStatus(args.status_dir) if args.realtime_status else None
     saver = None
     if args.save:                                                                          # play.py:93-94, 131-132
@@ -172,6 +173,8 @@ def parse_args(argv=None):
     p.add_argument('--memory_growth_rate', default=5000, type=int, help='rows the training threshold grows by per training (policy 3)')
     p.add_argument('--train_batch_size', default=1024, type=int, help='training batch size (--online)')
     p.add_argument('--train_max_iters', default=50000, type=int, help='most optimiser steps per training (--online; early stopping usually ends it)')
+    p.add_argument('--train_kind', default='fp64', choices=('fp64', 'tc'),
+                   help='trainer GEMMs (--online): fp64 CUDA cores, or tc = Hopper tensor cores with the 3xTF32 split')
     p.add_argument('--max_moves', default=0, type=int)
     return p.parse_args(argv)
 
