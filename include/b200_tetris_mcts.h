@@ -202,6 +202,7 @@ int b200_replay_policy_step(b200_engine *e, int64_t current_episode, int32_t *tr
 int b200_replay_policy_trained(b200_engine *e, int64_t current_episode);
 int b200_replay_peek_dev(b200_engine *e, void *out_dev, int n_rows);
 int b200_replay_append(b200_engine *e, const uint8_t *rows_host, int n_rows);   /* rows join the memory as a collection's would: in order, until it is full */
+int b200_replay_append_dev(b200_engine *e, const void *rows_dev, int n_rows);   /* the same from a DEVICE buffer (e.g. rows all-gathered from other ranks) */
 
 /* --- value-network training step (SURVEY 8f.2): Model_VV._loss / Model.train / Yogi.step / Model_VV.train_data of the reference
  *     (model/model_vv.py:94-153,227-231, model/model.py:52-119, model/yogi.py:39-90) on the device.  weights = the state_dict vector of
@@ -258,6 +259,24 @@ int b200_trainer_loss_rows_dev(b200_trainer *t, const void *rows_dev, int first,
 /* max(value), max(variance) and the fp64 sum of visits of device rows [0, n) (out_ubound, model_vv.py:227-231; the weight mean,
  * model/model.py:186-187), reduced in a fixed order on the trainer's stream */
 int b200_rows_stats_dev(b200_trainer *t, const void *rows_dev, int n, float *max_value, float *max_variance, double *visit_sum);
+/* --- data-parallel training: R ranks each compute the gradient of one slice of a batch, exchange the fp64 vectors and apply the same update.
+ *     b200_trainer_set_stream: all later work of the trainer runs on the caller's stream (NULL: a private one again), so an exchange can be
+ *       ordered on it without a host synchronisation.
+ *     b200_trainer_grad_rows_dev: rows [lo, hi) of the batch b200_trainer_train_rows_dev draws for iteration `iter` (the same row formula, with
+ *       the global row number i); forward, loss and backward on those rows with the gradient scaled by 1 / batch.  grad_dev (DEVICE) gets
+ *       B200_TRAIN_VEC = 478338 + 3 doubles: the unrounded fp64 gradient (the values the fp32 gradient is rounded from) and the slice's
+ *       {count, mean, M2} of (weight *) logl.  Asynchronous.  B200_ERR_BAD_ARG unless 0 <= lo < hi <= batch and hi - lo <= max_batch.
+ *     b200_trainer_apply_grads_dev: parts_dev (DEVICE) = n_parts such vectors in rank order; g = (float)(((p0 + p1) + p2) + ...) element-wise,
+ *       the loss moments joined in the same order, then train_rows_dev's gradient norm, clip and Yogi step; {loss, loss_std, grad_norm} go to
+ *       device log slot log_slot.  Asynchronous.  One part covering the whole batch is bit-identical to a train_rows_dev step (weights,
+ *       gradient, Yogi state, gradient norm; the loss may differ by reassociation).  Every rank applying the same parts holds the same bits.
+ *     b200_trainer_read_log: synchronises and copies log slots [0, n) as [n][3] doubles. */
+#define B200_TRAIN_VEC (478338 + 3)
+int b200_trainer_set_stream(b200_trainer *t, void *cuda_stream);
+int b200_trainer_grad_rows_dev(b200_trainer *t, const void *rows_dev, int n_train_rows, int batch, int lo, int hi, uint64_t seed, int64_t iter,
+                               float weight_scale, int weighted, double *grad_dev);
+int b200_trainer_apply_grads_dev(b200_trainer *t, const double *parts_dev, int n_parts, double grad_clip, int log_slot);
+int b200_trainer_read_log(b200_trainer *t, int n, double *host);
 
 #ifdef __cplusplus
 }

@@ -89,6 +89,7 @@ def lib():
         L.b200_replay_policy_trained.argtypes = [P, C.c_int64]
         L.b200_replay_peek_dev.argtypes = [P, P, C.c_int]
         L.b200_replay_append.argtypes = [P, P, C.c_int]
+        L.b200_replay_append_dev.argtypes = [P, P, C.c_int]
         L.b200_load_dist_weights.argtypes = [P, P, C.c_int]
         L.b200_distnet_forward.argtypes = [P, P, C.c_int, C.c_int, P]
         L.b200_export_dist.argtypes = [P, C.c_int, P, P]

@@ -1515,6 +1515,19 @@ extern "C" int b200_replay_append(b200_engine *e, const uint8_t *rows, int n) {
     return rp_set_count(e, count + (take > 0 ? take : 0));
 }
 
+// b200_replay_append from a DEVICE buffer: rank 0 of a data-parallel run appends the rows the other ranks' collections stored this move
+extern "C" int b200_replay_append_dev(b200_engine *e, const void *rows, int n) {
+    if (!e || !e->A.replay || (n > 0 && !rows) || n < 0) return fail(B200_ERR_BAD_ARG, "replay memory not enabled / bad argument");
+    CK(cudaSetDevice(e->cfg.device));
+    int32_t count = 0;
+    int rc = rp_count(e, &count);
+    if (rc) return rc;
+    int take = e->A.replay_cap - count;
+    if (take > n) take = n;
+    if (take > 0) CK(cudaMemcpyAsync(e->A.replay + (size_t)count * 212, rows, (size_t)take * 212, cudaMemcpyDeviceToDevice, e->stream));
+    return rp_set_count(e, count + (take > 0 ? take : 0));
+}
+
 // the first n rows of the memory, copied to a DEVICE buffer without emptying it (the arrays the reference hands to train(): m_state ... [:memory_index])
 extern "C" int b200_replay_peek_dev(b200_engine *e, void *out_dev, int n) {
     if (!e || !out_dev || n < 0 || !e->A.replay || n > e->replay_alloc) return fail(B200_ERR_BAD_ARG, "bad argument");

@@ -274,11 +274,14 @@ __global__ void __launch_bounds__(128) k_gemm_tc(const float *__restrict__ A, co
             }
 }
 
-// out[i] = float(sum_z part[z][i] (+ bias[i % N] when bias)), optional ReLU; also used to finish single-split GEMMs
-__global__ void k_finish(const double *__restrict__ part, int splits, size_t MN, int N, const float *__restrict__ bias, int relu, float *__restrict__ out) {
+// out[i] = float(sum_z part[z][i] (+ bias[i % N] when bias)), optional ReLU; also used to finish single-split GEMMs.  T = double: the
+// unrounded fp64 sum (a data-parallel gradient slice, b200_trainer_grad_rows_dev; no bias / ReLU there)
+template <typename T>
+__global__ void k_finish(const double *__restrict__ part, int splits, size_t MN, int N, const float *__restrict__ bias, int relu, T *__restrict__ out) {
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < MN; i += (size_t)gridDim.x * blockDim.x) {
         double s = 0.0;
         for (int z = 0; z < splits; ++z) s += part[(size_t)z * MN + i];
+        if (sizeof(T) == sizeof(double)) { out[i] = (T)s; continue; }
         float v = (float)s;
         if (bias) v = v + bias[i % N];
         if (relu) v = fmaxf(v, 0.f);
@@ -286,8 +289,9 @@ __global__ void k_finish(const double *__restrict__ part, int splits, size_t MN,
     }
 }
 
-// column sums: out[n] = float(sum_m X[m][n]) in fp64, one CTA per 32 columns, fixed order (rows strided over 8 warps, then a tree)
-__global__ void __launch_bounds__(256) k_colsum(const float *__restrict__ X, int M, int N, float *__restrict__ out) {
+// column sums: out[n] = T(sum_m X[m][n]) in fp64, one CTA per 32 columns, fixed order (rows strided over 8 warps, then a tree)
+template <typename T>
+__global__ void __launch_bounds__(256) k_colsum(const float *__restrict__ X, int M, int N, T *__restrict__ out) {
     __shared__ double s[8][32];
     const int n = blockIdx.x * 32 + (threadIdx.x & 31), w = threadIdx.x >> 5;
     double a = 0.0;
@@ -297,7 +301,7 @@ __global__ void __launch_bounds__(256) k_colsum(const float *__restrict__ X, int
     if (w == 0 && n < N) {
         double t = 0.0;
         for (int i = 0; i < 8; ++i) t += s[i][threadIdx.x & 31];
-        out[n] = (float)t;
+        out[n] = (T)t;
     }
 }
 
@@ -362,12 +366,12 @@ __global__ void k_flat_to_nhwc_relu(const float *__restrict__ dflat, const float
 }
 
 // ------------------------------------------------------------------------------------------------ head: fc_out, sigmoid, bounds, loss
-// One thread per sample: z = h . Wo^T + bo (fp64 accumulate), s = sigmoid(z), pred = s * ub + lb (model_vv.py:48-52), GaussianLL
+// One thread per sample of B (a slice of a batch of Bg rows; Bg = B but in b200_trainer_grad_rows_dev): z = h . Wo^T + bo (fp64 accumulate), s = sigmoid(z), pred = s * ub + lb (model_vv.py:48-52), GaussianLL
 // (model_vv.py:94-101) with the target variance clamped at 0.1 (:140), weight applied when `weighted` (:145-149); and the gradient of
 // mean(w * logl) with respect to z (the two pre-sigmoid outputs).
 __global__ void k_head(const float *__restrict__ h, const float *__restrict__ Wo, const float *__restrict__ bo, const float *__restrict__ ub,
                        const float *__restrict__ lb, const float *__restrict__ value, const float *__restrict__ variance, const float *__restrict__ weight,
-                       int B, int weighted, float *__restrict__ pred, float *__restrict__ lossv, float *__restrict__ dz) {
+                       int B, int Bg, int weighted, float *__restrict__ pred, float *__restrict__ lossv, float *__restrict__ dz) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= B) return;
     double z0 = 0.0, z1 = 0.0;
@@ -386,7 +390,7 @@ __global__ void k_head(const float *__restrict__ h, const float *__restrict__ Wo
     const float w = weighted ? weight[b] : 1.f;
     lossv[b] = w * l;
     if (!dz) return;
-    const float gl = w / (float)B;                                  // d mean(w * logl) / d logl_b
+    const float gl = w / (float)Bg;                                 // d mean(w * logl) / d logl_b over the whole batch of Bg rows
     const float dvp = gl * (1.f / vp - t2 / vp);                    // d/d var_pred
     const float dmp = gl * (-2.f * diff / vp);                      // d/d mean_pred
     dz[2 * b] = dmp * ub[0] * (s0 * (1.f - s0));
@@ -408,6 +412,23 @@ __global__ void __launch_bounds__(256) k_std_mean(const float *__restrict__ x, i
     __syncthreads();
     for (int d = 128; d > 0; d >>= 1) { if (threadIdx.x < d) s[threadIdx.x] += s[threadIdx.x + d]; __syncthreads(); }
     if (threadIdx.x == 0) { out2[0] = mean; out2[1] = sqrt(s[0] / n); }
+}
+// the same two passes, written as the moments {n, mean, M2 = sum (x - mean)^2} of a batch slice (k_loss_combine joins the slices)
+__global__ void __launch_bounds__(256) k_moments(const float *__restrict__ x, int n, double *out3) {
+    __shared__ double s[256];
+    double a = 0.0;
+    for (int i = threadIdx.x; i < n; i += 256) a += (double)x[i];
+    s[threadIdx.x] = a;
+    __syncthreads();
+    for (int d = 128; d > 0; d >>= 1) { if (threadIdx.x < d) s[threadIdx.x] += s[threadIdx.x + d]; __syncthreads(); }
+    const double mean = s[0] / n;
+    __syncthreads();
+    a = 0.0;
+    for (int i = threadIdx.x; i < n; i += 256) { const double d = (double)x[i] - mean; a += d * d; }
+    s[threadIdx.x] = a;
+    __syncthreads();
+    for (int d = 128; d > 0; d >>= 1) { if (threadIdx.x < d) s[threadIdx.x] += s[threadIdx.x + d]; __syncthreads(); }
+    if (threadIdx.x == 0) { out3[0] = (double)n; out3[1] = mean; out3[2] = s[0]; }
 }
 // dh[b][k] = (dz[b][0] * Wo[0][k] + dz[b][1] * Wo[1][k]) masked by h > 0
 __global__ void k_dh(const float *__restrict__ dz, const float *__restrict__ Wo, const float *__restrict__ h, int B, float *__restrict__ dh) {
@@ -459,9 +480,11 @@ __host__ __device__ inline uint64_t splitmix64(uint64_t x) {
     z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
     return z ^ (z >> 31);
 }
-__global__ void k_sample_idx(int32_t *idx, int n, int n_rows, uint64_t seed, uint64_t iteration) {
+// rows [first, first + n) of the batch: idx[i] is global row first + i
+__global__ void k_sample_idx(int32_t *idx, int n, int n_rows, uint64_t seed, uint64_t iteration, int first) {
     const uint64_t base = splitmix64(splitmix64(seed) + iteration);
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) idx[i] = (int32_t)(splitmix64(base + (uint64_t)i) % (uint64_t)n_rows);
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+        idx[i] = (int32_t)(splitmix64(base + (uint64_t)first + (uint64_t)i) % (uint64_t)n_rows);
 }
 __global__ void k_seq_idx(int32_t *idx, int n, int first) {
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) idx[i] = first + i;
@@ -522,13 +545,36 @@ __global__ void k_rows_stats_final(const float *__restrict__ pmax, const double 
     out_max[0] = mv; out_max[1] = mvar; *out_sum = w;
 }
 
+// ------------------------------------------------------------------------------------------------ data-parallel step (b200_trainer_apply_grads_dev)
+// parts: n_parts vectors of `stride` doubles (one per rank, ascending rank), each the unrounded fp64 gradient of a batch slice followed by
+// that slice's loss moments.  g[i] = (float)(((p0 + p1) + p2) + ...): one left-to-right fp64 sum in part order, rounded once.
+__global__ void k_grad_reduce(const double *__restrict__ parts, int n_parts, size_t stride, int n, float *__restrict__ g) {
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        double s = parts[i];
+        for (int r = 1; r < n_parts; ++r) s += parts[(size_t)r * stride + i];
+        g[i] = (float)s;
+    }
+}
+// the slices' {count, mean, M2} joined in part order (Chan et al.'s pairwise update) -> lg[0] = mean, lg[1] = population std
+__global__ void k_loss_combine(const double *__restrict__ mom, int n_parts, size_t stride, double *__restrict__ lg) {
+    double n = mom[0], mean = mom[1], m2 = mom[2];
+    for (int r = 1; r < n_parts; ++r) {
+        const double *q = mom + (size_t)r * stride;
+        const double nb = q[0], d = q[1] - mean, nn = n + nb;
+        mean = mean + d * nb / nn;
+        m2 = m2 + q[2] + d * d * n * nb / nn;
+        n = nn;
+    }
+    lg[0] = mean; lg[1] = sqrt(m2 / n);
+}
+
 inline int nblk(size_t n, int t = 256) { size_t b = (n + t - 1) / t; return (int)(b < 1 ? 1 : (b > 132 * 16 ? 132 * 16 : b)); }
 
 }  // namespace
 
 struct b200_trainer {
     int device = 0, max_batch = 0, kind = B200_TRAIN_FP64;
-    cudaStream_t stream = nullptr;
+    cudaStream_t stream = nullptr; bool own_stream = true;              // own_stream false: the caller's (b200_trainer_set_stream), never destroyed here
     std::vector<void *> allocs;
     float *w = nullptr, *grad = nullptr, *m = nullptr, *v = nullptr;     // [N_ALL] / [N_TRAIN]
     int *d_toff = nullptr; double *d_sumsq = nullptr, *d_lossstat = nullptr;
@@ -542,7 +588,7 @@ struct b200_trainer {
     double *part; size_t part_elems = 0;                                // split-k / chunk partial sums (fp64)
     // b200_trainer_train_rows_dev / _loss_rows_dev / b200_rows_stats_dev
     float *d_coef = nullptr, *d_pmax = nullptr, *d_max2 = nullptr; double *d_psum = nullptr, *d_dsum = nullptr;
-    double *d_log = nullptr; size_t log_cap = 0;                         // [iters][3] step log, grown on demand (not in allocs)
+    double *d_log = nullptr; size_t log_cap = 0;                         // [slots][3] step log, grown on demand (not in allocs)
 };
 
 namespace {
@@ -555,9 +601,10 @@ template <typename T> int talloc(b200_trainer *t, T **p, size_t n) {
     return 0;
 }
 
-// C = op(A) op(B) with fp64 accumulation, optional bias / ReLU; split-k for long reductions (fixed order)
+// C = op(A) op(B) with fp64 accumulation, optional bias / ReLU; split-k for long reductions (fixed order).  out64 (no bias / ReLU): C is not
+// written; out64 gets the fp64 values C would be rounded from (the accumulator itself for one k range, k_finish's sum for several).
 template <bool TA, bool TB>
-int gemm(b200_trainer *t, const float *A, const float *B, float *C, int M, int N, int K, const float *bias, int relu) {
+int gemm(b200_trainer *t, const float *A, const float *B, float *C, int M, int N, int K, const float *bias, int relu, double *out64 = nullptr) {
     int splits = 1;
     const int tiles = ((M + 63) / 64) * ((N + 63) / 64);
     if (K >= 4096 && tiles < 132 * 2) { splits = (132 * 4 + tiles - 1) / tiles; if (splits > (K + 511) / 512) splits = (K + 511) / 512; }
@@ -565,12 +612,14 @@ int gemm(b200_trainer *t, const float *A, const float *B, float *C, int M, int N
     splits = (K + kps - 1) / kps;
     dim3 grid((N + 63) / 64, (M + 63) / 64, splits);
     if (splits == 1) {
-        k_gemm<TA, TB><<<grid, 256, 0, t->stream>>>(A, B, nullptr, M, N, K, kps, C, bias, relu);
+        if (out64) k_gemm<TA, TB><<<grid, 256, 0, t->stream>>>(A, B, out64, M, N, K, kps, nullptr, nullptr, 0);
+        else k_gemm<TA, TB><<<grid, 256, 0, t->stream>>>(A, B, nullptr, M, N, K, kps, C, bias, relu);
         return 0;
     }
     if ((size_t)splits * M * N > t->part_elems) return tfail(B200_ERR_BAD_ARG, "trainer: partial-sum buffer too small");
     k_gemm<TA, TB><<<grid, 256, 0, t->stream>>>(A, B, t->part, M, N, K, kps, nullptr, nullptr, 0);
-    k_finish<<<nblk((size_t)M * N), 256, 0, t->stream>>>(t->part, splits, (size_t)M * N, N, bias, relu, C);
+    if (out64) k_finish<double><<<nblk((size_t)M * N), 256, 0, t->stream>>>(t->part, splits, (size_t)M * N, N, nullptr, 0, out64);
+    else k_finish<float><<<nblk((size_t)M * N), 256, 0, t->stream>>>(t->part, splits, (size_t)M * N, N, bias, relu, C);
     return 0;
 }
 
@@ -584,18 +633,22 @@ inline int tc_k_per_split(int M, int N, int K, int BN) {
     return ((K + splits - 1) / splits + TG_BK - 1) / TG_BK * TG_BK;
 }
 
-// C = op(A) op(B) on tensor cores (k_gemm_tc), optional bias / ReLU; ct: C stored transposed
+// C = op(A) op(B) on tensor cores (k_gemm_tc), optional bias / ReLU; ct: C stored transposed; out64 as in gemm (the fp32 accumulator of one
+// k range is exact in fp64)
 template <bool TA, bool TB, int BN>
-int gemm_tc(b200_trainer *t, const float *A, const float *B, float *C, int M, int N, int K, const float *bias, int relu, int ct = 0) {
+int gemm_tc(b200_trainer *t, const float *A, const float *B, float *C, int M, int N, int K, const float *bias, int relu, int ct = 0,
+            double *out64 = nullptr) {
     const int kps = tc_k_per_split(M, N, K, BN), splits = (K + kps - 1) / kps;
     dim3 grid((N + BN - 1) / BN, (M + TG_BM - 1) / TG_BM, splits);
     if (splits == 1) {
-        k_gemm_tc<TA, TB, BN><<<grid, 128, 0, t->stream>>>(A, B, nullptr, M, N, K, kps, C, bias, relu, ct);
+        if (out64) k_gemm_tc<TA, TB, BN><<<grid, 128, 0, t->stream>>>(A, B, out64, M, N, K, kps, nullptr, nullptr, 0, ct);
+        else k_gemm_tc<TA, TB, BN><<<grid, 128, 0, t->stream>>>(A, B, nullptr, M, N, K, kps, C, bias, relu, ct);
         return 0;
     }
     if ((size_t)splits * M * N > t->part_elems) return tfail(B200_ERR_BAD_ARG, "trainer: partial-sum buffer too small");
     k_gemm_tc<TA, TB, BN><<<grid, 128, 0, t->stream>>>(A, B, t->part, M, N, K, kps, nullptr, nullptr, 0, ct);
-    k_finish<<<nblk((size_t)M * N), 256, 0, t->stream>>>(t->part, splits, (size_t)M * N, ct ? M : N, bias, relu, C);
+    if (out64) k_finish<double><<<nblk((size_t)M * N), 256, 0, t->stream>>>(t->part, splits, (size_t)M * N, ct ? M : N, nullptr, 0, out64);
+    else k_finish<float><<<nblk((size_t)M * N), 256, 0, t->stream>>>(t->part, splits, (size_t)M * N, ct ? M : N, bias, relu, C);
     return 0;
 }
 
@@ -612,15 +665,20 @@ size_t tc_part_elems(int max_batch) {
 
 // C = op(A) op(B) (+ bias, ReLU) in the trainer's kind; BN is the tc kernel's tile width for this shape
 template <bool TA, bool TB, int BN>
-int mm(b200_trainer *t, const float *A, const float *B, float *C, int M, int N, int K, const float *bias, int relu) {
-    if (t->kind == B200_TRAIN_TC) return gemm_tc<TA, TB, BN>(t, A, B, C, M, N, K, bias, relu);
-    return gemm<TA, TB>(t, A, B, C, M, N, K, bias, relu);
+int mm(b200_trainer *t, const float *A, const float *B, float *C, int M, int N, int K, const float *bias, int relu, double *out64 = nullptr) {
+    if (t->kind == B200_TRAIN_TC) return gemm_tc<TA, TB, BN>(t, A, B, C, M, N, K, bias, relu, 0, out64);
+    return gemm<TA, TB>(t, A, B, C, M, N, K, bias, relu, out64);
 }
 // conv weight gradient dW[32][Kc] = dout^T [32 x P] . col [P x Kc]; the tc kind computes dW^T = col^T dout (32 output columns) and stores
 // it transposed
-int conv_wgrad(b200_trainer *t, const float *dout, const float *col, float *dW, int Kc, int P) {
-    if (t->kind == B200_TRAIN_TC) return gemm_tc<true, false, 32>(t, col, dout, dW, Kc, 32, P, nullptr, 0, 1);
-    return gemm<true, false>(t, dout, col, dW, 32, Kc, P, nullptr, 0);
+int conv_wgrad(b200_trainer *t, const float *dout, const float *col, float *dW, int Kc, int P, double *out64) {
+    if (t->kind == B200_TRAIN_TC) return gemm_tc<true, false, 32>(t, col, dout, dW, Kc, 32, P, nullptr, 0, 1, out64);
+    return gemm<true, false>(t, dout, col, dW, 32, Kc, P, nullptr, 0, out64);
+}
+// bias gradients: column sums of X [M][N], rounded to out or (g64) unrounded
+void colsum(b200_trainer *t, const float *X, int M, int N, float *out, double *out64) {
+    if (out64) k_colsum<double><<<(N + 31) / 32, 256, 0, t->stream>>>(X, M, N, out64);
+    else k_colsum<float><<<(N + 31) / 32, 256, 0, t->stream>>>(X, M, N, out);
 }
 
 int forward(b200_trainer *t, int B) {
@@ -649,8 +707,8 @@ int upload_batch(b200_trainer *t, const int8_t *states, const float *value, cons
 
 int loss_and_head(b200_trainer *t, int B, int weighted, bool want_grad, double *loss, double *loss_std) {
     float *W = t->w;
-    k_head<<<(B + 127) / 128, 128, 0, t->stream>>>(t->h, W + O_FOW, W + O_FOB, W + O_UB, W + O_LB, t->value, t->variance, t->weight, B, weighted,
-                                                   t->pred, t->lossv, want_grad ? t->dz : nullptr);
+    k_head<<<(B + 127) / 128, 128, 0, t->stream>>>(t->h, W + O_FOW, W + O_FOB, W + O_UB, W + O_LB, t->value, t->variance, t->weight, B, B,
+                                                   weighted, t->pred, t->lossv, want_grad ? t->dz : nullptr);
     k_std_mean<<<1, 256, 0, t->stream>>>(t->lossv, B, t->d_lossstat);
     double h2[2];
     TCK(cudaMemcpyAsync(h2, t->d_lossstat, 16, cudaMemcpyDeviceToHost, t->stream));
@@ -660,32 +718,69 @@ int loss_and_head(b200_trainer *t, int B, int weighted, bool want_grad, double *
     return 0;
 }
 
-int backward(b200_trainer *t, int B) {
+// the parameter gradient of the B rows in the batch buffers -> t->grad (fp32), or, g64 != nullptr, g64[0 : N_TRAIN] in fp64: the values the
+// fp32 gradient would be rounded from (same kernels, same order; only the last rounding is left out)
+int backward(b200_trainer *t, int B, double *g64 = nullptr) {
     float *W = t->w, *G = t->grad;
+    auto G64 = [&](int off) { return g64 ? g64 + off : nullptr; };
     int rc = 0;
     // fc_out: dWo[j][k] = sum_b dz[b][j] h[b][k]; dbo[j] = sum_b dz[b][j]  (k_gemm in both kinds: 2 x 256 outputs)
-    rc |= gemm<true, false>(t, t->dz, t->h, G + O_FOW, 2, 256, B, nullptr, 0);
-    k_colsum<<<1, 256, 0, t->stream>>>(t->dz, B, 2, G + O_FOB);
+    rc |= gemm<true, false>(t, t->dz, t->h, G + O_FOW, 2, 256, B, nullptr, 0, G64(O_FOW));
+    colsum(t, t->dz, B, 2, G + O_FOB, G64(O_FOB));
     k_dh<<<nblk((size_t)B * 256), 256, 0, t->stream>>>(t->dz, W + O_FOW, t->h, B, t->dh);
     // fc1: dW1[n][k] = sum_b dh[b][n] flat[b][k]; db1; dflat = dh . W1
-    rc |= mm<true, false, 64>(t, t->dh, t->flat, G + O_F1W, 256, 1792, B, nullptr, 0);
-    k_colsum<<<8, 256, 0, t->stream>>>(t->dh, B, 256, G + O_F1B);
+    rc |= mm<true, false, 64>(t, t->dh, t->flat, G + O_F1W, 256, 1792, B, nullptr, 0, G64(O_F1W));
+    colsum(t, t->dh, B, 256, G + O_F1B, G64(O_F1B));
     rc |= mm<false, false, 64>(t, t->dh, W + O_F1W, t->dflat, B, 1792, 256, nullptr, 0);
     k_flat_to_nhwc_relu<<<nblk((size_t)B * 1792), 256, 0, t->stream>>>(t->dflat, t->flat, B, t->dc3);   // ReLU after conv3 (act3)
     // conv3
-    rc |= conv_wgrad(t, t->dc3, t->col3, G + O_C3W, 288, B * 56);
-    k_colsum<<<1, 256, 0, t->stream>>>(t->dc3, B * 56, 32, G + O_C3B);
+    rc |= conv_wgrad(t, t->dc3, t->col3, G + O_C3W, 288, B * 56, G64(O_C3W));
+    colsum(t, t->dc3, B * 56, 32, G + O_C3B, G64(O_C3B));
     rc |= mm<false, false, 64>(t, t->dc3, W + O_C3W, t->dcol3, B * 56, 288, 32, nullptr, 0);
     k_col2im_relu<<<nblk((size_t)B * 96 * 32), 256, 0, t->stream>>>(t->dcol3, t->a2, B, 16, 6, 32, t->da2);
     // conv2
-    rc |= conv_wgrad(t, t->da2, t->col2, G + O_C2W, 288, B * 96);
-    k_colsum<<<1, 256, 0, t->stream>>>(t->da2, B * 96, 32, G + O_C2B);
+    rc |= conv_wgrad(t, t->da2, t->col2, G + O_C2W, 288, B * 96, G64(O_C2W));
+    colsum(t, t->da2, B * 96, 32, G + O_C2B, G64(O_C2B));
     rc |= mm<false, false, 64>(t, t->da2, W + O_C2W, t->dcol2, B * 96, 288, 32, nullptr, 0);
     k_col2im_relu<<<nblk((size_t)B * 144 * 32), 256, 0, t->stream>>>(t->dcol2, t->a1, B, 18, 8, 32, t->da1);
     // conv1 (no input gradient needed)
-    rc |= conv_wgrad(t, t->da1, t->col1, G + O_C1W, 9, B * 144);
-    k_colsum<<<1, 256, 0, t->stream>>>(t->da1, B * 144, 32, G + O_C1B);
+    rc |= conv_wgrad(t, t->da1, t->col1, G + O_C1W, 9, B * 144, G64(O_C1W));
+    colsum(t, t->da1, B * 144, 32, G + O_C1B, G64(O_C1B));
     return rc;
+}
+
+// the step's tail on the device, after t->grad holds the fp32 gradient: gradient norm (lg[2]), clip, Yogi
+int finish_step_dev(b200_trainer *t, double grad_clip, double *lg) {
+    k_sumsq<<<N_TENSORS, 256, 0, t->stream>>>(t->grad, t->d_toff, t->d_sumsq);
+    k_grad_norm<<<1, 1, 0, t->stream>>>(t->d_sumsq, grad_clip, lg + 2, t->d_coef);
+    if (grad_clip > 0.0) k_scale_dev<<<nblk(N_TRAIN), 256, 0, t->stream>>>(t->grad, N_TRAIN, t->d_coef);
+    // Yogi constants from the step counter alone (step_common)
+    const bool first = !t->have_state;
+    if (first) { t->step = 0; t->have_state = true; }
+    t->step += 1;
+    const double bc1 = 1.0 - pow(t->beta1, (double)t->step), bc2 = 1.0 - pow(t->beta2, (double)t->step);
+    YogiConst c;
+    c.beta1 = (float)t->beta1; c.one_minus_beta1 = (float)(1.0 - t->beta1); c.neg_one_minus_beta2 = (float)(-(1.0 - t->beta2));
+    c.wd = (float)t->wd; c.eps = (float)t->eps; c.sqrt_bc2 = (float)sqrt(bc2); c.step_size = (float)(t->lr / bc1); c.first = first ? 1 : 0;
+    k_yogi<<<nblk(N_TRAIN), 256, 0, t->stream>>>(t->w, t->grad, t->m, t->v, N_TRAIN, c);
+    return 0;
+}
+
+// the device step log holds at least `slots` rows of 3; earlier rows are kept
+int ensure_log(b200_trainer *t, size_t slots) {
+    if (slots * 3 <= t->log_cap) return 0;
+    double *nl = nullptr;
+    TCK(cudaStreamSynchronize(t->stream));
+    TCK(cudaMalloc(&nl, slots * 3 * sizeof(double)));
+    if (t->d_log) {
+        const cudaError_t e = cudaMemcpy(nl, t->d_log, t->log_cap * sizeof(double), cudaMemcpyDeviceToDevice);
+        cudaFree(t->d_log);
+        t->d_log = nl; t->log_cap = slots * 3;
+        TCK(e);
+        return 0;
+    }
+    t->d_log = nl; t->log_cap = slots * 3;
+    return 0;
 }
 
 }  // namespace
@@ -697,7 +792,7 @@ extern "C" int b200_trainer_destroy(b200_trainer *t) {
     if (t->stream) cudaStreamSynchronize(t->stream);
     for (void *p : t->allocs) cudaFree(p);
     if (t->d_log) cudaFree(t->d_log);
-    if (t->stream) cudaStreamDestroy(t->stream);
+    if (t->stream && t->own_stream) cudaStreamDestroy(t->stream);
     delete t;
     return B200_OK;
 }
@@ -889,36 +984,21 @@ extern "C" int b200_trainer_train_rows_dev(b200_trainer *t, const void *rows_dev
         return tfail(B200_ERR_BAD_ARG, "trainer: bad argument");
     TCK(cudaSetDevice(t->device));
     if (iters == 0) return B200_OK;
-    if ((size_t)iters * 3 > t->log_cap) {
-        TCK(cudaStreamSynchronize(t->stream));
-        if (t->d_log) { cudaFree(t->d_log); t->d_log = nullptr; t->log_cap = 0; }
-        TCK(cudaMalloc(&t->d_log, (size_t)iters * 3 * sizeof(double)));
-        t->log_cap = (size_t)iters * 3;
-    }
+    int rc = ensure_log(t, (size_t)iters);
+    if (rc) return rc;
     float *W = t->w;
     for (int it = 0; it < iters; ++it) {
         double *lg = t->d_log + (size_t)it * 3;
-        k_sample_idx<<<nblk(batch), 256, 0, t->stream>>>(t->d_idx, batch, n_train_rows, seed, (uint64_t)(first_iter + it));
+        k_sample_idx<<<nblk(batch), 256, 0, t->stream>>>(t->d_idx, batch, n_train_rows, seed, (uint64_t)(first_iter + it), 0);
         k_gather_rows<<<nblk((size_t)batch * 203), 256, 0, t->stream>>>((const uint8_t *)rows_dev, t->d_idx, batch, weight_scale, t->x0, t->value, t->variance, t->weight);
-        int rc = forward(t, batch);
+        rc = forward(t, batch);
         if (rc) return rc;
-        k_head<<<(batch + 127) / 128, 128, 0, t->stream>>>(t->h, W + O_FOW, W + O_FOB, W + O_UB, W + O_LB, t->value, t->variance, t->weight, batch, weighted,
-                                                           t->pred, t->lossv, t->dz);
+        k_head<<<(batch + 127) / 128, 128, 0, t->stream>>>(t->h, W + O_FOW, W + O_FOB, W + O_UB, W + O_LB, t->value, t->variance, t->weight, batch, batch,
+                                                           weighted, t->pred, t->lossv, t->dz);
         k_std_mean<<<1, 256, 0, t->stream>>>(t->lossv, batch, lg);
         rc = backward(t, batch);
         if (rc) return rc;
-        k_sumsq<<<N_TENSORS, 256, 0, t->stream>>>(t->grad, t->d_toff, t->d_sumsq);
-        k_grad_norm<<<1, 1, 0, t->stream>>>(t->d_sumsq, grad_clip, lg + 2, t->d_coef);
-        if (grad_clip > 0.0) k_scale_dev<<<nblk(N_TRAIN), 256, 0, t->stream>>>(t->grad, N_TRAIN, t->d_coef);
-        // Yogi constants from the step counter alone (step_common)
-        const bool first = !t->have_state;
-        if (first) { t->step = 0; t->have_state = true; }
-        t->step += 1;
-        const double bc1 = 1.0 - pow(t->beta1, (double)t->step), bc2 = 1.0 - pow(t->beta2, (double)t->step);
-        YogiConst c;
-        c.beta1 = (float)t->beta1; c.one_minus_beta1 = (float)(1.0 - t->beta1); c.neg_one_minus_beta2 = (float)(-(1.0 - t->beta2));
-        c.wd = (float)t->wd; c.eps = (float)t->eps; c.sqrt_bc2 = (float)sqrt(bc2); c.step_size = (float)(t->lr / bc1); c.first = first ? 1 : 0;
-        k_yogi<<<nblk(N_TRAIN), 256, 0, t->stream>>>(t->w, t->grad, t->m, t->v, N_TRAIN, c);
+        finish_step_dev(t, grad_clip, lg);
     }
     TCK(cudaGetLastError());
     TCK(cudaMemcpyAsync(log_out, t->d_log, (size_t)iters * 3 * sizeof(double), cudaMemcpyDeviceToHost, t->stream));
@@ -959,5 +1039,68 @@ extern "C" int b200_rows_stats_dev(b200_trainer *t, const void *rows_dev, int n,
     TCK(cudaMemcpyAsync(&sum, t->d_dsum, sizeof(double), cudaMemcpyDeviceToHost, t->stream));
     TCK(cudaStreamSynchronize(t->stream));
     *max_value = mx[0]; *max_variance = mx[1]; *visit_sum = sum;
+    return B200_OK;
+}
+
+// All later work of the trainer is issued on `cuda_stream` (nullptr: a private non-blocking stream again); the current stream is drained first.
+// The caller keeps ownership of its stream and keeps it alive.  Lets a collective be ordered on the trainer's stream without a host wait.
+extern "C" int b200_trainer_set_stream(b200_trainer *t, void *cuda_stream) {
+    if (!t) return tfail(B200_ERR_BAD_ARG, "null trainer");
+    TCK(cudaSetDevice(t->device));
+    TCK(cudaStreamSynchronize(t->stream));
+    cudaStream_t ns = (cudaStream_t)cuda_stream;
+    const bool own = ns == nullptr;
+    if (own) TCK(cudaStreamCreateWithFlags(&ns, cudaStreamNonBlocking));
+    if (t->own_stream) cudaStreamDestroy(t->stream);
+    t->stream = ns; t->own_stream = own;
+    return B200_OK;
+}
+
+// Data-parallel step, part 1: rows [lo, hi) of the batch train_rows_dev draws for iteration `iter` (global row numbers in k_sample_idx), forward,
+// head with the gradient scale of the whole batch (every sample's dz is the single-GPU step's), backward into grad_dev[0 : N_TRAIN] unrounded
+// (fp64), then the slice's loss moments {count, mean, M2} of (weight *) logl in grad_dev[N_TRAIN : N_TRAIN + 3].  Asynchronous.
+extern "C" int b200_trainer_grad_rows_dev(b200_trainer *t, const void *rows_dev, int n_train_rows, int batch, int lo, int hi, uint64_t seed, int64_t iter,
+                                          float weight_scale, int weighted, double *grad_dev) {
+    if (!t || !rows_dev || !grad_dev || n_train_rows < 1 || iter < 0 || lo < 0 || lo >= hi || hi > batch || hi - lo > t->max_batch)
+        return tfail(B200_ERR_BAD_ARG, "trainer: bad argument (0 <= lo < hi <= batch, hi - lo <= max_batch)");
+    TCK(cudaSetDevice(t->device));
+    const int n = hi - lo;
+    float *W = t->w;
+    k_sample_idx<<<nblk(n), 256, 0, t->stream>>>(t->d_idx, n, n_train_rows, seed, (uint64_t)iter, lo);
+    k_gather_rows<<<nblk((size_t)n * 203), 256, 0, t->stream>>>((const uint8_t *)rows_dev, t->d_idx, n, weight_scale, t->x0, t->value, t->variance, t->weight);
+    int rc = forward(t, n);
+    if (rc) return rc;
+    k_head<<<(n + 127) / 128, 128, 0, t->stream>>>(t->h, W + O_FOW, W + O_FOB, W + O_UB, W + O_LB, t->value, t->variance, t->weight, n, batch,
+                                                   weighted, t->pred, t->lossv, t->dz);
+    k_moments<<<1, 256, 0, t->stream>>>(t->lossv, n, grad_dev + N_TRAIN);
+    rc = backward(t, n, grad_dev);
+    if (rc) return rc;
+    TCK(cudaGetLastError());
+    return B200_OK;
+}
+
+// Data-parallel step, part 2: g = (float)(p0 + p1 + ... ) in part order (k_grad_reduce), the parts' loss moments joined in part order, then
+// train_rows_dev's gradient norm / clip / Yogi.  {loss, loss_std, grad_norm} go to device log slot `log_slot` (b200_trainer_read_log).
+// Asynchronous.  One part with the whole batch is bit-identical to a train_rows_dev step (its loss up to reassociation).
+extern "C" int b200_trainer_apply_grads_dev(b200_trainer *t, const double *parts_dev, int n_parts, double grad_clip, int log_slot) {
+    if (!t || !parts_dev || n_parts < 1 || log_slot < 0) return tfail(B200_ERR_BAD_ARG, "trainer: bad argument (n_parts >= 1, log_slot >= 0)");
+    TCK(cudaSetDevice(t->device));
+    int rc = ensure_log(t, (size_t)log_slot + 1);
+    if (rc) return rc;
+    double *lg = t->d_log + (size_t)log_slot * 3;
+    const size_t stride = (size_t)N_TRAIN + 3;
+    k_grad_reduce<<<nblk(N_TRAIN), 256, 0, t->stream>>>(parts_dev, n_parts, stride, N_TRAIN, t->grad);
+    k_loss_combine<<<1, 1, 0, t->stream>>>(parts_dev + N_TRAIN, n_parts, stride, lg);
+    finish_step_dev(t, grad_clip, lg);
+    TCK(cudaGetLastError());
+    return B200_OK;
+}
+
+// synchronises the trainer's stream and copies log slots [0, n) ([n][3] doubles) to the host
+extern "C" int b200_trainer_read_log(b200_trainer *t, int n, double *host) {
+    if (!t || n < 0 || (n > 0 && !host) || (size_t)n * 3 > t->log_cap) return tfail(B200_ERR_BAD_ARG, "trainer: bad argument (n <= log slots written)");
+    TCK(cudaSetDevice(t->device));
+    if (n > 0) TCK(cudaMemcpyAsync(host, t->d_log, (size_t)n * 3 * sizeof(double), cudaMemcpyDeviceToHost, t->stream));
+    TCK(cudaStreamSynchronize(t->stream));
     return B200_OK;
 }

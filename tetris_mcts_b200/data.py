@@ -74,8 +74,8 @@ def rows_from_move(recs_before, actions, stats, cycle, episodes, value=None, var
 class DataSaver:
     """util/Data.py:42-132 for batched rows: add_rows(rows) appends, flushing every `chunksize` rows; close() flushes and closes."""
 
-    def __init__(self, save_dir, save_file, cycle, chunksize=500):
-        self.file_name = save_dir + save_file + str(cycle)          # util/Data.py:46
+    def __init__(self, save_dir, save_file, cycle, chunksize=500, suffix=""):
+        self.file_name = save_dir + save_file + str(cycle) + suffix  # util/Data.py:46; suffix: one file per rank of a multi-GPU run
         self.chunksize, self.cycle, self.pending, self.n_rows = chunksize, cycle, [], 0
         self.hdf5 = have_pytables()
         if self.hdf5:

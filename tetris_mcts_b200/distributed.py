@@ -92,3 +92,66 @@ def decode_samples(rows):
     states = a[:, :200].view(np.int8).reshape(-1, 1, 20, 10).copy()
     f = np.ascontiguousarray(a[:, 200:212]).view(np.float32).reshape(-1, 3)
     return states, f[:, 0:1].copy(), f[:, 1:2].copy(), f[:, 2:3].copy()
+
+
+# ---------------------------------------------------------------------------------------------------- data-parallel online training
+# NCCL moves device tensors and is the product path.  gloo (CPU; several ranks sharing one GPU, where NCCL refuses) stages through the host.
+
+def rank_world():
+    """(rank, world) of the initialised process group, (0, 1) without one"""
+    if not dist.is_initialized():
+        return 0, 1
+    return dist.get_rank(), dist.get_world_size()
+
+
+def on_device():
+    """the process group's collectives take device tensors (NCCL), else host tensors (gloo)"""
+    return dist.get_backend() == "nccl"
+
+
+def batch_slice(batch, rank, world):
+    """Rows [lo, hi) of a training batch a rank computes the gradient of: shard_range of the batch.  Every rank needs one row at least."""
+    if batch < world:
+        raise ValueError("a data-parallel batch needs at least one row per rank (batch %d < %d ranks)" % (batch, world))
+    return shard_range(batch, rank, world)
+
+
+def allgather_grads(local, parts, stream):
+    """local: float64 [n] device tensor written on `stream`; parts: float64 [world, n] device tensor <- every rank's `local`, row r = rank r.
+    Ordered on `stream` (NCCL: no host synchronisation; gloo: one, through the host)."""
+    with torch.cuda.stream(stream):
+        if on_device():
+            dist.all_gather_into_tensor(parts.view(-1), local)
+        else:
+            host = local.cpu()                                   # copies on `stream` and waits for it
+            gathered = [torch.empty_like(host) for _ in range(dist.get_world_size())]
+            dist.all_gather(gathered, host)
+            parts.copy_(torch.stack(gathered))
+
+
+def broadcast_rows(buf, n):
+    """buf[:n] (uint8 device rows) of rank 0 -> every rank's buf[:n]; the rows are in place when this returns."""
+    if n <= 0 or not dist.is_initialized():
+        return
+    if on_device():
+        dist.broadcast(buf[:n], src=0)
+    else:
+        host = buf[:n].cpu() if dist.get_rank() == 0 else torch.empty((n,) + tuple(buf.shape[1:]), dtype=buf.dtype)
+        dist.broadcast(host, src=0)
+        if dist.get_rank() != 0:
+            buf[:n].copy_(host)
+    torch.cuda.current_stream(buf.device).synchronize()
+
+
+def broadcast_ints(values):
+    """a list of ints of rank 0 -> every rank"""
+    t = torch.tensor([int(v) for v in values], dtype=torch.int64, device="cuda" if on_device() else "cpu")
+    dist.broadcast(t, src=0)
+    return [int(v) for v in t.tolist()]
+
+
+def gather_objects(obj):
+    """every rank's picklable obj, in rank order"""
+    out = [None] * dist.get_world_size()
+    dist.all_gather_object(out, obj)
+    return out

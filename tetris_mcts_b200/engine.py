@@ -254,6 +254,10 @@ class BatchedEngine:
         r = np.ascontiguousarray(rows, np.uint8).reshape(-1, 212)
         L.check(L.lib().b200_replay_append(self.h, L.ptr(r), len(r)))
 
+    def replay_append_dev(self, dev_ptr, n_rows):
+        """replay_append from a DEVICE buffer of n_rows 212-byte rows (rows all-gathered from other ranks)."""
+        L.check(L.lib().b200_replay_append_dev(self.h, C.c_void_p(int(dev_ptr)), int(n_rows)))
+
     def replay_peek_into(self, dev_ptr, n_rows):
         L.check(L.lib().b200_replay_peek_dev(self.h, C.c_void_p(int(dev_ptr)), int(n_rows)))
 

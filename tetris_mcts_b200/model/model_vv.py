@@ -3,6 +3,7 @@ for the calls the agents make: Model_VV().load(); .training(False); .inference(b
 The forward pass runs on the GPU through the C-ABI (b200_valuenet_forward); weights are the reference's state_dict
 tensors (head.conv1.weight ... head.fc_out.bias, out_ubound, out_lbound) concatenated in that order."""
 import os
+import sys
 from collections import OrderedDict
 from sys import stderr
 
@@ -127,6 +128,7 @@ class Model_VV:
         self._eng = BatchedEngine(1, max_nodes=64, eval_kind=kwargs.get("eval_kind", "net"), device=device)
         self._eng.load_weights(self.weights)
         self._trainer = None
+        self._dp = None                                            # data-parallel buffers: (stream, own gradient slice, every rank's)
         self._opt_state = None                                     # (exp_avg, exp_avg_sq, step) loaded from a checkpoint before the trainer exists
         self._training = False
 
@@ -265,7 +267,13 @@ class Model_VV:
         mean come from b200_rows_stats_dev, batches are drawn on the device (Trainer.train_rows_dev, seeded by `seed`; the reference's draw is
         np.random.choice), a validation interval runs with one synchronisation, and the validation loss is computed chunk by chunk on the device
         and combined as compute_loss combines it.  Same split (the last 10 % of the rows, no shuffle), early stopping, checkpoint and log lines
-        as train_data.  Returns False without training when the split leaves no validation rows (the reference fails on d[:-0])."""
+        as train_data.  Returns False without training when the split leaves no validation rows (the reference fails on d[:-0]).
+
+        Under a torch.distributed process group of world > 1 (play_batched under torchrun) every rank holds the same rows and trains data-
+        parallel: each step, rank r computes the gradient of rows shard_range(batch_size, r, world) of the batch, the fp64 gradients are all-
+        gathered and every rank adds them in rank order and applies the same update (Trainer.apply_grads_dev), so all ranks keep bit-identical
+        weights.  Everything else (row statistics, validation, early stopping) runs redundantly on every rank; rank 0 alone prints and writes
+        the checkpoint, the other ranks keep the best weights and optimiser state in memory."""
         bad = {k: v for k, v in options.items() if k not in _TRAIN_ROWS_FIXED or v != _TRAIN_ROWS_FIXED[k]}
         if bad:
             raise ValueError("train_rows implements train_data with %s only; got %s" % (_TRAIN_ROWS_FIXED, bad))
@@ -274,22 +282,33 @@ class Model_VV:
         if validation_size == 0:
             print("Not enough training data ({} < {}), collecting more data.".format(n_rows, int(np.ceil(1 / _TRAIN_ROWS_FIXED["validation_fraction"]))), **perr)
             return False
+        from .. import distributed as D
+        rank, world = D.rank_world()
+        if world > 1:
+            lo, hi = D.batch_slice(int(batch_size), rank, world)
+        def say(msg, **where):                                    # rank 0 alone prints
+            if rank == 0:
+                print(msg, **(where or perr))
+        best = None
         t = self._trainer_obj()
         max_value, max_variance, visit_sum = t.rows_stats(rows_dev_ptr, n_rows)
         t.set_out_ubound(max_value, max_variance)                                             # model_vv.py:228-229
         scale = float(n_rows / visit_sum)                                                     # weights / weights.mean(), model/model.py:186-187
         n_train = n_rows - validation_size
-        print("Training data size: {}    Validation data size: {}".format(n_train, validation_size), **perr)
+        say("Training data size: {}    Validation data size: {}".format(n_train, validation_size))
         patience, threshold = _TRAIN_ROWS_FIXED["early_stopping_patience"], _TRAIN_ROWS_FIXED["early_stopping_threshold"]
         fails, loss_val_min = 0, float("inf")
         self.training(True)
         for it0 in range(0, int(max_iters), int(iters_per_val)):
             k = min(int(iters_per_val), int(max_iters) - it0)
-            log = t.train_rows_dev(rows_dev_ptr, n_train, batch_size, k, seed, it0, scale, weighted=True)
+            if world > 1:
+                log = self._train_interval_dp(rows_dev_ptr, n_train, batch_size, lo, hi, k, seed, it0, scale)
+            else:
+                log = t.train_rows_dev(rows_dev_ptr, n_train, batch_size, k, seed, it0, scale, weighted=True)
             loss_avg = g_norm_avg = 0
             for loss, _std, g_norm in log:
                 if g_norm > 1e3:
-                    print("Large gradient ({}) detected".format(g_norm), **perr)             # Model.train's g_norm_warn (model/model.py:103-105)
+                    say("Large gradient ({}) detected".format(g_norm))             # Model.train's g_norm_warn (model/model.py:103-105)
                 loss_avg += loss
                 g_norm_avg += g_norm
             if k < iters_per_val:
@@ -301,18 +320,46 @@ class Model_VV:
                 fails = 0
                 if loss_val_mean < loss_val_min:
                     suffix = "*"
-                    self.save(checkpoint, verbose=False)
+                    if rank == 0:
+                        self.save(checkpoint, verbose=False)
+                    if world > 1:
+                        best = (t.weights(), t.state())
                     loss_val_min = loss_val_mean
             else:
                 fails += 1
                 if fails >= patience:
                     break
-            print("Iteration:{:7d}  training loss:{:6.4f}  validation loss:{:6.4f}±{:6.4f}  gradient norm:{:6.3f}    {}"
-                  .format(it0 + k, loss_avg / iters_per_val, loss_val_mean, loss_val_std, g_norm_avg / iters_per_val, suffix), **perr)
-        self.load(checkpoint)                                                                 # model/model.py:240-241: back to the best model
+            say("Iteration:{:7d}  training loss:{:6.4f}  validation loss:{:6.4f}±{:6.4f}  gradient norm:{:6.3f}    {}"
+                .format(it0 + k, loss_avg / iters_per_val, loss_val_mean, loss_val_std, g_norm_avg / iters_per_val, suffix))
+        if world > 1:                                                                         # back to the best model, from memory on every rank
+            say("Loading model...", file=sys.stdout, flush=True)
+            if best is not None:
+                t.set_weights(best[0])
+                t.set_state(*best[1])
+        else:
+            self.load(checkpoint)                                                             # model/model.py:240-241: back to the best model
         self._publish()
         self.training(False)
         return True
+
+    def _train_interval_dp(self, rows_dev_ptr, n_train, batch, lo, hi, iters, seed, first_iter, weight_scale):
+        """`iters` data-parallel steps (rows [lo, hi) of each batch on this rank) -> the [iters, 3] log train_rows_dev returns"""
+        import torch
+        from .. import distributed as D
+        from .trainer import GRAD_VEC
+        t = self._trainer_obj()
+        if self._dp is None:
+            dev = torch.device("cuda", int(self.device))
+            stream = torch.cuda.Stream(device=dev)
+            t.set_stream(stream.cuda_stream)                     # the exchange is ordered on the trainer's own stream
+            self._dp = (stream, torch.empty(GRAD_VEC, dtype=torch.float64, device=dev),
+                        torch.empty((D.rank_world()[1], GRAD_VEC), dtype=torch.float64, device=dev))
+        stream, local, parts = self._dp
+        for it in range(int(iters)):
+            t.grad_rows_dev(rows_dev_ptr, n_train, batch, lo, hi, seed, first_iter + it, weight_scale, local.data_ptr())
+            D.allgather_grads(local, parts, stream)
+            t.apply_grads_dev(parts.data_ptr(), parts.shape[0], 0.0, it)
+        return t.read_log(iters)
 
     def _loss_rows(self, rows_dev_ptr, first, end, weight_scale, chunksize=1024):
         """compute_loss(weighted=True) on device rows [first, end)"""

@@ -11,6 +11,7 @@ import numpy as np
 from .. import _lib as L
 
 N_TRAIN = 478338            # trainable floats (state_dict order without out_ubound / out_lbound)
+GRAD_VEC = N_TRAIN + 3      # doubles of one data-parallel gradient slice: the fp64 gradient, then the slice's loss {count, mean, M2}
 KINDS = {"fp64": 0, "tc": 1}  # B200_TRAIN_FP64, B200_TRAIN_TC
 P = C.c_void_p
 _sig_done = False
@@ -37,6 +38,10 @@ def _lib():
         lib.b200_trainer_train_rows_dev.argtypes = [P, P, C.c_int, C.c_int, C.c_int, C.c_uint64, C.c_int64, C.c_float, C.c_int, C.c_double, P]
         lib.b200_trainer_loss_rows_dev.argtypes = [P, P, C.c_int, C.c_int, C.c_float, C.c_int, P, P, P]
         lib.b200_rows_stats_dev.argtypes = [P, P, C.c_int, P, P, P]
+        lib.b200_trainer_set_stream.argtypes = [P, P]
+        lib.b200_trainer_grad_rows_dev.argtypes = [P, P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_uint64, C.c_int64, C.c_float, C.c_int, P]
+        lib.b200_trainer_apply_grads_dev.argtypes = [P, P, C.c_int, C.c_double, C.c_int]
+        lib.b200_trainer_read_log.argtypes = [P, C.c_int, P]
         _sig_done = True
     return lib
 
@@ -163,6 +168,28 @@ class Trainer:
         log = np.zeros((int(iters), 3), np.float64)
         _check(_lib().b200_trainer_train_rows_dev(self.h, P(int(rows_dev_ptr)), int(n_train_rows), int(batch), int(iters), int(seed) & 0xFFFFFFFFFFFFFFFF,
                                                   int(first_iter), float(weight_scale), int(bool(weighted)), float(grad_clip), L.ptr(log)))
+        return log
+
+    def set_stream(self, stream_ptr):
+        """All later work runs on the CUDA stream `stream_ptr` (e.g. torch.cuda.Stream().cuda_stream; 0 / None: a private stream again)."""
+        _check(_lib().b200_trainer_set_stream(self.h, P(int(stream_ptr)) if stream_ptr else None))
+
+    def grad_rows_dev(self, rows_dev_ptr, n_train_rows, batch, lo, hi, seed, iteration, weight_scale, grad_dev_ptr, weighted=True):
+        """Rows [lo, hi) of train_rows_dev's batch of iteration `iteration`: their fp64 gradient (scaled by 1 / batch) and loss moments ->
+        GRAD_VEC doubles at grad_dev_ptr (device).  Asynchronous on the trainer's stream."""
+        _check(_lib().b200_trainer_grad_rows_dev(self.h, P(int(rows_dev_ptr)), int(n_train_rows), int(batch), int(lo), int(hi),
+                                                 int(seed) & 0xFFFFFFFFFFFFFFFF, int(iteration), float(weight_scale), int(bool(weighted)),
+                                                 P(int(grad_dev_ptr))))
+
+    def apply_grads_dev(self, parts_dev_ptr, n_parts, grad_clip=0.0, log_slot=0):
+        """Sum n_parts GRAD_VEC slices (device, rank order) left to right in fp64, round once, clip and take the Yogi step; the step's
+        (loss, loss_std, grad_norm) go to log slot `log_slot` (read_log).  Asynchronous."""
+        _check(_lib().b200_trainer_apply_grads_dev(self.h, P(int(parts_dev_ptr)), int(n_parts), float(grad_clip), int(log_slot)))
+
+    def read_log(self, n):
+        """log slots [0, n) -> float64 [n, 3] = (loss, loss_std, grad_norm); synchronises the trainer's stream"""
+        log = np.zeros((int(n), 3), np.float64)
+        _check(_lib().b200_trainer_read_log(self.h, int(n), L.ptr(log)))
         return log
 
     def loss_rows_dev(self, rows_dev_ptr, first, n, weight_scale, weighted=True):
