@@ -9,9 +9,10 @@
 //   k_tc_conv  persistent CTAs of TCC_WGS warpgroups; each warpgroup carries its own boards through the whole stack:
 //              obs key -> im2col (exact fp16) -> conv1 as one K=16 wgmma per 64-row tile -> epilogue (bias, ReLU, split) -> smem
 //              conv2 / conv3 as shift-GEMMs: activations live in shared memory channel-chunk-major
-//              ([8-channel chunk][pixel row][16 B]) on an 8-wide pixel grid, so the A operand of filter row dy is the SAME
-//              array started dy*8 rows later — a no-swizzle K-major operand layout with SBO = 128 B, LBO = rows*16 B; the
-//              three horizontal taps are stacked along N (N = 96) and summed by the epilogue with two lane shuffles.
+//              ([8-channel chunk][pixel row][16 B]), so the A operand of a filter tap is the SAME array started a few rows
+//              later — a no-swizzle K-major operand layout with SBO = 128 B, LBO = rows*16 B.  conv2 runs on an 8-wide
+//              row-major grid with the three horizontal taps stacked along N (N = 96) and summed by two lane shuffles; conv3
+//              runs on a column-major grid of column height 16, where its 56 outputs fit one 64-row tile (see below).
 //              wgmma.mma_async (M=64 pixels, K=16) from shared-memory descriptors, accumulators in registers; the epilogues
 //              apply bias+ReLU, re-split (fp16 x2) and write the next layer's operand (or act3 to HBM in the FC kernel's tile layout).
 //   k_tc_fc    [R,1792] x [1792,256]: 128-row tiles, operands streamed by cp.async.bulk (1-D TMA) into an mbarrier ring —
@@ -31,6 +32,16 @@ constexpr float TC_SCALE_A = 16.f, TC_SCALE_W = 64.f, TC_UNSCALE = 1.f / 1024.f;
 // D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, fp16 operands from shared memory (both K-major), fp32 accumulators: thread t of the
 // warpgroup holds rows 16*(t/32) + (t%32)/4 (+8) and columns 8j + 2*(t%4) (+1) in d[4j + {0,1}] (row) / d[4j + {2,3}] (row + 8).
 // accumulate == 0 overwrites D.
+__device__ __forceinline__ void wgmma_n32(float (&d)[16], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {"
+        "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15"
+        "}, %16, %17, p, 1, 1, 0, 0;\n}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
 __device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
     asm volatile(
         "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
@@ -119,21 +130,36 @@ __device__ __forceinline__ void split2(float x0, float x1, uint32_t &hi, uint32_
 }
 
 // ---------------------------------------------------------------------------------------------------- conv kernel
-// The three horizontal taps (dx) of a 3x3 filter are stacked along N, so a layer is a few wide MMAs instead of many narrow ones:
+// In conv2 the three horizontal taps (dx) of a 3x3 filter are stacked along N, so the layer is a few wide MMAs instead of many narrow ones:
 //   D'[p][dx*32 + cout] = sum_{dy, cin} act[p + dy*8][cin] * W[dy][dx][cin][cout]          (A operand shifted by dy*8 rows only)
 //   out[p][cout]        = D'[p][0*32+cout] + D'[p+1][1*32+cout] + D'[p+2][2*32+cout]        (epilogue: two lane shuffles)
-// All three layers live on an 8-wide pixel grid (p = y*8 + x).  In the wgmma accumulator layout pixel x of a row sits in lanes 4x..4x+3,
-// so p+1 / p+2 are 4 / 8 lanes further in the same register, and p+dx never leaves the row.  A layer is 18 MMAs per 64-row tile
-// (3 dy x 2 channel halves x 3 split products, N = 96); conv1 (K = 9 taps, exact {-1,0,1} inputs) runs on the tensor core too,
-// from an im2col operand the warpgroup builds.
+// conv1 and conv2 live on an 8-wide pixel grid (p = y*8 + x).  In the wgmma accumulator layout pixel x of a row sits in lanes 4x..4x+3,
+// so p+1 / p+2 are 4 / 8 lanes further in the same register, and p+dx never leaves the row.  conv2 is 18 MMAs per 64-row tile
+// (3 dy x 2 channel halves x 3 split products, N = 96), two tiles; conv1 (K = 9 taps, exact {-1,0,1} inputs) runs on the tensor core
+// too, from an im2col operand the warpgroup builds.
+// conv3 has only 14x4 valid outputs, which the 8-wide grid spreads over two tiles.  Its input (act2) and output use a column-major grid
+// of column height 16 instead (q = x*16 + y): every valid output has p <= 61, one 64-row tile, and tap (dy, dx) reads row p + 16 dx + dy.
+// The three dx taps get an accumulator each (N = 32), so no shuffles are needed:
+//   D_dx[p][cout] = sum_{dy, cin} act2[p + 16 dx + dy][cin] * W[dy][dx][cin][cout],    out[p] = (D_2 + D_1) + D_0
+// Each D_dx receives exactly the MMA sequence (dy, half, split product) that the N = 96 form issued into its 32 columns, from the same
+// operands, so act3 is the same bits as with two N = 96 tiles, for 54 n32 MMAs per board instead of 36 n96.
 constexpr int TCC_WGS = 4;                  // warpgroups per CTA; each evaluates its own boards from key to act3
 constexpr int TCC_THREADS = TCC_WGS * 128;
-constexpr int TCC_R = 144;                  // activation rows per board: 18x8 grid (act1) / 16x8 grid + the dy shifts (act2)
-constexpr int TCC_WBLOCK = 2 * 2 * 96 * 16;  // one (dy, channel half) block: [weight split 2][chunk 2][n = dx*32 + cout][16 B]
+constexpr int TCC_R = 144;                  // act1 rows per board: the 18x8 grid of conv1's outputs
+constexpr int TCC_WBLOCK = 2 * 2 * 96 * 16;  // conv2: one (dy, channel half) block: [weight split 2][chunk 2][n = dx*32 + cout][16 B]
 constexpr int TCC_WBYTES = 6 * TCC_WBLOCK;   // one conv layer = 36864 B
+constexpr int TCC_W3BLOCK = 2 * 32 * 16;     // conv3: one (dx, dy, channel half, weight split) block: [chunk 2][cout 32][16 B]
+static_assert(36 * TCC_W3BLOCK == TCC_WBYTES, "conv3 weight layout");
 constexpr int TCC_W1BYTES = 2 * 64 * 16;     // conv1: [chunk 2][n = split*32 + cout][16 B], k = tap (9 of 16 used)
 constexpr int TCC_RUN = 4;                  // consecutive requests handed to a warpgroup at a time
-constexpr int TCC_ASLOT = 2 * 4 * TCC_R * 16;    // operand buffer of one board: act1 / act2 [split][chunk 4][144 rows][16 B]
+constexpr int TCC_ASLOT = 2 * 4 * TCC_R * 16;    // act1 of one board: [split][chunk 4][144 rows][16 B]
+// act2 of one board: [split][chunk 4][98 rows][16 B], row q = x*16 + y (x < 6, y < 16) plus rows 96..97, which conv3's dy shift reads
+// for discarded outputs only (zeroed once).  98 = 2 (mod 8) puts the four chunks 8 banks apart, and the split stride of 4*98*16 + 16 B
+// puts the second term 4 banks from the first: the eight words a lane stores per pixel fall on eight disjoint 4-bank groups.
+constexpr int TCC_R2 = 98;
+constexpr int TCC_A2SPLIT = 4 * TCC_R2 * 16 + 16;
+constexpr int TCC_A2SLOT = 2 * TCC_A2SPLIT;
+static_assert((TCC_R2 * 4) % 32 == 8 && (TCC_A2SPLIT / 4) % 32 == 4, "act2 bank layout");
 constexpr int TCC_IMROWS = 192;             // im2col rows per board: 144 used, three 64-row tiles
 constexpr int TCC_IMSLOT = 2 * TCC_IMROWS * 16;  // [chunk 2][192 rows][16 B] fp16
 constexpr int TCC_OFF_W2 = 0;
@@ -141,7 +167,8 @@ constexpr int TCC_OFF_W3 = TCC_OFF_W2 + TCC_WBYTES;
 constexpr int TCC_OFF_W1 = TCC_OFF_W3 + TCC_WBYTES;
 constexpr int TCC_OFF_A1 = TCC_OFF_W1 + TCC_W1BYTES;
 constexpr int TCC_OFF_IM = TCC_OFF_A1 + TCC_WGS * TCC_ASLOT;
-constexpr int TCC_OFF_BIAS = TCC_OFF_IM + TCC_WGS * TCC_IMSLOT;    // 96 floats, pre-scaled by TC_SCALE_A
+constexpr int TCC_OFF_A2 = TCC_OFF_IM + TCC_WGS * TCC_IMSLOT;
+constexpr int TCC_OFF_BIAS = TCC_OFF_A2 + TCC_WGS * TCC_A2SLOT;    // 96 floats, pre-scaled by TC_SCALE_A
 constexpr int TCC_OFF_KEY = TCC_OFF_BIAS + 96 * 4;                  // TCC_WGS x 32 words: row table (20 rows: settled | piece << 16)
 constexpr int TCC_SMEM = TCC_OFF_KEY + TCC_WGS * 32 * 4;
 constexpr int ACT3_KCHUNKS = 224;           // 1792 / 8
@@ -158,8 +185,8 @@ __device__ __forceinline__ size_t act3_off(int split, int n_tiles, int ridx, int
     return ((((size_t)split * n_tiles + (ridx >> 7)) * ACT3_KCHUNKS + kchunk) * 128 + (ridx & 127)) * 16;
 }
 
-// One 3x3 layer on one 64-row tile = 18 wgmma of N = 96: for each (dy, channel half): a1*W1, a1*W2, a2*W1 into the same 96 columns.
-__device__ __forceinline__ void issue_conv_layer(float (&d)[48], uint32_t a_addr, uint32_t w_addr) {
+// conv2 on one 64-row tile = 18 wgmma of N = 96: for each (dy, channel half): a1*W1, a1*W2, a2*W1 into the same 96 columns.
+__device__ __forceinline__ void issue_conv2(float (&d)[48], uint32_t a_addr, uint32_t w_addr) {
     const uint64_t a0 = gmma_desc(a_addr, TCC_R * 16, 128), b0 = gmma_desc(w_addr, 96 * 16, 128);
 #pragma unroll
     for (int dy = 0; dy < 3; ++dy) {
@@ -170,6 +197,26 @@ __device__ __forceinline__ void issue_conv_layer(float (&d)[48], uint32_t a_addr
             wgmma_n96(d, a0 + a_hi, b0 + b_hi, (dy | h) ? 1u : 0u);
             wgmma_n96(d, a0 + a_hi, b0 + b_lo, 1u);
             wgmma_n96(d, a0 + a_lo, b0 + b_hi, 1u);
+        }
+    }
+}
+
+// conv3 on its one 64-row tile = 3 accumulators x 18 wgmma of N = 32: for each (dy, channel half) and each dx, a1*W1, a1*W2, a2*W1.
+// The A operand of tap (dy, dx) starts 16 dx + dy rows (16-byte units) into act2.
+__device__ __forceinline__ void issue_conv3(float (&d)[3][16], uint32_t a_addr, uint32_t w_addr) {
+    const uint64_t a0 = gmma_desc(a_addr, TCC_R2 * 16, 128), b0 = gmma_desc(w_addr, 32 * 16, 128);
+#pragma unroll
+    for (int dy = 0; dy < 3; ++dy) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+#pragma unroll
+            for (int dx = 0; dx < 3; ++dx) {
+                const uint32_t a_hi = 2 * h * TCC_R2 + 16 * dx + dy, a_lo = a_hi + TCC_A2SPLIT / 16;    // 16-byte units
+                const uint32_t b_hi = ((dx * 3 + dy) * 2 + h) * 2 * (TCC_W3BLOCK / 16), b_lo = b_hi + TCC_W3BLOCK / 16;
+                wgmma_n32(d[dx], a0 + a_hi, b0 + b_hi, (dy | h) ? 1u : 0u);
+                wgmma_n32(d[dx], a0 + a_hi, b0 + b_lo, 1u);
+                wgmma_n32(d[dx], a0 + a_lo, b0 + b_hi, 1u);
+            }
         }
     }
 }
@@ -199,7 +246,7 @@ k_tc_conv(NetWeights W, TcWeights TW, const uint2 *req, const int32_t *n_req_ptr
     extern __shared__ __align__(128) uint8_t smem[];
     float *sB = reinterpret_cast<float *>(smem + TCC_OFF_BIAS);
     const int t = threadIdx.x, wg = t >> 7, wt = t & 127, w = wt >> 5, lane = t & 31;
-    // ---- one-time setup: weights into smem, zeroed operands (the im2col rows past 144 stay zero)
+    // ---- one-time setup: weights into smem, zeroed operands (the im2col rows past 144 and act2 rows 96..97 stay zero)
     for (int i = t; i < TCC_WBYTES / 16; i += TCC_THREADS) {
         reinterpret_cast<uint4 *>(smem + TCC_OFF_W2)[i] = reinterpret_cast<const uint4 *>(TW.wc2)[i];
         reinterpret_cast<uint4 *>(smem + TCC_OFF_W3)[i] = reinterpret_cast<const uint4 *>(TW.wc3)[i];
@@ -219,13 +266,13 @@ k_tc_conv(NetWeights W, TcWeights TW, const uint2 *req, const int32_t *n_req_ptr
     int n_local = 0;
     for (int run = wid; run < n_runs; run += n_workers) n_local += min(TCC_RUN, n_req - run * TCC_RUN);
     auto board_of = [&](int i) -> int { return first + ((i / TCC_RUN) * n_workers + wid) * TCC_RUN + (i % TCC_RUN); };
-    uint8_t *act = smem + TCC_OFF_A1 + wg * TCC_ASLOT, *im = smem + TCC_OFF_IM + wg * TCC_IMSLOT;
+    uint8_t *act = smem + TCC_OFF_A1 + wg * TCC_ASLOT, *act2 = smem + TCC_OFF_A2 + wg * TCC_A2SLOT, *im = smem + TCC_OFF_IM + wg * TCC_IMSLOT;
     uint32_t *sKey = reinterpret_cast<uint32_t *>(smem + TCC_OFF_KEY) + wg * 32;
-    const uint32_t s_act = smem_u32(act), s_im = smem_u32(im);
+    const uint32_t s_act = smem_u32(act), s_act2 = smem_u32(act2), s_im = smem_u32(im);
     const uint32_t s_w1 = smem_u32(smem + TCC_OFF_W1), s_w2 = smem_u32(smem + TCC_OFF_W2), s_w3 = smem_u32(smem + TCC_OFF_W3);
     const int qd = lane & 3, rl = lane >> 2;             // accumulator rows 16w + rl (+8), columns 8j + 2qd (+1)
     constexpr float K23 = TC_UNSCALE * TC_SCALE_A, K1 = TC_SCALE_A / TC_SCALE_W;
-    constexpr int SPLIT = 4 * TCC_R * 16;                // act1 / act2: second fp16 term
+    constexpr int SPLIT = 4 * TCC_R * 16;                // act1: second fp16 term
     const bool do_prof = prof && blockIdx.x == 0 && t == 0;
     long long pacc[4] = {0, 0, 0, 0}, ptick = clock64();
     auto prof_t = [&](int k) { if (do_prof) { const long long n = clock64(); pacc[k] += n - ptick; ptick = n; } };
@@ -287,53 +334,91 @@ k_tc_conv(NetWeights W, TcWeights TW, const uint2 *req, const int32_t *n_req_ptr
         fence_async_smem();
         wg_sync(wg);
         prof_t(1);
-        // ---- conv2 (model_vv.py:34) on act1 (18x8 grid) and conv3 (:36) on act2 (16x8 grid).  act2 overwrites act1 in place: the epilogue
-        // of tile 0 writes rows 0..63, tile 1 reads rows 64..143 only.  Rows of act2 that no valid conv3 output reads keep act1 values.
+        // ---- conv2 (model_vv.py:34) on act1 (18x8 grid) -> act2 (column-major, its own buffer: tile 0's outputs reach row 87 of act2
+        // while tile 1 still reads act1 rows 64..143)
 #pragma unroll 1
-        for (int layer = 0; layer < 2; ++layer) {
-            const float *bias = sB + 32 * (layer + 1);
-#pragma unroll 1
-            for (int mt = 0; mt < 2; ++mt) {
-                float d[48];
+        for (int mt = 0; mt < 2; ++mt) {
+            float d[48];
 #pragma unroll
-                for (int k = 0; k < 48; ++k) d[k] = 0.f;
-                wgmma_fence();
-                issue_conv_layer(d, s_act + mt * 1024, layer ? s_w3 : s_w2);
-                wgmma_commit();
-                wgmma_wait<0>();
-                fence_regs(d);
+            for (int k = 0; k < 48; ++k) d[k] = 0.f;
+            wgmma_fence();
+            issue_conv2(d, s_act + mt * 1024, s_w2);
+            wgmma_commit();
+            wgmma_wait<0>();
+            fence_regs(d);
 #pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const int y = mt * 8 + 2 * w + h, x = rl;
+            for (int h = 0; h < 2; ++h) {
+                const int y = mt * 8 + 2 * w + h, x = rl;
+                uint32_t v[8];                                   // v[j + 4s]: channels 8j + 2qd (+1), fp16 term s
 #pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        float o[2];
+                for (int j = 0; j < 4; ++j) {
+                    float o[2];
 #pragma unroll
-                        for (int e = 0; e < 2; ++e) {            // out[p] = D'[p][dx=0] + D'[p+1][dx=1] + D'[p+2][dx=2]
-                            const int k = 4 * j + 2 * h + e;
-                            const float s1 = __shfl_down_sync(0xffffffffu, d[16 + k], 4), s2 = __shfl_down_sync(0xffffffffu, d[32 + k], 8);
-                            o[e] = fmaxf(fmaf((s2 + s1) + d[k], K23, bias[8 * j + 2 * qd + e]), 0.f);
-                        }
-                        uint32_t hi, lo;
-                        split2(o[0], o[1], hi, lo);
-                        if (layer == 0) {
-                            if (x < 6) {                         // act2: 16x6 valid pixels on the 8-wide grid
-                                uint8_t *dst = act + (j * TCC_R + y * 8 + x) * 16 + qd * 4;
-                                *reinterpret_cast<uint32_t *>(dst) = hi;
-                                *reinterpret_cast<uint32_t *>(dst + SPLIT) = lo;
-                            }
-                        } else if (y < 14 && x < 4) {            // act3 -> HBM
-                            const int kc = (y * 4 + x) * 4 + j;
-                            *reinterpret_cast<uint32_t *>(act3 + act3_off(0, n_tiles, ridx, kc) + qd * 4) = hi;
-                            *reinterpret_cast<uint32_t *>(act3 + act3_off(1, n_tiles, ridx, kc) + qd * 4) = lo;
-                        }
+                    for (int e = 0; e < 2; ++e) {                // out[p] = D'[p][dx=0] + D'[p+1][dx=1] + D'[p+2][dx=2]
+                        const int k = 4 * j + 2 * h + e;
+                        const float s1 = __shfl_down_sync(0xffffffffu, d[16 + k], 4), s2 = __shfl_down_sync(0xffffffffu, d[32 + k], 8);
+                        o[e] = fmaxf(fmaf((s2 + s1) + d[k], K23, sB[32 + 8 * j + 2 * qd + e]), 0.f);
+                    }
+                    split2(o[0], o[1], v[j], v[4 + j]);
+                }
+                // Store k of lane (x, qd) writes word i = (k + x) & 7 at split i/4, chunk i%4, row x*16 + y: in 4-byte banks that is
+                // (8 (i%4) + 4 (i/4) + 4y + qd) mod 32 (row x*16 is 256 B, a multiple of the 128-B bank line), so the six pixels x < 6
+                // hit six disjoint 4-bank groups: one wavefront per store instead of a 6-way conflict.  The words are rotated into place
+                // by x with selects (a dynamically indexed array would live in local memory).
+#pragma unroll
+                for (int b = 1; b < 8; b <<= 1) {
+                    uint32_t r[8];
+#pragma unroll
+                    for (int k = 0; k < 8; ++k) r[k] = (x & b) ? v[(k + b) & 7] : v[k];
+#pragma unroll
+                    for (int k = 0; k < 8; ++k) v[k] = r[k];
+                }
+                if (x < 6) {                                     // act2: 16x6 valid pixels
+#pragma unroll
+                    for (int k = 0; k < 8; ++k) {
+                        const int i = (k + x) & 7;
+                        *reinterpret_cast<uint32_t *>(act2 + (i >> 2) * TCC_A2SPLIT + ((i & 3) * TCC_R2 + x * 16 + y) * 16 + qd * 4) = v[k];
                     }
                 }
             }
-            fence_async_smem();
-            wg_sync(wg);
-            prof_t(2 + layer);
         }
+        fence_async_smem();
+        wg_sync(wg);
+        prof_t(2);
+        // ---- conv3 (:36) on act2: one tile, warp w holds column x = w, lane rows y = 8h + rl; act3 -> HBM
+        {
+            float d[3][16];
+#pragma unroll
+            for (int k = 0; k < 16; ++k) d[0][k] = d[1][k] = d[2][k] = 0.f;
+            wgmma_fence();
+            issue_conv3(d, s_act2, s_w3);
+            wgmma_commit();
+            wgmma_wait<0>();
+            fence_regs(d[0]); fence_regs(d[1]); fence_regs(d[2]);
+            const int x = w;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int y = 8 * h + rl;
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    float o[2];
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const int k = 4 * j + 2 * h + e;
+                        o[e] = fmaxf(fmaf((d[2][k] + d[1][k]) + d[0][k], K23, sB[64 + 8 * j + 2 * qd + e]), 0.f);
+                    }
+                    uint32_t hi, lo;
+                    split2(o[0], o[1], hi, lo);
+                    if (y < 14) {
+                        const int kc = (y * 4 + x) * 4 + j;
+                        *reinterpret_cast<uint32_t *>(act3 + act3_off(0, n_tiles, ridx, kc) + qd * 4) = hi;
+                        *reinterpret_cast<uint32_t *>(act3 + act3_off(1, n_tiles, ridx, kc) + qd * 4) = lo;
+                    }
+                }
+            }
+        }
+        wg_sync(wg);
+        prof_t(3);
     }
     if (do_prof) for (int k = 0; k < 4; ++k) atomicAdd(&prof[k], (unsigned long long)pacc[k]);
 }
@@ -486,23 +571,23 @@ static int tc_prepare(void **state, const float *w, cudaStream_t stream) {
                 if (tap < 9) host_split2(c1w[n * 9 + tap] * TC_SCALE_W, s2);
                 for (int s = 0; s < 2; ++s) p1[((size_t)c2 * 64 + s * 32 + n) * 8 + e] = s2[s];
             }
-    for (int layer = 0; layer < 2; ++layer) {                    // conv2/3: [(shift tap, half)][split][chunk][n = stacked tap*32 + cout][8]
-        const float *cw = layer ? c3w : c2w;
-        uint16_t *dst = layer ? p3 : p2;
-        for (int dy = 0; dy < 3; ++dy)
-            for (int hh = 0; hh < 2; ++hh)
-                for (int c2 = 0; c2 < 2; ++c2)
-                    for (int dx = 0; dx < 3; ++dx)
-                        for (int n = 0; n < 32; ++n)
-                            for (int e = 0; e < 8; ++e) {
-                                int ci = 16 * hh + 8 * c2 + e;
-                                uint16_t s2[2];
-                                host_split2(cw[(n * 32 + ci) * 9 + dy * 3 + dx] * TC_SCALE_W, s2);
-                                // the tap that shifts the A operand (dy) selects the block, the other one (dx) is stacked along N
-                                for (int s = 0; s < 2; ++s)
-                                    dst[(((((size_t)(dy * 2 + hh)) * 2 + s) * 2 + c2) * 96 + dx * 32 + n) * 8 + e] = s2[s];
+    for (int dy = 0; dy < 3; ++dy)
+        for (int hh = 0; hh < 2; ++hh)
+            for (int c2 = 0; c2 < 2; ++c2)
+                for (int dx = 0; dx < 3; ++dx)
+                    for (int n = 0; n < 32; ++n)
+                        for (int e = 0; e < 8; ++e) {
+                            int ci = 16 * hh + 8 * c2 + e, tap = dy * 3 + dx;
+                            uint16_t s2[2], s3[2];
+                            host_split2(c2w[(n * 32 + ci) * 9 + tap] * TC_SCALE_W, s2);
+                            host_split2(c3w[(n * 32 + ci) * 9 + tap] * TC_SCALE_W, s3);
+                            for (int s = 0; s < 2; ++s) {
+                                // conv2: [(dy, half)][split][chunk][n = dx*32 + cout][8] (dx stacked along N)
+                                p2[(((((size_t)(dy * 2 + hh)) * 2 + s) * 2 + c2) * 96 + dx * 32 + n) * 8 + e] = s2[s];
+                                // conv3: [(dx, dy, half)][split][chunk][cout][8] (one block per accumulator and A shift)
+                                p3[((((((size_t)(dx * 3 + dy)) * 2 + hh) * 2 + s) * 2 + c2) * 32 + n) * 8 + e] = s3[s];
                             }
-    }
+                        }
     for (int j = 0; j < TCF_KBLOCKS; ++j)
         for (int c2 = 0; c2 < 2; ++c2)
             for (int n = 0; n < 256; ++n)
