@@ -35,8 +35,15 @@ enum { B200_MODE_LP = 0,        /* agents/ValueSimLP.py:13-70 */
        B200_MODE_DIST = 3 };    /* agents/core_distributional.py:82-124 driven as agents/DistValueSimOnline.py:36-75 sketches */
 enum { B200_EVAL_SYNTHETIC = 0, /* test evaluator (hash of the observation), shared with the CPU oracle */
        B200_EVAL_NET = 1,       /* model/model_vv.py Model_VV.inference, fp32 CUDA cores */
-       B200_EVAL_NET_TC = 2 };  /* same network on wgmma tensor cores (fp16 x 2 operand split, 3 products per product); in B200_MODE_DIST:
+       B200_EVAL_NET_TC = 2,    /* same network on wgmma tensor cores (fp16 x 2 operand split, 3 products per product); in B200_MODE_DIST:
                                    model/model_distributional.py on tensor cores (csrc/distnet_tc.cuh) instead of the fp32 CUDA-core kernels */
+       B200_EVAL_NET_FP16 = 3 };/* same weights and tensor-core kernels as B200_EVAL_NET_TC with ONE fp16 term per operand and one product per
+                                   product (about 1/3 of the MMA work).  Every activation and conv / fc1 weight is rounded to fp16 (2^-11
+                                   relative) instead of split (2^-22), so outputs are NOT within 1e-5 of Model_VV: DESIGN §5 states
+                                   the bounds (act3 per element within 2^-10 of the board's largest |term| sum, v and var within
+                                   2^-11 relative plus two ill-conditioned cases); the search on those outputs is exact.  Same weight
+                                   limits as B200_EVAL_NET_TC.  Not available in B200_MODE_DIST (b200_engine_create returns
+                                   B200_ERR_BAD_ARG) nor for b200_load_dist_weights. */
 
 typedef struct b200_engine b200_engine;
 
@@ -77,8 +84,9 @@ int b200_engine_set_stream(b200_engine *e, void *cuda_stream);
 int b200_engine_get_stream(b200_engine *e, void **cuda_stream_out);
 
 /* --- Model.load (model/model.py:163-174): weights = the state_dict tensors concatenated (B200_N_WEIGHTS floats).
- *     A B200_EVAL_NET_TC engine returns B200_ERR_BAD_ARG, keeping its previous weights, when a conv or fc1 weight is non-finite or has
- *     |w| * 64 > 65504 (fp16 overflow in the tensor cores' operand split); the same holds for b200_load_dist_weights. */
+ *     A B200_EVAL_NET_TC or B200_EVAL_NET_FP16 engine returns B200_ERR_BAD_ARG, keeping its previous weights, when a conv or fc1 weight
+ *     is non-finite or has |w| * 64 > 65504 (fp16 overflow in the tensor cores' scaled operands); the same holds for
+ *     b200_load_dist_weights (B200_EVAL_NET_TC). */
 int b200_load_weights(b200_engine *e, const float *weights);
 
 /* --- TreeAgent.update_root (agents/agent.py:296-301) for all games: recs[n_games][20] */
@@ -95,7 +103,7 @@ int b200_set_gc_headroom(b200_engine *e, int min_free);
 
 /* --- scheduling only (no reference counterpart, no effect on any result): the up to max_games games whose last trace was longest walk the tree
  * on a second stream, so that a simulation step of the other games does not last as long as the deepest walk of all (ValueSim / ValueSimLP with
- * B200_EVAL_NET_TC; ignored otherwise).  0 (default) = one lane. */
+ * B200_EVAL_NET_TC or B200_EVAL_NET_FP16; ignored otherwise).  0 (default) = one lane. */
 int b200_set_deep_lane(b200_engine *e, int max_games);
 
 /* --- memory traffic only (no reference counterpart, no effect on any result): the PATH CACHE.  Consecutive simulations of a game walk almost

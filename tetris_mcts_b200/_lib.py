@@ -14,7 +14,7 @@ N_ACTIONS = 7
 N_WEIGHTS = 478342
 
 MODE_LP, MODE_SINGLE, MODE_VANILLA, MODE_DIST = 0, 1, 2, 3
-EVAL_SYNTHETIC, EVAL_NET, EVAL_NET_TC = 0, 1, 2
+EVAL_SYNTHETIC, EVAL_NET, EVAL_NET_TC, EVAL_NET_FP16 = 0, 1, 2, 3
 ERR_NAMES = {1: "BAD_ARG", 2: "CUDA", 3: "ARENA_FULL", 4: "TRACE_FULL", 5: "NO_WEIGHTS"}
 
 

@@ -181,6 +181,8 @@ extern "C" int b200_engine_create(const b200_config *cfg, b200_engine **out) {
     if (cfg->mode < 0 || cfg->mode > 3) return fail(B200_ERR_BAD_ARG, "mode");
     if (cfg->mode == MODE_DIST && (cfg->dist_bins < 2 || cfg->dist_bins > 64 || !(cfg->dist_vmax > cfg->dist_vmin)))
         return fail(B200_ERR_BAD_ARG, "distributional mode needs 2 <= dist_bins <= 64 and dist_vmax > dist_vmin");
+    if (cfg->mode == MODE_DIST && cfg->eval_kind == B200_EVAL_NET_FP16)
+        return fail(B200_ERR_BAD_ARG, "eval_kind net_fp16 has no distributional network: use net_tc or net in B200_MODE_DIST");
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail(B200_ERR_CUDA, "no CUDA device: this library has no CPU path");
     CK(cudaSetDevice(cfg->device));
@@ -296,12 +298,22 @@ extern "C" int b200_engine_get_stream(b200_engine *e, void **cuda_stream_out) {
 }
 
 // ---------------------------------------------------------------------------------------------------- weights
+#ifdef B200_WITH_TC
+// net_tc and net_fp16 run the same tensor-core kernels and weight layout, with two fp16 terms per operand or one (valuenet_tc.cuh)
+static bool tc_net(const b200_engine *e) { return e->cfg.eval_kind == B200_EVAL_NET_TC || e->cfg.eval_kind == B200_EVAL_NET_FP16; }
+static decltype(&k_tc_conv<2>) tc_conv_kernel(const b200_engine *e) { return e->cfg.eval_kind == B200_EVAL_NET_FP16 ? k_tc_conv<1> : k_tc_conv<2>; }
+static decltype(&k_tc_fc<2>) tc_fc_kernel(const b200_engine *e) { return e->cfg.eval_kind == B200_EVAL_NET_FP16 ? k_tc_fc<1> : k_tc_fc<2>; }
+#endif
+
 extern "C" int b200_load_weights(b200_engine *e, const float *w) {
     if (!e || !w) return fail(B200_ERR_BAD_ARG, "null argument");
 #ifdef B200_WITH_TC
-    if (e->cfg.eval_kind == B200_EVAL_NET_TC && !tc_weights_fit(w))
-        return fail(B200_ERR_BAD_ARG, "net_tc: a conv or fc1 weight is non-finite or has |w| * 64 > 65504, which overflows the tensor cores' "
-                                      "fp16 x 2 operand split (eval_kind net takes finite weights of any size)");
+    if (tc_net(e) && !tc_weights_fit(w))
+        return fail(B200_ERR_BAD_ARG, e->cfg.eval_kind == B200_EVAL_NET_TC
+                    ? "net_tc: a conv or fc1 weight is non-finite or has |w| * 64 > 65504, which overflows the tensor cores' "
+                      "fp16 x 2 operand split (eval_kind net takes finite weights of any size)"
+                    : "net_fp16: a conv or fc1 weight is non-finite or has |w| * 64 > 65504, which overflows the tensor cores' "
+                      "scaled fp16 operands (eval_kind net takes finite weights of any size)");
 #endif
     CK(cudaSetDevice(e->cfg.device));
     const float *c1w = w, *c1b = c1w + 288, *c2w = c1b + 32, *c2b = c2w + 9216, *c3w = c2b + 32, *c3b = c3w + 9216;
@@ -365,19 +377,19 @@ static int launch_net(b200_engine *e, const uint2 *req, const int32_t *n_req, co
                       size_t max_rows) {
     if (!e->have_weights) return fail(B200_ERR_NO_WEIGHTS, "b200_load_weights was not called");
 #ifdef B200_WITH_TC
-    if (e->cfg.eval_kind == B200_EVAL_NET_TC) {
+    if (tc_net(e)) {
         TcState *st = (TcState *)e->tc_state;
         const uint8_t *act3_before = st->d_act3;
         if (tc_ensure_act3(st, max_rows, e->stream)) return fail(B200_ERR_CUDA, "act3 (tensor-core layout) allocation failed");
         if (act3_before && st->d_act3 != act3_before) drop_step_graph(e);   // a larger standalone batch moved the activation buffer
         {
             PhaseTimer t(e, PH_CONV);
-            k_tc_conv<<<e->n_sm, TCC_THREADS, TCC_SMEM, e->stream>>>(e->W, st->TW, req, n_req, nullptr, keys, M, st->d_act3, (int)st->tiles,
-                                                                    e->timing ? e->A.counters + 16 : nullptr);
+            tc_conv_kernel(e)<<<e->n_sm, TCC_THREADS, TCC_SMEM, e->stream>>>(e->W, st->TW, req, n_req, nullptr, keys, M, st->d_act3, (int)st->tiles,
+                                                                             e->timing ? e->A.counters + 16 : nullptr);
         }
         {
             PhaseTimer t(e, PH_FC);
-            k_tc_fc<<<e->n_sm, TCF_THREADS, TCF_SMEM, e->stream>>>(e->W, st->TW, st->d_act3, (int)st->tiles, req, n_req, eval_out);
+            tc_fc_kernel(e)<<<e->n_sm, TCF_THREADS, TCF_SMEM, e->stream>>>(e->W, st->TW, st->d_act3, (int)st->tiles, req, n_req, eval_out);
         }
         CK(cudaGetLastError());
         return B200_OK;
@@ -405,6 +417,7 @@ __global__ void k_states_to_keys(const int8_t *states, int k, uint32_t *keys, ui
 
 extern "C" int b200_load_dist_weights(b200_engine *e, const float *w, int atoms) {
     if (!e || !w || atoms < 2 || atoms > 64) return fail(B200_ERR_BAD_ARG, "bad argument");
+    if (e->cfg.eval_kind == B200_EVAL_NET_FP16) return fail(B200_ERR_BAD_ARG, "eval_kind net_fp16 has no distributional network");
     CK(cudaSetDevice(e->cfg.device));
     if (e->A.mode == MODE_DIST && atoms != e->A.dist_bins) return fail(B200_ERR_BAD_ARG, "atoms must equal dist_bins");
 #ifdef B200_WITH_TC
@@ -617,7 +630,7 @@ extern "C" int b200_get_games(b200_engine *e, uint32_t *recs) {
 // ---------------------------------------------------------------------------------------------------- simulations
 static bool deep_lane_on(const b200_engine *e) {
 #ifdef B200_WITH_TC
-    return e->deep_cap > 0 && (e->A.mode == MODE_LP || e->A.mode == MODE_SINGLE) && e->cfg.eval_kind == B200_EVAL_NET_TC && !B200_FUSED_BACKUP;
+    return e->deep_cap > 0 && (e->A.mode == MODE_LP || e->A.mode == MODE_SINGLE) && tc_net(e) && !B200_FUSED_BACKUP;
 #else
     return false;
 #endif
@@ -661,18 +674,18 @@ static int enqueue_step_lanes(b200_engine *e) {
     }
     {
         PhaseTimer t(e, PH_CONV);
-        k_tc_conv<<<e->n_sm, TCC_THREADS, TCC_SMEM, s0>>>(e->W, st->TW, A.req, A.n_req, nullptr, A.key, A.M, st->d_act3, (int)st->tiles,
-                                                          e->timing ? A.counters + 16 : nullptr);
+        tc_conv_kernel(e)<<<e->n_sm, TCC_THREADS, TCC_SMEM, s0>>>(e->W, st->TW, A.req, A.n_req, nullptr, A.key, A.M, st->d_act3, (int)st->tiles,
+                                                                  e->timing ? A.counters + 16 : nullptr);
     }
     if (s1 != s0) { CK(cudaEventRecord(e->ev_join, s1)); CK(cudaStreamWaitEvent(s0, e->ev_join, 0)); }
     {
         PhaseTimer t(e, PH_CONV);
         k_merge_requests<<<1, 256, 0, s0>>>(A.req, A.n_req, e->d_req_deep, e->d_nreq_deep);
-        k_tc_conv<<<e->n_sm, TCC_THREADS, TCC_SMEM, s0>>>(e->W, st->TW, A.req, A.n_req, A.n_req + 2, A.key, A.M, st->d_act3, (int)st->tiles, nullptr);
+        tc_conv_kernel(e)<<<e->n_sm, TCC_THREADS, TCC_SMEM, s0>>>(e->W, st->TW, A.req, A.n_req, A.n_req + 2, A.key, A.M, st->d_act3, (int)st->tiles, nullptr);
     }
     {
         PhaseTimer t(e, PH_FC);
-        k_tc_fc<<<e->n_sm, TCF_THREADS, TCF_SMEM, s0>>>(e->W, st->TW, st->d_act3, (int)st->tiles, A.req, A.n_req, A.eval_out);
+        tc_fc_kernel(e)<<<e->n_sm, TCF_THREADS, TCF_SMEM, s0>>>(e->W, st->TW, st->d_act3, (int)st->tiles, A.req, A.n_req, A.eval_out);
     }
     {
         PhaseTimer t(e, PH_BACKUP);
@@ -1012,8 +1025,9 @@ extern "C" int b200_debug_act3(b200_engine *e, const int8_t *states, int k, floa
     int rc = b200_valuenet_forward(e, states, k, v.data(), var.data());   // leaves act3 of these k boards in the scratch buffers
     if (rc) return rc;
 #ifdef B200_WITH_TC
-    if (e->cfg.eval_kind == B200_EVAL_NET_TC) {
+    if (tc_net(e)) {
         TcState *st = (TcState *)e->tc_state;
+        const int planes = e->cfg.eval_kind == B200_EVAL_NET_FP16 ? 1 : 2;   // net_fp16 writes the first term only
         size_t bytes = (size_t)2 * st->tiles * ACT3_KCHUNKS * 2048;
         std::vector<uint8_t> h(bytes);
         CK(cudaMemcpy(h.data(), st->d_act3, bytes, cudaMemcpyDeviceToHost));
@@ -1021,7 +1035,7 @@ extern "C" int b200_debug_act3(b200_engine *e, const int8_t *states, int k, floa
             for (int kp = 0; kp < 1792; ++kp) {
                 int p = kp >> 5, c = kp & 31;
                 float sum = 0.f;
-                for (int s = 1; s >= 0; --s) {
+                for (int s = planes - 1; s >= 0; --s) {
                     size_t off = ((((size_t)s * st->tiles + (r >> 7)) * ACT3_KCHUNKS + (kp >> 3)) * 128 + (r & 127)) * 16 + (kp & 7) * 2;
                     uint16_t hb; memcpy(&hb, &h[off], 2);
                     sum += host_half_f(hb);

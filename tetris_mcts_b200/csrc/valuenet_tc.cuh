@@ -19,6 +19,12 @@
 //              both operands are stored in HBM already in the no-swizzle K-major layout, so one bulk copy per operand block needs
 //              no tensor map; one producer warp, two consumer warpgroups (64 rows each, N = 256 accumulators in registers);
 //              the epilogue fuses bias+ReLU+fc_out+sigmoid+affine and scatters (v, var) to the requesting tree slot.
+//
+// Both kernels take the number of fp16 terms per operand, NT, as a template argument.  NT = 2 is the split above (eval_kind net_tc).
+// NT = 1 (eval_kind net_fp16) keeps only x1 of every activation and weight and issues the single product a1*b1: conv1 runs at N = 32
+// (the second weight term is no longer stacked along N), conv2 / conv3 / fc1 issue one MMA where the split issues three, the epilogues
+// round to one fp16, and act3 in HBM is one plane.  Same scaling, same layouts (the x2 slots stay allocated and are not read), so the
+// overflow and subnormal limits of the split carry over; each rounded operand is exact to 2^-11 relative instead of 2^-22.
 #pragma once
 #include <cuda_fp16.h>
 #include "gmma.cuh"
@@ -128,6 +134,11 @@ __device__ __forceinline__ void split2(float x0, float x1, uint32_t &hi, uint32_
     const __half2 l = __floats2half2_rn(x0 - f.x, x1 - f.y);
     hi = *reinterpret_cast<const uint32_t *>(&h); lo = *reinterpret_cast<const uint32_t *>(&l);
 }
+// the NT = 1 form: x ~= x1, one fp16 per value (round-to-nearest)
+__device__ __forceinline__ uint32_t round1(float x0, float x1) {
+    const __half2 h = __floats2half2_rn(x0, x1);
+    return *reinterpret_cast<const uint32_t *>(&h);
+}
 
 // ---------------------------------------------------------------------------------------------------- conv kernel
 // In conv2 the three horizontal taps (dx) of a 3x3 filter are stacked along N, so the layer is a few wide MMAs instead of many narrow ones:
@@ -174,6 +185,14 @@ constexpr int TCC_SMEM = TCC_OFF_KEY + TCC_WGS * 32 * 4;
 constexpr int ACT3_KCHUNKS = 224;           // 1792 / 8
 static_assert(TCC_SMEM <= 227 * 1024, "k_tc_conv shared memory");
 
+// MMA work issued per board, in n-units: one column of an m64 k16 wgmma = 64 * 16 * 2 = 2048 FLOP.  NT = 2 / NT = 1:
+//   conv1  3 tiles x N = 64 / 32;  conv2  2 tiles x (18 / 6) x N = 96;  conv3  (54 / 18) x N = 32
+// fc1 issues 1792 x 256 x 2 FLOP per board per product (3 / 1 products).  scripts/eval_kind_bench.py reads these four lines.
+constexpr int TC_NUNIT_FLOP = 64 * 16 * 2;
+constexpr int TC_CONV_NUNITS_NT2 = 3 * 64 + 2 * 18 * 96 + 54 * 32;   // 5376 -> 11.01 MFLOP per board
+constexpr int TC_CONV_NUNITS_NT1 = 3 * 32 + 2 * 6 * 96 + 18 * 32;    // 1824 -> 3.74 MFLOP per board
+constexpr int TC_FC_FLOP_PER_PRODUCT = 1792 * 256 * 2;                // x3 -> 2.75 MFLOP, x1 -> 0.92 MFLOP per board
+
 struct TcWeights {
     const uint8_t *wc1;         // TCC_W1BYTES
     const uint8_t *wc2, *wc3;   // TCC_WBYTES each, already in the shared-memory layout
@@ -185,7 +204,9 @@ __device__ __forceinline__ size_t act3_off(int split, int n_tiles, int ridx, int
     return ((((size_t)split * n_tiles + (ridx >> 7)) * ACT3_KCHUNKS + kchunk) * 128 + (ridx & 127)) * 16;
 }
 
-// conv2 on one 64-row tile = 18 wgmma of N = 96: for each (dy, channel half): a1*W1, a1*W2, a2*W1 into the same 96 columns.
+// conv2 on one 64-row tile = 18 wgmma of N = 96: for each (dy, channel half): a1*W1, a1*W2, a2*W1 into the same 96 columns
+// (NT = 1: a1*W1 only, 6 wgmma).
+template <int NT>
 __device__ __forceinline__ void issue_conv2(float (&d)[48], uint32_t a_addr, uint32_t w_addr) {
     const uint64_t a0 = gmma_desc(a_addr, TCC_R * 16, 128), b0 = gmma_desc(w_addr, 96 * 16, 128);
 #pragma unroll
@@ -195,14 +216,17 @@ __device__ __forceinline__ void issue_conv2(float (&d)[48], uint32_t a_addr, uin
             const uint32_t a_hi = 2 * h * TCC_R + dy * 8, a_lo = a_hi + 4 * TCC_R;          // 16-byte units
             const uint32_t b_hi = (dy * 2 + h) * (TCC_WBLOCK / 16), b_lo = b_hi + 2 * 96;
             wgmma_n96(d, a0 + a_hi, b0 + b_hi, (dy | h) ? 1u : 0u);
-            wgmma_n96(d, a0 + a_hi, b0 + b_lo, 1u);
-            wgmma_n96(d, a0 + a_lo, b0 + b_hi, 1u);
+            if (NT == 2) {
+                wgmma_n96(d, a0 + a_hi, b0 + b_lo, 1u);
+                wgmma_n96(d, a0 + a_lo, b0 + b_hi, 1u);
+            }
         }
     }
 }
 
-// conv3 on its one 64-row tile = 3 accumulators x 18 wgmma of N = 32: for each (dy, channel half) and each dx, a1*W1, a1*W2, a2*W1.
-// The A operand of tap (dy, dx) starts 16 dx + dy rows (16-byte units) into act2.
+// conv3 on its one 64-row tile = 3 accumulators x 18 wgmma of N = 32: for each (dy, channel half) and each dx, a1*W1, a1*W2, a2*W1
+// (NT = 1: a1*W1 only, 3 x 6 wgmma).  The A operand of tap (dy, dx) starts 16 dx + dy rows (16-byte units) into act2.
+template <int NT>
 __device__ __forceinline__ void issue_conv3(float (&d)[3][16], uint32_t a_addr, uint32_t w_addr) {
     const uint64_t a0 = gmma_desc(a_addr, TCC_R2 * 16, 128), b0 = gmma_desc(w_addr, 32 * 16, 128);
 #pragma unroll
@@ -214,8 +238,10 @@ __device__ __forceinline__ void issue_conv3(float (&d)[3][16], uint32_t a_addr, 
                 const uint32_t a_hi = 2 * h * TCC_R2 + 16 * dx + dy, a_lo = a_hi + TCC_A2SPLIT / 16;    // 16-byte units
                 const uint32_t b_hi = ((dx * 3 + dy) * 2 + h) * 2 * (TCC_W3BLOCK / 16), b_lo = b_hi + TCC_W3BLOCK / 16;
                 wgmma_n32(d[dx], a0 + a_hi, b0 + b_hi, (dy | h) ? 1u : 0u);
-                wgmma_n32(d[dx], a0 + a_hi, b0 + b_lo, 1u);
-                wgmma_n32(d[dx], a0 + a_lo, b0 + b_hi, 1u);
+                if (NT == 2) {
+                    wgmma_n32(d[dx], a0 + a_hi, b0 + b_lo, 1u);
+                    wgmma_n32(d[dx], a0 + a_lo, b0 + b_hi, 1u);
+                }
             }
         }
     }
@@ -240,6 +266,7 @@ __device__ __forceinline__ void build_im2col3(uint8_t *im, const uint32_t *tab, 
     }
 }
 
+template <int NT>
 __global__ void __launch_bounds__(TCC_THREADS, 1)
 k_tc_conv(NetWeights W, TcWeights TW, const uint2 *req, const int32_t *n_req_ptr, const int32_t *first_ptr, const uint32_t *keys, int M, uint8_t *act3,
           int n_tiles, unsigned long long *prof) {
@@ -303,13 +330,16 @@ k_tc_conv(NetWeights W, TcWeights TW, const uint2 *req, const int32_t *n_req_ptr
         wg_sync(wg);
         prof_t(0);
         // ---- conv1 (model_vv.py:32): im2col [192 x 16] x W1 [16 x 64] in three 64-row tiles; epilogue: bias + ReLU + split -> act1
+        // (NT = 1: x W1 [16 x 32], the first weight term only; epilogue rounds to one fp16)
 #pragma unroll 1
         for (int mt = 0; mt < 3; ++mt) {
-            float d[32];
+            float d[16 * NT];
 #pragma unroll
-            for (int k = 0; k < 32; ++k) d[k] = 0.f;
+            for (int k = 0; k < 16 * NT; ++k) d[k] = 0.f;
             wgmma_fence();
-            wgmma_n64(d, gmma_desc(s_im + mt * 1024, TCC_IMROWS * 16, 128), gmma_desc(s_w1, 64 * 16, 128), 0u);
+            const uint64_t ad = gmma_desc(s_im + mt * 1024, TCC_IMROWS * 16, 128), bd = gmma_desc(s_w1, 64 * 16, 128);
+            if constexpr (NT == 2) wgmma_n64(d, ad, bd, 0u);
+            else wgmma_n32(d, ad, bd, 0u);                       // cout 0..31 of each k chunk: the first weight term
             wgmma_commit();
             wgmma_wait<0>();
             fence_regs(d);
@@ -320,13 +350,19 @@ k_tc_conv(NetWeights W, TcWeights TW, const uint2 *req, const int32_t *n_req_ptr
 #pragma unroll
                     for (int j = 0; j < 4; ++j) {                // cout 8j + 2qd + e: weight split 1 sits 32 columns (4 blocks) further
                         const int c = 8 * j + 2 * qd;
-                        const float o0 = fmaxf(fmaf(d[4 * (j + 4) + 2 * h] + d[4 * j + 2 * h], K1, sB[c]), 0.f);
-                        const float o1 = fmaxf(fmaf(d[4 * (j + 4) + 2 * h + 1] + d[4 * j + 2 * h + 1], K1, sB[c + 1]), 0.f);
-                        uint32_t hi, lo;
-                        split2(o0, o1, hi, lo);
                         uint8_t *dst = act + (j * TCC_R + r) * 16 + qd * 4;
-                        *reinterpret_cast<uint32_t *>(dst) = hi;
-                        *reinterpret_cast<uint32_t *>(dst + SPLIT) = lo;
+                        if constexpr (NT == 2) {
+                            const float o0 = fmaxf(fmaf(d[4 * (j + 4) + 2 * h] + d[4 * j + 2 * h], K1, sB[c]), 0.f);
+                            const float o1 = fmaxf(fmaf(d[4 * (j + 4) + 2 * h + 1] + d[4 * j + 2 * h + 1], K1, sB[c + 1]), 0.f);
+                            uint32_t hi, lo;
+                            split2(o0, o1, hi, lo);
+                            *reinterpret_cast<uint32_t *>(dst) = hi;
+                            *reinterpret_cast<uint32_t *>(dst + SPLIT) = lo;
+                        } else {
+                            const float o0 = fmaxf(fmaf(d[4 * j + 2 * h], K1, sB[c]), 0.f);
+                            const float o1 = fmaxf(fmaf(d[4 * j + 2 * h + 1], K1, sB[c + 1]), 0.f);
+                            *reinterpret_cast<uint32_t *>(dst) = round1(o0, o1);
+                        }
                     }
                 }
             }
@@ -342,14 +378,15 @@ k_tc_conv(NetWeights W, TcWeights TW, const uint2 *req, const int32_t *n_req_ptr
 #pragma unroll
             for (int k = 0; k < 48; ++k) d[k] = 0.f;
             wgmma_fence();
-            issue_conv2(d, s_act + mt * 1024, s_w2);
+            issue_conv2<NT>(d, s_act + mt * 1024, s_w2);
             wgmma_commit();
             wgmma_wait<0>();
             fence_regs(d);
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const int y = mt * 8 + 2 * w + h, x = rl;
-                uint32_t v[8];                                   // v[j + 4s]: channels 8j + 2qd (+1), fp16 term s
+                constexpr int NW = 4 * NT;                       // words per pixel and lane
+                uint32_t v[NW];                                  // v[j + 4s]: channels 8j + 2qd (+1), fp16 term s
 #pragma unroll
                 for (int j = 0; j < 4; ++j) {
                     float o[2];
@@ -359,24 +396,26 @@ k_tc_conv(NetWeights W, TcWeights TW, const uint2 *req, const int32_t *n_req_ptr
                         const float s1 = __shfl_down_sync(0xffffffffu, d[16 + k], 4), s2 = __shfl_down_sync(0xffffffffu, d[32 + k], 8);
                         o[e] = fmaxf(fmaf((s2 + s1) + d[k], K23, sB[32 + 8 * j + 2 * qd + e]), 0.f);
                     }
-                    split2(o[0], o[1], v[j], v[4 + j]);
+                    if constexpr (NT == 2) split2(o[0], o[1], v[j], v[4 + j]);
+                    else v[j] = round1(o[0], o[1]);
                 }
                 // Store k of lane (x, qd) writes word i = (k + x) & 7 at split i/4, chunk i%4, row x*16 + y: in 4-byte banks that is
                 // (8 (i%4) + 4 (i/4) + 4y + qd) mod 32 (row x*16 is 256 B, a multiple of the 128-B bank line), so the six pixels x < 6
                 // hit six disjoint 4-bank groups: one wavefront per store instead of a 6-way conflict.  The words are rotated into place
-                // by x with selects (a dynamically indexed array would live in local memory).
+                // by x with selects (a dynamically indexed array would live in local memory).  NT = 1 rotates its four words by x & 3:
+                // pixels x and x + 4 share a bank group, two wavefronts for each of four stores.
 #pragma unroll
-                for (int b = 1; b < 8; b <<= 1) {
-                    uint32_t r[8];
+                for (int b = 1; b < NW; b <<= 1) {
+                    uint32_t r[NW];
 #pragma unroll
-                    for (int k = 0; k < 8; ++k) r[k] = (x & b) ? v[(k + b) & 7] : v[k];
+                    for (int k = 0; k < NW; ++k) r[k] = (x & b) ? v[(k + b) & (NW - 1)] : v[k];
 #pragma unroll
-                    for (int k = 0; k < 8; ++k) v[k] = r[k];
+                    for (int k = 0; k < NW; ++k) v[k] = r[k];
                 }
                 if (x < 6) {                                     // act2: 16x6 valid pixels
 #pragma unroll
-                    for (int k = 0; k < 8; ++k) {
-                        const int i = (k + x) & 7;
+                    for (int k = 0; k < NW; ++k) {
+                        const int i = (k + x) & (NW - 1);
                         *reinterpret_cast<uint32_t *>(act2 + (i >> 2) * TCC_A2SPLIT + ((i & 3) * TCC_R2 + x * 16 + y) * 16 + qd * 4) = v[k];
                     }
                 }
@@ -391,7 +430,7 @@ k_tc_conv(NetWeights W, TcWeights TW, const uint2 *req, const int32_t *n_req_ptr
 #pragma unroll
             for (int k = 0; k < 16; ++k) d[0][k] = d[1][k] = d[2][k] = 0.f;
             wgmma_fence();
-            issue_conv3(d, s_act2, s_w3);
+            issue_conv3<NT>(d, s_act2, s_w3);
             wgmma_commit();
             wgmma_wait<0>();
             fence_regs(d[0]); fence_regs(d[1]); fence_regs(d[2]);
@@ -407,12 +446,17 @@ k_tc_conv(NetWeights W, TcWeights TW, const uint2 *req, const int32_t *n_req_ptr
                         const int k = 4 * j + 2 * h + e;
                         o[e] = fmaxf(fmaf((d[2][k] + d[1][k]) + d[0][k], K23, sB[64 + 8 * j + 2 * qd + e]), 0.f);
                     }
-                    uint32_t hi, lo;
-                    split2(o[0], o[1], hi, lo);
-                    if (y < 14) {
-                        const int kc = (y * 4 + x) * 4 + j;
-                        *reinterpret_cast<uint32_t *>(act3 + act3_off(0, n_tiles, ridx, kc) + qd * 4) = hi;
-                        *reinterpret_cast<uint32_t *>(act3 + act3_off(1, n_tiles, ridx, kc) + qd * 4) = lo;
+                    if constexpr (NT == 2) {
+                        uint32_t hi, lo;
+                        split2(o[0], o[1], hi, lo);
+                        if (y < 14) {
+                            const int kc = (y * 4 + x) * 4 + j;
+                            *reinterpret_cast<uint32_t *>(act3 + act3_off(0, n_tiles, ridx, kc) + qd * 4) = hi;
+                            *reinterpret_cast<uint32_t *>(act3 + act3_off(1, n_tiles, ridx, kc) + qd * 4) = lo;
+                        }
+                    } else {
+                        const uint32_t hi = round1(o[0], o[1]);
+                        if (y < 14) *reinterpret_cast<uint32_t *>(act3 + act3_off(0, n_tiles, ridx, (y * 4 + x) * 4 + j) + qd * 4) = hi;
                     }
                 }
             }
@@ -438,6 +482,7 @@ static_assert(2 * TCF_STAGES * 8 <= 256, "barrier block overflows into the epilo
 constexpr int TCF_SMEM = TCF_OFF_EPI + (256 * 3 + 8) * 4;
 static_assert(TCF_SMEM <= 227 * 1024, "k_tc_fc shared memory");
 
+template <int NT>
 __global__ void __launch_bounds__(TCF_THREADS, 1)
 k_tc_fc(NetWeights W, TcWeights TW, const uint8_t *act3, int n_tiles_alloc, const uint2 *req, const int32_t *n_req_ptr, float2 *eval_out) {
     extern __shared__ __align__(128) uint8_t smem[];
@@ -460,10 +505,10 @@ k_tc_fc(NetWeights W, TcWeights TW, const uint8_t *act3, int n_tiles_alloc, cons
             for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
                 for (int j = 0; j < TCF_KBLOCKS; ++j) {
                     mbar_wait(&empty[stage], ph ^ 1);
-                    mbar_expect_tx(&full[stage], TCF_STAGE);
+                    mbar_expect_tx(&full[stage], NT * (TCF_A_BYTES + TCF_B_BYTES));
                     uint8_t *dst = smem + stage * TCF_STAGE;
 #pragma unroll
-                    for (int s = 0; s < 2; ++s) {
+                    for (int s = 0; s < NT; ++s) {               // NT = 1: the first term of each operand; its second-term slots stay unused
                         bulk_g2s(dst + s * TCF_A_BYTES, act3 + (((size_t)s * n_tiles_alloc + tile) * ACT3_KCHUNKS + 2 * j) * 2048, TCF_A_BYTES, &full[stage]);
                         bulk_g2s(dst + 2 * TCF_A_BYTES + s * TCF_B_BYTES, TW.wfc + ((size_t)s * TCF_KBLOCKS + j) * TCF_B_BYTES, TCF_B_BYTES, &full[stage]);
                     }
@@ -471,8 +516,9 @@ k_tc_fc(NetWeights W, TcWeights TW, const uint8_t *act3, int n_tiles_alloc, cons
                 }
             }
         }
-    } else {   // ===== consumers: D[64 x 256] += A[64 x 16] * B[256 x 16]^T per warpgroup, three split terms per k block
+    } else {   // ===== consumers: D[64 x 256] += A[64 x 16] * B[256 x 16]^T per warpgroup, three split terms per k block (NT = 1: one)
         const int wg = t >> 7, w = warp & 3, qd = lane & 3, rl = lane >> 2;
+        constexpr int T0 = NT == 2 ? 0 : 2;              // first of the three products issued
         int stage = 0; uint32_t ph = 0;
         for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
             float d[128];
@@ -484,11 +530,11 @@ k_tc_fc(NetWeights W, TcWeights TW, const uint8_t *act3, int n_tiles_alloc, cons
                 const uint32_t sbase = smem_u32(smem + stage * TCF_STAGE);
                 wgmma_fence();
 #pragma unroll
-                for (int term = 0; term < 3; ++term) {   // a1*b2, a2*b1, a1*b1 (small terms first)
+                for (int term = T0; term < 3; ++term) {  // a1*b2, a2*b1, a1*b1 (small terms first); NT = 1: a1*b1
                     const int sa = term == 1 ? 1 : 0, sb = term == 0 ? 1 : 0;
                     const uint64_t ad = gmma_desc(sbase + sa * TCF_A_BYTES + wg * 1024, 128 * 16, 128);
                     const uint64_t bd = gmma_desc(sbase + 2 * TCF_A_BYTES + sb * TCF_B_BYTES, 256 * 16, 128);
-                    wgmma_n256(d, ad, bd, (j | term) ? 1u : 0u);
+                    wgmma_n256(d, ad, bd, (j > 0 || term > T0) ? 1u : 0u);
                 }
                 wgmma_commit();
                 wgmma_wait<1>();                         // the previous k block's MMAs are done with their stage
@@ -601,8 +647,10 @@ static int tc_prepare(void **state, const float *w, cudaStream_t stream) {
     if (cudaMemcpyAsync(st->d_w, h.data(), h.size(), cudaMemcpyHostToDevice, stream) != cudaSuccess) return 1;
     if (cudaStreamSynchronize(stream) != cudaSuccess) return 1;
     st->TW.wc1 = st->d_w; st->TW.wc2 = st->d_w + TCC_W1BYTES; st->TW.wc3 = st->TW.wc2 + TCC_WBYTES; st->TW.wfc = st->TW.wc3 + TCC_WBYTES;
-    if (cudaFuncSetAttribute(k_tc_conv, cudaFuncAttributeMaxDynamicSharedMemorySize, TCC_SMEM) != cudaSuccess) return 1;
-    if (cudaFuncSetAttribute(k_tc_fc, cudaFuncAttributeMaxDynamicSharedMemorySize, TCF_SMEM) != cudaSuccess) return 1;
+    if (cudaFuncSetAttribute(k_tc_conv<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, TCC_SMEM) != cudaSuccess) return 1;
+    if (cudaFuncSetAttribute(k_tc_conv<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, TCC_SMEM) != cudaSuccess) return 1;
+    if (cudaFuncSetAttribute(k_tc_fc<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, TCF_SMEM) != cudaSuccess) return 1;
+    if (cudaFuncSetAttribute(k_tc_fc<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, TCF_SMEM) != cudaSuccess) return 1;
     return 0;
 }
 

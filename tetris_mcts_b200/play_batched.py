@@ -107,7 +107,7 @@ def run(args, out=sys.stdout, timing=None):
             weights = init_weights(0)
     # k_init_arena seeds game g's search stream with seed + 0x9E3779B9 * (g + 1): offset by the shard's first global index
     eng = BatchedEngine(hi - lo, max_nodes=args.max_nodes, mode=mode, gamma=gamma, low=low,
-                        eval_kind="net_tc" if mode != "vanilla" else "synthetic", weights=weights, env_args=env_args,
+                        eval_kind=args.eval_kind if mode != "vanilla" else "synthetic", weights=weights, env_args=env_args,
                         seed=(args.seed + 0x9E3779B9 * lo) & 0xFFFFFFFF, device=device, overflow_reset=True)
     eng.set_games(PT.new_games(hi - lo, env_args, D.shard_seeds(args.seed, args.n_parallel, rank, world)))
     eng.set_gc_headroom(args.max_nodes * 5 // 32)
@@ -236,6 +236,9 @@ def parse_args(argv=None):
     p.add_argument('--train_max_iters', default=50000, type=int, help='most optimiser steps per training (--online; early stopping usually ends it)')
     p.add_argument('--train_kind', default='fp64', choices=('fp64', 'tc'),
                    help='trainer GEMMs (--online): fp64 CUDA cores, or tc = Hopper tensor cores with the 3xTF32 split')
+    p.add_argument('--eval_kind', default='net_tc', choices=('net_tc', 'net_fp16'),
+                   help='value network of the search (not Vanilla): net_tc = tensor cores within 1e-5 of fp32, net_fp16 = one fp16 product per '
+                        'product, about a third of the tensor-core work (DESIGN §5).  --online trains in fp32 / fp64 either way')
     p.add_argument('--max_moves', default=0, type=int)
     p.add_argument('--dist_backend', default='nccl', choices=('nccl', 'gloo'),
                    help='under torchrun: collectives over NCCL (one GPU per rank), or gloo through the host (several ranks may share a GPU)')
