@@ -15,7 +15,7 @@ ROOT = os.path.dirname(HERE)
 sys.path.insert(0, os.path.join(ROOT, "oracle"))
 
 
-@pytest.fixture(scope="module", params=[(), ("-DB200_PLAY_UNIFIED=0",)], ids=["default", "branchy-step"])
+@pytest.fixture(scope="module", params=[()], ids=["default"])
 def host_env(request, tmp_path_factory):
     so = str(tmp_path_factory.mktemp("hostenv") / "host_env.so")
     subprocess.run(["g++", "-O2", "-shared", "-fPIC", "-x", "c++", *request.param, "-I", os.path.join(ROOT, "tetris_mcts_b200", "csrc"),

@@ -6,7 +6,7 @@ import os
 import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("B200_TETRIS_LIB") or os.path.join(HERE, "libb200_tetris_mcts.so")   # the variable is a development aid (A/B builds)
+LIB_PATH = os.path.join(HERE, "libb200_tetris_mcts.so")
 
 REC_WORDS = 20
 KEY_WORDS = 12

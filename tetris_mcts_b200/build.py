@@ -19,21 +19,18 @@ def _stale():
     return any(os.path.exists(d) and os.path.getmtime(d) > t for d in deps)
 
 
-def build(force=False, verbose=False, out=None, defines=()):
-    """out / defines: development aid — build a variant (e.g. -DB200_WARM_SELECT=1) next to the product library; the
-    variant is loaded instead when the environment names it in B200_TETRIS_LIB (tetris_mcts_b200/_lib.py)."""
-    if out is None and not force and not _stale():
+def build(force=False, verbose=False):
+    if not force and not _stale():
         return LIB
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
     if not os.path.exists(nvcc):
         nvcc = "nvcc"
-    defs = ["-DB200_WITH_TC"] if os.path.exists(os.path.join(CSRC, "valuenet_tc.cuh")) else []
-    cmd = [nvcc] + FLAGS + defs + list(defines) + [os.path.join(CSRC, s) for s in SOURCES] + ["-o", out or LIB, "-lcuda"]
+    cmd = [nvcc] + FLAGS + [os.path.join(CSRC, s) for s in SOURCES] + ["-o", LIB, "-lcuda"]
     if verbose:
         cmd.insert(1, "-Xptxas=-v")
         print(" ".join(cmd), flush=True)
     subprocess.run(cmd, check=True)
-    return out or LIB
+    return LIB
 
 
 if __name__ == "__main__":

@@ -15,10 +15,8 @@
 #include "dist_dev.cuh"
 #include "distnet_simt.cuh"
 #include "replay_policy.cuh"
-#ifdef B200_WITH_TC
 #include "valuenet_tc.cuh"
 #include "distnet_tc.cuh"
-#endif
 
 using namespace b200;
 
@@ -260,10 +258,8 @@ extern "C" int b200_engine_destroy(b200_engine *e) {
     if (!e) return B200_OK;
     if (e->stream) cudaStreamSynchronize(e->stream);
     if (e->step_exec) cudaGraphExecDestroy(e->step_exec);
-#ifdef B200_WITH_TC
     tc_destroy(e->tc_state);
     dn_tc_destroy(e->dn_tc_state);
-#endif
     for (void *p : e->allocs) cudaFree(p);
     for (auto &ev : e->ev) cudaEventDestroy(ev);
     if (e->t0) { cudaEventDestroy(e->t0); cudaEventDestroy(e->t1); }
@@ -298,23 +294,19 @@ extern "C" int b200_engine_get_stream(b200_engine *e, void **cuda_stream_out) {
 }
 
 // ---------------------------------------------------------------------------------------------------- weights
-#ifdef B200_WITH_TC
 // net_tc and net_fp16 run the same tensor-core kernels and weight layout, with two fp16 terms per operand or one (valuenet_tc.cuh)
 static bool tc_net(const b200_engine *e) { return e->cfg.eval_kind == B200_EVAL_NET_TC || e->cfg.eval_kind == B200_EVAL_NET_FP16; }
 static decltype(&k_tc_conv<2>) tc_conv_kernel(const b200_engine *e) { return e->cfg.eval_kind == B200_EVAL_NET_FP16 ? k_tc_conv<1> : k_tc_conv<2>; }
 static decltype(&k_tc_fc<2>) tc_fc_kernel(const b200_engine *e) { return e->cfg.eval_kind == B200_EVAL_NET_FP16 ? k_tc_fc<1> : k_tc_fc<2>; }
-#endif
 
 extern "C" int b200_load_weights(b200_engine *e, const float *w) {
     if (!e || !w) return fail(B200_ERR_BAD_ARG, "null argument");
-#ifdef B200_WITH_TC
     if (tc_net(e) && !tc_weights_fit(w))
         return fail(B200_ERR_BAD_ARG, e->cfg.eval_kind == B200_EVAL_NET_TC
                     ? "net_tc: a conv or fc1 weight is non-finite or has |w| * 64 > 65504, which overflows the tensor cores' "
                       "fp16 x 2 operand split (eval_kind net takes finite weights of any size)"
                     : "net_fp16: a conv or fc1 weight is non-finite or has |w| * 64 > 65504, which overflows the tensor cores' "
                       "scaled fp16 operands (eval_kind net takes finite weights of any size)");
-#endif
     CK(cudaSetDevice(e->cfg.device));
     const float *c1w = w, *c1b = c1w + 288, *c2w = c1b + 32, *c2b = c2w + 9216, *c3w = c2b + 32, *c3b = c3w + 9216;
     const float *f1w = c3b + 32, *f1b = f1w + 458752, *fow = f1b + 256, *fob = fow + 512, *ub = fob + 2, *lb = ub + 2;
@@ -353,12 +345,10 @@ extern "C" int b200_load_weights(b200_engine *e, const float *w) {
     e->W.wfc1 = e->W.b1 + 96; e->W.bfc1 = e->W.wfc1 + (size_t)1792 * 256; e->W.wout = e->W.bfc1 + 256;
     e->W.bout = e->W.wout + 512; e->W.ub = e->W.bout + 2; e->W.lb = e->W.bout + 4;
     CK(cudaFuncSetAttribute(k_vn_conv, cudaFuncAttributeMaxDynamicSharedMemorySize, VN_SMEM_BYTES));
-#ifdef B200_WITH_TC
     {
         int rc = tc_prepare(&e->tc_state, w, e->stream);
         if (rc) return fail(B200_ERR_CUDA, "tensor-core weight preparation failed");
     }
-#endif
     e->have_weights = true;
     drop_step_graph(e);
     return B200_OK;
@@ -376,7 +366,6 @@ static int ensure_act3(b200_engine *e, size_t rows) {
 static int launch_net(b200_engine *e, const uint2 *req, const int32_t *n_req, const uint32_t *keys, int M, float2 *eval_out,
                       size_t max_rows) {
     if (!e->have_weights) return fail(B200_ERR_NO_WEIGHTS, "b200_load_weights was not called");
-#ifdef B200_WITH_TC
     if (tc_net(e)) {
         TcState *st = (TcState *)e->tc_state;
         const uint8_t *act3_before = st->d_act3;
@@ -394,7 +383,6 @@ static int launch_net(b200_engine *e, const uint2 *req, const int32_t *n_req, co
         CK(cudaGetLastError());
         return B200_OK;
     }
-#endif
     {
         const float *act3_before = e->d_act3;
         if (ensure_act3(e, max_rows)) return B200_ERR_CUDA;
@@ -420,11 +408,9 @@ extern "C" int b200_load_dist_weights(b200_engine *e, const float *w, int atoms)
     if (e->cfg.eval_kind == B200_EVAL_NET_FP16) return fail(B200_ERR_BAD_ARG, "eval_kind net_fp16 has no distributional network");
     CK(cudaSetDevice(e->cfg.device));
     if (e->A.mode == MODE_DIST && atoms != e->A.dist_bins) return fail(B200_ERR_BAD_ARG, "atoms must equal dist_bins");
-#ifdef B200_WITH_TC
     if (e->cfg.eval_kind == B200_EVAL_NET_TC && !dn_tc_weights_fit(w))
         return fail(B200_ERR_BAD_ARG, "net_tc: a conv or fc1 weight is non-finite or has |w| * 64 > 65504, which overflows the tensor cores' "
                                       "fp16 x 2 operand split (eval_kind net takes finite weights of any size)");
-#endif
     std::vector<float> h;
     dn_relayout(w, atoms, h);
     if (!e->d_dnw) { if (dalloc(e, &e->d_dnw, h.size(), false)) return B200_ERR_CUDA; }
@@ -433,9 +419,7 @@ extern "C" int b200_load_dist_weights(b200_engine *e, const float *w, int atoms)
     e->DW = dn_pointers(e->d_dnw, atoms);
     CK(cudaFuncSetAttribute(k_dn_conv, cudaFuncAttributeMaxDynamicSharedMemorySize, DN_CONV_SMEM));
     CK(cudaFuncSetAttribute(k_dn_fc, cudaFuncAttributeMaxDynamicSharedMemorySize, DN_FC_SMEM));
-#ifdef B200_WITH_TC
     if (dn_tc_prepare(&e->dn_tc_state, w, atoms, e->stream)) return fail(B200_ERR_CUDA, "tensor-core weight preparation (distributional network) failed");
-#endif
     e->have_dist_weights = true;
     drop_step_graph(e);
     return B200_OK;
@@ -443,7 +427,6 @@ extern "C" int b200_load_dist_weights(b200_engine *e, const float *w, int atoms)
 
 static int launch_distnet_on(b200_engine *e, const uint2 *req, const int32_t *n_req, const uint32_t *keys, int M, float *out, size_t max_rows) {
     if (!e->have_dist_weights) return fail(B200_ERR_NO_WEIGHTS, "b200_load_dist_weights was not called");
-#ifdef B200_WITH_TC
     if (e->cfg.eval_kind == B200_EVAL_NET_TC) {
         DnTcState *st = (DnTcState *)e->dn_tc_state;
         bool moved = false;
@@ -460,7 +443,6 @@ static int launch_distnet_on(b200_engine *e, const uint2 *req, const int32_t *n_
         CK(cudaGetLastError());
         return B200_OK;
     }
-#endif
     if (e->dn_rows < max_rows) {
         const bool had = e->d_dn_act != nullptr;
         if (had) { cudaStreamSynchronize(e->stream); dfree(e, e->d_dn_act); e->d_dn_act = nullptr; e->dn_rows = 0; }
@@ -548,7 +530,6 @@ extern "C" int b200_set_path_cache(b200_engine *e, int on) {
     if (on) {
         if (e->A.mode != MODE_LP) return fail(B200_ERR_BAD_ARG, "the path cache serves B200_MODE_LP (its coherence rules rest on the LP backup)");
         if (e->A.M > PC_MAX_NODES) return fail(B200_ERR_BAD_ARG, "the path cache needs max_nodes <= 65536 (k_backup's bitmap of the trace's observations)");
-        if (B200_FUSED_BACKUP) return fail(B200_ERR_BAD_ARG, "the path cache needs the separate k_backup launch (B200_FUSED_BACKUP=0)");
     }
     CK(cudaStreamSynchronize(e->stream));
     drop_step_graph(e);
@@ -629,14 +610,9 @@ extern "C" int b200_get_games(b200_engine *e, uint32_t *recs) {
 
 // ---------------------------------------------------------------------------------------------------- simulations
 static bool deep_lane_on(const b200_engine *e) {
-#ifdef B200_WITH_TC
-    return e->deep_cap > 0 && (e->A.mode == MODE_LP || e->A.mode == MODE_SINGLE) && tc_net(e) && !B200_FUSED_BACKUP;
-#else
-    return false;
-#endif
+    return e->deep_cap > 0 && (e->A.mode == MODE_LP || e->A.mode == MODE_SINGLE) && tc_net(e);
 }
 
-#ifdef B200_WITH_TC
 // The step with the deep lane: the deepest games (k_classify, once per move) walk on stream1 while the others walk, collect AND run their
 // network launch on the engine's stream; the lanes join, the deep lane's requests go behind the others' (k_merge_requests), a second, small
 // k_tc_conv evaluates them, and k_tc_fc / k_backup work on all of them as before.  With phase timing on everything runs on one stream
@@ -662,8 +638,8 @@ static int enqueue_step_lanes(b200_engine *e) {
     const int deep_groups = blocks_groups(e->deep_cap);
     {
         PhaseTimer t(e, PH_SELECT);
-        k_select_expand<<<(G + SE_GAMES_PER_BLOCK - 1) / SE_GAMES_PER_BLOCK, TPB, 0, s0>>>(A0);
-        k_select_expand<<<(e->deep_cap + SE_GAMES_PER_BLOCK - 1) / SE_GAMES_PER_BLOCK, TPB, 0, s1>>>(A1);
+        k_select_expand<<<(G + GROUPS_PER_BLOCK - 1) / GROUPS_PER_BLOCK, TPB, 0, s0>>>(A0);
+        k_select_expand<<<(e->deep_cap + GROUPS_PER_BLOCK - 1) / GROUPS_PER_BLOCK, TPB, 0, s1>>>(A1);
     }
     {
         PhaseTimer t(e, PH_GC);
@@ -694,21 +670,18 @@ static int enqueue_step_lanes(b200_engine *e) {
     CK(cudaGetLastError());
     return B200_OK;
 }
-#endif
 
 // One simulation step of every game: select+expand -> (collect garbage, resume) -> evaluate -> backup.
 static int enqueue_step(b200_engine *e) {
     const Arena &A = e->A;
     const int G = A.G;
-#ifdef B200_WITH_TC
     if (deep_lane_on(e)) return enqueue_step_lanes(e);
-#endif
     CK(cudaMemsetAsync(A.n_req, 0, 2 * sizeof(int32_t), e->stream));
     {
         PhaseTimer t(e, PH_SELECT);
         Arena Ap = A;
         Ap.prof = e->timing ? A.counters + 32 : nullptr;
-        k_select_expand<<<(G + SE_GAMES_PER_BLOCK - 1) / SE_GAMES_PER_BLOCK, TPB, 0, e->stream>>>(Ap);
+        k_select_expand<<<(G + GROUPS_PER_BLOCK - 1) / GROUPS_PER_BLOCK, TPB, 0, e->stream>>>(Ap);
     }
     {   // remove_nodes for the games that ran out of free slots in this step, then the rest of their expansion
         PhaseTimer t(e, PH_GC);
@@ -733,7 +706,7 @@ static int enqueue_step(b200_engine *e) {
         int rc = launch_net(e, A.req, A.n_req, A.key, A.M, A.eval_out, (size_t)G * (A.mode == MODE_LP ? 7 : 1));
         if (rc) return rc;
     }
-    if (A.mode == MODE_DIST || !B200_FUSED_BACKUP) {   // otherwise the next k_select_expand (or run_sims' final k_backup) folds this step's traces
+    {
         PhaseTimer t(e, PH_BACKUP);
         if (A.mode == MODE_DIST) k_dist_backup<<<(G + 3) / 4, 128, 0, e->stream>>>(A);
         else k_backup<<<(G + 3) / 4, 128, backup_smem(A), e->stream>>>(A, backup_bitmap_words(A));
@@ -778,10 +751,6 @@ extern "C" int b200_run_sims(b200_engine *e, int sims) {
         int rc = enqueue_step(e);
         if (rc) return rc;
         if (!e->timing && !e->step_exec && !e->step_graph_failed) capture_step(e);
-    }
-    if (B200_FUSED_BACKUP && A.mode != MODE_DIST && sims > 0) {   // the last simulation's traces (the others were folded by the next step's k_select_expand)
-        PhaseTimer t(e, PH_BACKUP);
-        k_backup<<<(A.G + 3) / 4, 128, backup_smem(A), e->stream>>>(A, backup_bitmap_words(A));
     }
     CK(cudaGetLastError());
     return B200_OK;
@@ -868,18 +837,10 @@ extern "C" int b200_debug_prof(b200_engine *e, uint64_t *out16) {   // clock64 p
     return B200_OK;
 }
 
-extern "C" int b200_debug_prof_tree(b200_engine *e, uint64_t *out16) {   // clock64 sums of sampled groups of k_select_expand (timing mode); 8..11: per-level split (B200_SELECT_PROF builds)
+extern "C" int b200_debug_prof_tree(b200_engine *e, uint64_t *out16) {   // clock64 sums of sampled groups of k_select_expand (timing mode)
     if (!e || !out16) return fail(B200_ERR_BAD_ARG, "null argument");
     CK(cudaSetDevice(e->cfg.device));
     CK(cudaMemcpyAsync(out16, e->A.counters + 32, 16 * 8, cudaMemcpyDeviceToHost, e->stream));
-    CK(cudaStreamSynchronize(e->stream));
-    return B200_OK;
-}
-
-extern "C" int b200_debug_trace_lens(b200_engine *e, int32_t *out) {   // development aid: trace length of every game's last simulation
-    if (!e || !out) return fail(B200_ERR_BAD_ARG, "null argument");
-    CK(cudaSetDevice(e->cfg.device));
-    CK(cudaMemcpyAsync(out, e->A.trace_len, (size_t)e->A.G * 4, cudaMemcpyDeviceToHost, e->stream));
     CK(cudaStreamSynchronize(e->stream));
     return B200_OK;
 }
@@ -1024,7 +985,6 @@ extern "C" int b200_debug_act3(b200_engine *e, const int8_t *states, int k, floa
     std::vector<float> v(k), var(k);
     int rc = b200_valuenet_forward(e, states, k, v.data(), var.data());   // leaves act3 of these k boards in the scratch buffers
     if (rc) return rc;
-#ifdef B200_WITH_TC
     if (tc_net(e)) {
         TcState *st = (TcState *)e->tc_state;
         const int planes = e->cfg.eval_kind == B200_EVAL_NET_FP16 ? 1 : 2;   // net_fp16 writes the first term only
@@ -1044,7 +1004,6 @@ extern "C" int b200_debug_act3(b200_engine *e, const int8_t *states, int k, floa
             }
         return B200_OK;
     }
-#endif
     std::vector<float> h((size_t)k * 1792);
     CK(cudaMemcpy(h.data(), e->d_act3, h.size() * 4, cudaMemcpyDeviceToHost));
     for (int r = 0; r < k; ++r)
