@@ -37,13 +37,21 @@ enum { B200_EVAL_SYNTHETIC = 0, /* test evaluator (hash of the observation), sha
        B200_EVAL_NET = 1,       /* model/model_vv.py Model_VV.inference, fp32 CUDA cores */
        B200_EVAL_NET_TC = 2,    /* same network on wgmma tensor cores (fp16 x 2 operand split, 3 products per product); in B200_MODE_DIST:
                                    model/model_distributional.py on tensor cores (csrc/distnet_tc.cuh) instead of the fp32 CUDA-core kernels */
-       B200_EVAL_NET_FP16 = 3 };/* same weights and tensor-core kernels as B200_EVAL_NET_TC with ONE fp16 term per operand and one product per
+       B200_EVAL_NET_FP16 = 3,  /* same weights and tensor-core kernels as B200_EVAL_NET_TC with ONE fp16 term per operand and one product per
                                    product (about 1/3 of the MMA work).  Every activation and conv / fc1 weight is rounded to fp16 (2^-11
                                    relative) instead of split (2^-22), so outputs are NOT within 1e-5 of Model_VV: DESIGN §5 states
                                    the bounds (act3 per element within 2^-10 of the board's largest |term| sum, v and var within
                                    2^-11 relative plus two ill-conditioned cases); the search on those outputs is exact.  Same weight
                                    limits as B200_EVAL_NET_TC.  Not available in B200_MODE_DIST (b200_engine_create returns
                                    B200_ERR_BAD_ARG) nor for b200_load_dist_weights. */
+       B200_EVAL_DIST_FP16 = 4 };/* model/model_distributional.py on the tensor-core kernels of B200_EVAL_NET_TC in B200_MODE_DIST, with ONE
+                                   fp16 term per operand and one product per product (about 1/3 of the MMA work).  Every conv activation
+                                   and conv / fc1 weight is rounded to fp16 (2^-11 relative), so the probabilities are NOT within 1e-5 of
+                                   the fp32 network: DESIGN §5 states the bounds (act2 per element within 2^-10 of the board's largest
+                                   |term| sum plus a floor, probabilities within 2 e_z p); the search on those outputs is exact.  Valid
+                                   only in B200_MODE_DIST (b200_engine_create returns B200_ERR_BAD_ARG otherwise: net_fp16 is the value
+                                   network's one-term kind); b200_load_weights returns B200_ERR_BAD_ARG (no value network);
+                                   b200_load_dist_weights takes the weight limits of B200_EVAL_NET_TC. */
 
 typedef struct b200_engine b200_engine;
 
@@ -86,7 +94,7 @@ int b200_engine_get_stream(b200_engine *e, void **cuda_stream_out);
 /* --- Model.load (model/model.py:163-174): weights = the state_dict tensors concatenated (B200_N_WEIGHTS floats).
  *     A B200_EVAL_NET_TC or B200_EVAL_NET_FP16 engine returns B200_ERR_BAD_ARG, keeping its previous weights, when a conv or fc1 weight
  *     is non-finite or has |w| * 64 > 65504 (fp16 overflow in the tensor cores' scaled operands); the same holds for
- *     b200_load_dist_weights (B200_EVAL_NET_TC). */
+ *     b200_load_dist_weights (B200_EVAL_NET_TC, B200_EVAL_DIST_FP16). */
 int b200_load_weights(b200_engine *e, const float *weights);
 
 /* --- TreeAgent.update_root (agents/agent.py:296-301) for all games: recs[n_games][20] */
@@ -185,6 +193,9 @@ int b200_dist_backup_trace(const int32_t *trace, int D, float *node_stats, float
  *     the 20x10 observation gets two empty rows on top). */
 int b200_load_dist_weights(b200_engine *e, const float *weights, int atoms);
 int b200_distnet_forward(b200_engine *e, const int8_t *states, int k, int atoms, float *dist);
+/* test aid: the conv stack's output of the tensor-core distributional network (B200_EVAL_NET_TC or B200_EVAL_DIST_FP16; other kinds
+ * return B200_ERR_BAD_ARG) on states[k][200]: out[k][2048] in torch flatten order c*64 + y*4 + x, as the tensor cores' fp16 operands hold it */
+int b200_debug_dist_act2(b200_engine *e, const int8_t *states, int k, float *out);
 int b200_export_dist(b200_engine *e, int game, float *node_stats /* [M][5] */, float *node_dist /* [M][bins] */);
 
 /* --- replay samples of the live search (ValueSim.store_nodes, agents/ValueSim.py:122-159): observations with

@@ -14,7 +14,7 @@ N_ACTIONS = 7
 N_WEIGHTS = 478342
 
 MODE_LP, MODE_SINGLE, MODE_VANILLA, MODE_DIST = 0, 1, 2, 3
-EVAL_SYNTHETIC, EVAL_NET, EVAL_NET_TC, EVAL_NET_FP16 = 0, 1, 2, 3
+EVAL_SYNTHETIC, EVAL_NET, EVAL_NET_TC, EVAL_NET_FP16, EVAL_DIST_FP16 = 0, 1, 2, 3, 4
 ERR_NAMES = {1: "BAD_ARG", 2: "CUDA", 3: "ARENA_FULL", 4: "TRACE_FULL", 5: "NO_WEIGHTS"}
 
 
@@ -92,6 +92,7 @@ def lib():
         L.b200_replay_append_dev.argtypes = [P, P, C.c_int]
         L.b200_load_dist_weights.argtypes = [P, P, C.c_int]
         L.b200_distnet_forward.argtypes = [P, P, C.c_int, C.c_int, P]
+        L.b200_debug_dist_act2.argtypes = [P, P, C.c_int, P]
         L.b200_export_dist.argtypes = [P, C.c_int, P, P]
         L.b200_dist_shift_distribution.argtypes = [P, C.c_int, C.c_double, C.c_double, C.c_double, P]
         L.b200_dist_mean_variance.argtypes = [P, C.c_int, C.c_double, C.c_double, P, P]

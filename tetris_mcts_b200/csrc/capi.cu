@@ -181,6 +181,9 @@ extern "C" int b200_engine_create(const b200_config *cfg, b200_engine **out) {
         return fail(B200_ERR_BAD_ARG, "distributional mode needs 2 <= dist_bins <= 64 and dist_vmax > dist_vmin");
     if (cfg->mode == MODE_DIST && cfg->eval_kind == B200_EVAL_NET_FP16)
         return fail(B200_ERR_BAD_ARG, "eval_kind net_fp16 has no distributional network: use net_tc or net in B200_MODE_DIST");
+    if (cfg->mode != MODE_DIST && cfg->eval_kind == B200_EVAL_DIST_FP16)
+        return fail(B200_ERR_BAD_ARG, "eval_kind dist_fp16 is the distributional network's one-term form and needs B200_MODE_DIST: "
+                                      "use net_fp16 for the value network");
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail(B200_ERR_CUDA, "no CUDA device: this library has no CPU path");
     CK(cudaSetDevice(cfg->device));
@@ -301,6 +304,7 @@ static decltype(&k_tc_fc<2>) tc_fc_kernel(const b200_engine *e) { return e->cfg.
 
 extern "C" int b200_load_weights(b200_engine *e, const float *w) {
     if (!e || !w) return fail(B200_ERR_BAD_ARG, "null argument");
+    if (e->cfg.eval_kind == B200_EVAL_DIST_FP16) return fail(B200_ERR_BAD_ARG, "eval_kind dist_fp16 has no value network (use net_fp16)");
     if (tc_net(e) && !tc_weights_fit(w))
         return fail(B200_ERR_BAD_ARG, e->cfg.eval_kind == B200_EVAL_NET_TC
                     ? "net_tc: a conv or fc1 weight is non-finite or has |w| * 64 > 65504, which overflows the tensor cores' "
@@ -403,6 +407,9 @@ static int launch_net(b200_engine *e, const uint2 *req, const int32_t *n_req, co
 // ---------------------------------------------------------------------------------------------------- distributional network
 __global__ void k_states_to_keys(const int8_t *states, int k, uint32_t *keys, uint2 *req);   // defined with the standalone value net below
 
+// net_tc and dist_fp16 run the same tensor-core distributional kernels and weight layout, with two fp16 terms per operand or one (distnet_tc.cuh)
+static bool dn_tc_net(const b200_engine *e) { return e->cfg.eval_kind == B200_EVAL_NET_TC || e->cfg.eval_kind == B200_EVAL_DIST_FP16; }
+
 extern "C" int b200_load_dist_weights(b200_engine *e, const float *w, int atoms) {
     if (!e || !w || atoms < 2 || atoms > 64) return fail(B200_ERR_BAD_ARG, "bad argument");
     if (e->cfg.eval_kind == B200_EVAL_NET_FP16) return fail(B200_ERR_BAD_ARG, "eval_kind net_fp16 has no distributional network");
@@ -411,6 +418,9 @@ extern "C" int b200_load_dist_weights(b200_engine *e, const float *w, int atoms)
     if (e->cfg.eval_kind == B200_EVAL_NET_TC && !dn_tc_weights_fit(w))
         return fail(B200_ERR_BAD_ARG, "net_tc: a conv or fc1 weight is non-finite or has |w| * 64 > 65504, which overflows the tensor cores' "
                                       "fp16 x 2 operand split (eval_kind net takes finite weights of any size)");
+    if (e->cfg.eval_kind == B200_EVAL_DIST_FP16 && !dn_tc_weights_fit(w))
+        return fail(B200_ERR_BAD_ARG, "dist_fp16: a conv or fc1 weight is non-finite or has |w| * 64 > 65504, which overflows the tensor cores' "
+                                      "scaled fp16 operands (eval_kind net takes finite weights of any size)");
     std::vector<float> h;
     dn_relayout(w, atoms, h);
     if (!e->d_dnw) { if (dalloc(e, &e->d_dnw, h.size(), false)) return B200_ERR_CUDA; }
@@ -427,18 +437,20 @@ extern "C" int b200_load_dist_weights(b200_engine *e, const float *w, int atoms)
 
 static int launch_distnet_on(b200_engine *e, const uint2 *req, const int32_t *n_req, const uint32_t *keys, int M, float *out, size_t max_rows) {
     if (!e->have_dist_weights) return fail(B200_ERR_NO_WEIGHTS, "b200_load_dist_weights was not called");
-    if (e->cfg.eval_kind == B200_EVAL_NET_TC) {
+    if (dn_tc_net(e)) {
         DnTcState *st = (DnTcState *)e->dn_tc_state;
         bool moved = false;
         if (dn_tc_ensure_act2(st, max_rows, e->stream, &moved)) return fail(B200_ERR_CUDA, "act2 (tensor-core layout) allocation failed");
         if (moved) drop_step_graph(e);
+        const bool one = e->cfg.eval_kind == B200_EVAL_DIST_FP16;
         {
             PhaseTimer t(e, PH_CONV);
-            k_tdc_conv<<<e->n_sm, TDC_THREADS, TDC_SMEM, e->stream>>>(e->DW, st->TW, req, n_req, keys, M, st->d_act2, (int)st->tiles);
+            (one ? k_tdc_conv<1> : k_tdc_conv<2>)<<<e->n_sm, TDC_THREADS, TDC_SMEM, e->stream>>>(e->DW, st->TW, req, n_req, keys, M, st->d_act2,
+                                                                                               (int)st->tiles);
         }
         {
             PhaseTimer t(e, PH_FC);
-            k_tdc_fc<<<e->n_sm, TDF_THREADS, TDF_SMEM, e->stream>>>(e->DW, st->TW, st->d_act2, (int)st->tiles, req, n_req, out);
+            (one ? k_tdc_fc<1> : k_tdc_fc<2>)<<<e->n_sm, TDF_THREADS, TDF_SMEM, e->stream>>>(e->DW, st->TW, st->d_act2, (int)st->tiles, req, n_req, out);
         }
         CK(cudaGetLastError());
         return B200_OK;
@@ -1010,6 +1022,34 @@ extern "C" int b200_debug_act3(b200_engine *e, const int8_t *states, int k, floa
         for (int y = 0; y < 14; ++y)
             for (int c = 0; c < 32; ++c)
                 for (int x = 0; x < 4; ++x) out[(size_t)r * 1792 + c * 56 + y * 4 + x] = h[(size_t)r * 1792 + (y * 32 + c) * 4 + x];
+    return B200_OK;
+}
+
+// development / test aid: the distributional conv stack's output (flatten input of fc1) in torch order c*64 + y*4 + x, read back from the
+// tensor-core kernels' act2 (net_tc: both fp16 terms, dist_fp16: the one it writes)
+extern "C" int b200_debug_dist_act2(b200_engine *e, const int8_t *states, int k, float *out) {
+    if (!e || !states || !out || k < 1) return fail(B200_ERR_BAD_ARG, "bad argument");
+    if (!dn_tc_net(e)) return fail(B200_ERR_BAD_ARG, "b200_debug_dist_act2 reads the tensor-core distributional network: eval_kind net_tc or dist_fp16");
+    if (!e->have_dist_weights) return fail(B200_ERR_NO_WEIGHTS, "b200_load_dist_weights was not called");
+    std::vector<float> dist((size_t)k * e->DW.atoms);
+    int rc = b200_distnet_forward(e, states, k, e->DW.atoms, dist.data());   // leaves act2 of these k boards in the scratch buffer
+    if (rc) return rc;
+    DnTcState *st = (DnTcState *)e->dn_tc_state;
+    const int planes = e->cfg.eval_kind == B200_EVAL_DIST_FP16 ? 1 : 2;
+    size_t bytes = (size_t)2 * st->tiles * DACT2_KCHUNKS * 2048;
+    std::vector<uint8_t> h(bytes);
+    CK(cudaMemcpy(h.data(), st->d_act2, bytes, cudaMemcpyDeviceToHost));
+    for (int r = 0; r < k; ++r)
+        for (int kp = 0; kp < 2048; ++kp) {
+            int p = kp >> 5, c = kp & 31;
+            float sum = 0.f;
+            for (int s = planes - 1; s >= 0; --s) {
+                size_t off = ((((size_t)s * st->tiles + (r >> 7)) * DACT2_KCHUNKS + (kp >> 3)) * 128 + (r & 127)) * 16 + (kp & 7) * 2;
+                uint16_t hb; memcpy(&hb, &h[off], 2);
+                sum += host_half_f(hb);
+            }
+            out[(size_t)r * 2048 + c * 64 + p] = sum / TC_SCALE_A;
+        }
     return B200_OK;
 }
 

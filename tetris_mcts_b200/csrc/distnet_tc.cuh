@@ -9,6 +9,12 @@
 //               LeakyReLU(0.01), re-splits and writes act2 (16x4 pixels x 32 channels = 2048 per board) to HBM in k_tdc_fc's tile layout.
 //   k_tdc_fc    [R,2048] x [2048,128] like k_tc_fc (1-D TMA ring, producer warp + two consumer warpgroups); epilogue: bias + LeakyReLU ->
 //               shared memory -> fc_v (128 x atoms, CUDA cores, one thread per board) -> softmax (model_distributional.py:47-50) -> dist[game][atoms].
+//
+// Both kernels take the number of fp16 terms per operand, NT, as a template argument, as k_tc_conv / k_tc_fc do.  NT = 2 is the split
+// above (eval_kind net_tc).  NT = 1 (eval_kind dist_fp16) keeps only x1 of every activation and conv / fc1 weight and issues the single
+// product a1*b1: conv1 runs at N = 32 (the second weight term is no longer stacked along N), conv2 issues 8 wgmma per tile instead of 24,
+// fc1 one per k16 block instead of three, the epilogues round to one fp16, and act2 in HBM is one plane (4096 B per board).  Same scaling,
+// same layouts (the x2 slots stay allocated and are not read); fc_v and the softmax stay fp32.
 #pragma once
 #include "valuenet_tc.cuh"
 #include "distnet_simt.cuh"
@@ -35,6 +41,13 @@ constexpr int TDC_SMEM = TDC_OFF_KEY + TDC_WGS * 32 * 4;
 constexpr int DACT2_KCHUNKS = 256;               // 2048 / 8
 static_assert(TDC_SMEM <= 227 * 1024, "k_tdc_conv shared memory");
 
+// MMA work issued per board, in n-units of TC_NUNIT_FLOP (one column of an m64 k16 wgmma).  NT = 2 / NT = 1:
+//   conv1  3 tiles x N = 64 / 32;  conv2  2 tiles x (24 / 8) x N = 128
+// fc1 issues 2048 x 128 x 2 FLOP per board per product (3 / 1 products).  scripts/dist_kind_bench.py reads these three lines.
+constexpr int TDC_CONV_NUNITS_NT2 = 3 * 64 + 2 * 24 * 128;   // 6336 -> 12.98 MFLOP per board
+constexpr int TDC_CONV_NUNITS_NT1 = 3 * 32 + 2 * 8 * 128;    // 2144 -> 4.39 MFLOP per board
+constexpr int TDF_FLOP_PER_PRODUCT = 2048 * 128 * 2;          // x3 -> 1.57 MFLOP, x1 -> 0.52 MFLOP per board
+
 struct DnTcWeights {
     const uint8_t *wc1;   // TDC_W1BYTES
     const uint8_t *wc2;   // TDC_WBYTES, already in the shared-memory layout
@@ -47,6 +60,8 @@ __device__ __forceinline__ size_t dact2_off(int split, int n_tiles, int ridx, in
 }
 
 // conv2 on one 64-row tile = 24 wgmma of N = 128: for each (dy, channel half): a1*W1, a1*W2, a2*W1 into the same 128 columns
+// (NT = 1: a1*W1 only, 8 wgmma)
+template <int NT>
 __device__ __forceinline__ void issue_dconv2(float (&d)[64], uint32_t a_addr, uint32_t w_addr) {
     const uint64_t a0 = gmma_desc(a_addr, TDC_R * 16, 128), b0 = gmma_desc(w_addr, 128 * 16, 128);
 #pragma unroll
@@ -56,12 +71,15 @@ __device__ __forceinline__ void issue_dconv2(float (&d)[64], uint32_t a_addr, ui
             const uint32_t a_hi = 2 * h * TDC_R + dy * 8, a_lo = a_hi + 4 * TDC_R;          // 16-byte units
             const uint32_t b_hi = (dy * 2 + h) * (TDC_WBLOCK / 16), b_lo = b_hi + 2 * 128;
             wgmma_n128(d, a0 + a_hi, b0 + b_hi, (dy | h) ? 1u : 0u);
-            wgmma_n128(d, a0 + a_hi, b0 + b_lo, 1u);
-            wgmma_n128(d, a0 + a_lo, b0 + b_hi, 1u);
+            if (NT == 2) {
+                wgmma_n128(d, a0 + a_hi, b0 + b_lo, 1u);
+                wgmma_n128(d, a0 + a_lo, b0 + b_hi, 1u);
+            }
         }
     }
 }
 
+template <int NT>
 __global__ void __launch_bounds__(TDC_THREADS, 1)
 k_tdc_conv(DistNetWeights W, DnTcWeights TW, const uint2 *req, const int32_t *n_req_ptr, const uint32_t *keys, int M, uint8_t *act2, int n_tiles) {
     extern __shared__ __align__(128) uint8_t smem[];
@@ -128,13 +146,16 @@ k_tdc_conv(DistNetWeights W, DnTcWeights TW, const uint2 *req, const int32_t *n_
         fence_async_smem();
         wg_sync(wg);
         // ---- conv1 (model_distributional.py:20): im2col [192 x 16] x W1 [16 x 64], three 64-row tiles; epilogue: bias + LeakyReLU + split -> act1
+        // (NT = 1: x W1 [16 x 32], the first weight term only; the epilogue rounds to one fp16)
 #pragma unroll 1
         for (int mt = 0; mt < 3; ++mt) {
-            float d[32];
+            float d[16 * NT];
 #pragma unroll
-            for (int k = 0; k < 32; ++k) d[k] = 0.f;
+            for (int k = 0; k < 16 * NT; ++k) d[k] = 0.f;
             wgmma_fence();
-            wgmma_n64(d, gmma_desc(s_im + mt * 1024, TDC_IMROWS * 16, 128), gmma_desc(s_w1, 64 * 16, 128), 0u);
+            const uint64_t ad = gmma_desc(s_im + mt * 1024, TDC_IMROWS * 16, 128), bd = gmma_desc(s_w1, 64 * 16, 128);
+            if constexpr (NT == 2) wgmma_n64(d, ad, bd, 0u);
+            else wgmma_n32(d, ad, bd, 0u);                       // cout 0..31 of each k chunk: the first weight term
             wgmma_commit();
             wgmma_wait<0>();
             fence_regs(d);
@@ -145,13 +166,19 @@ k_tdc_conv(DistNetWeights W, DnTcWeights TW, const uint2 *req, const int32_t *n_
 #pragma unroll
                     for (int j = 0; j < 4; ++j) {
                         const int c = 8 * j + 2 * qd;
-                        const float o0 = leaky(fmaf(d[4 * (j + 4) + 2 * h] + d[4 * j + 2 * h], K1, sB[c]));
-                        const float o1 = leaky(fmaf(d[4 * (j + 4) + 2 * h + 1] + d[4 * j + 2 * h + 1], K1, sB[c + 1]));
-                        uint32_t hi, lo;
-                        split2(o0, o1, hi, lo);
                         uint8_t *dst = act + (j * TDC_R + r) * 16 + qd * 4;
-                        *reinterpret_cast<uint32_t *>(dst) = hi;
-                        *reinterpret_cast<uint32_t *>(dst + SPLIT) = lo;
+                        if constexpr (NT == 2) {
+                            const float o0 = leaky(fmaf(d[4 * (j + 4) + 2 * h] + d[4 * j + 2 * h], K1, sB[c]));
+                            const float o1 = leaky(fmaf(d[4 * (j + 4) + 2 * h + 1] + d[4 * j + 2 * h + 1], K1, sB[c + 1]));
+                            uint32_t hi, lo;
+                            split2(o0, o1, hi, lo);
+                            *reinterpret_cast<uint32_t *>(dst) = hi;
+                            *reinterpret_cast<uint32_t *>(dst + SPLIT) = lo;
+                        } else {
+                            const float o0 = leaky(fmaf(d[4 * j + 2 * h], K1, sB[c]));
+                            const float o1 = leaky(fmaf(d[4 * j + 2 * h + 1], K1, sB[c + 1]));
+                            *reinterpret_cast<uint32_t *>(dst) = round1(o0, o1);
+                        }
                     }
                 }
             }
@@ -165,7 +192,7 @@ k_tdc_conv(DistNetWeights W, DnTcWeights TW, const uint2 *req, const int32_t *n_
 #pragma unroll
             for (int k = 0; k < 64; ++k) d[k] = 0.f;
             wgmma_fence();
-            issue_dconv2(d, s_act + mt * 1024, s_w2);
+            issue_dconv2<NT>(d, s_act + mt * 1024, s_w2);
             wgmma_commit();
             wgmma_wait<0>();
             fence_regs(d);
@@ -182,12 +209,17 @@ k_tdc_conv(DistNetWeights W, DnTcWeights TW, const uint2 *req, const int32_t *n_
                                     s3 = __shfl_down_sync(0xffffffffu, d[48 + k], 12);
                         o[e] = leaky(fmaf(((s3 + s2) + s1) + d[k], K2, sB[32 + 8 * j + 2 * qd + e]));
                     }
-                    uint32_t hi, lo;
-                    split2(o[0], o[1], hi, lo);
-                    if (x < 4) {
-                        const int kc = (y * 4 + x) * 4 + j;
-                        *reinterpret_cast<uint32_t *>(act2 + dact2_off(0, n_tiles, ridx, kc) + qd * 4) = hi;
-                        *reinterpret_cast<uint32_t *>(act2 + dact2_off(1, n_tiles, ridx, kc) + qd * 4) = lo;
+                    if constexpr (NT == 2) {
+                        uint32_t hi, lo;
+                        split2(o[0], o[1], hi, lo);
+                        if (x < 4) {
+                            const int kc = (y * 4 + x) * 4 + j;
+                            *reinterpret_cast<uint32_t *>(act2 + dact2_off(0, n_tiles, ridx, kc) + qd * 4) = hi;
+                            *reinterpret_cast<uint32_t *>(act2 + dact2_off(1, n_tiles, ridx, kc) + qd * 4) = lo;
+                        }
+                    } else {
+                        const uint32_t hi = round1(o[0], o[1]);
+                        if (x < 4) *reinterpret_cast<uint32_t *>(act2 + dact2_off(0, n_tiles, ridx, (y * 4 + x) * 4 + j) + qd * 4) = hi;
                     }
                 }
             }
@@ -212,6 +244,7 @@ static_assert(2 * TDF_STAGES * 8 <= 256, "barrier block overflows into the epilo
 constexpr int TDF_SMEM = TDF_OFF_EPI + (128 + 128 * TDF_ATOMS + TDF_ATOMS + TDF_CONSUMERS * 64 * TDF_HSTRIDE) * 4;
 static_assert(TDF_SMEM <= 227 * 1024, "k_tdc_fc shared memory");
 
+template <int NT>
 __global__ void __launch_bounds__(TDF_THREADS, 1)
 k_tdc_fc(DistNetWeights W, DnTcWeights TW, const uint8_t *act2, int n_tiles_alloc, const uint2 *req, const int32_t *n_req_ptr, float *out) {
     extern __shared__ __align__(128) uint8_t smem[];
@@ -235,10 +268,10 @@ k_tdc_fc(DistNetWeights W, DnTcWeights TW, const uint8_t *act2, int n_tiles_allo
             for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
                 for (int j = 0; j < TDF_KBLOCKS; ++j) {
                     mbar_wait(&empty[stage], ph ^ 1);
-                    mbar_expect_tx(&full[stage], TDF_STAGE);
+                    mbar_expect_tx(&full[stage], NT * (TDF_A_BYTES + TDF_B_BYTES));
                     uint8_t *dst = smem + stage * TDF_STAGE;
 #pragma unroll
-                    for (int s = 0; s < 2; ++s) {
+                    for (int s = 0; s < NT; ++s) {               // NT = 1: the first term of each operand; its second-term slots stay unused
                         bulk_g2s(dst + s * TDF_A_BYTES, act2 + (((size_t)s * n_tiles_alloc + tile) * DACT2_KCHUNKS + 2 * j) * 2048, TDF_A_BYTES, &full[stage]);
                         bulk_g2s(dst + 2 * TDF_A_BYTES + s * TDF_B_BYTES, TW.wfc + ((size_t)s * TDF_KBLOCKS + j) * TDF_B_BYTES, TDF_B_BYTES, &full[stage]);
                     }
@@ -246,8 +279,9 @@ k_tdc_fc(DistNetWeights W, DnTcWeights TW, const uint8_t *act2, int n_tiles_allo
                 }
             }
         }
-    } else {   // ===== consumers: D[64 x 128] += A[64 x 16] * B[128 x 16]^T per warpgroup, three split terms per k block
+    } else {   // ===== consumers: D[64 x 128] += A[64 x 16] * B[128 x 16]^T per warpgroup, three split terms per k block (NT = 1: one)
         const int wg = t >> 7, wt = t & 127, w = warp & 3, qd = lane & 3, rl = lane >> 2;
+        constexpr int T0 = NT == 2 ? 0 : 2;              // first of the three products issued
         float *hrow = sH + wg * 64 * TDF_HSTRIDE;
         int stage = 0; uint32_t ph = 0;
         for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
@@ -260,11 +294,11 @@ k_tdc_fc(DistNetWeights W, DnTcWeights TW, const uint8_t *act2, int n_tiles_allo
                 const uint32_t sbase = smem_u32(smem + stage * TDF_STAGE);
                 wgmma_fence();
 #pragma unroll
-                for (int term = 0; term < 3; ++term) {   // a1*b2, a2*b1, a1*b1 (small terms first)
+                for (int term = T0; term < 3; ++term) {  // a1*b2, a2*b1, a1*b1 (small terms first); NT = 1: a1*b1
                     const int sa = term == 1 ? 1 : 0, sb = term == 0 ? 1 : 0;
                     const uint64_t ad = gmma_desc(sbase + sa * TDF_A_BYTES + wg * 1024, 128 * 16, 128);
                     const uint64_t bd = gmma_desc(sbase + 2 * TDF_A_BYTES + sb * TDF_B_BYTES, 128 * 16, 128);
-                    wgmma_n128(d, ad, bd, (j | term) ? 1u : 0u);
+                    wgmma_n128(d, ad, bd, (j > 0 || term > T0) ? 1u : 0u);
                 }
                 wgmma_commit();
                 wgmma_wait<1>();
@@ -323,7 +357,7 @@ struct DnTcState {
     uint8_t *d_act2 = nullptr; size_t tiles = 0;
 };
 
-// conv1, conv2 and fc1 go through the fp16 x 2 split (see tc_weights_fit); fc_v stays fp32
+// conv1, conv2 and fc1 go through the fp16 x 2 split, or one scaled fp16 term (see tc_weights_fit); fc_v stays fp32
 static bool dn_tc_weights_fit(const float *w) {
     const float *c1w = w, *c2w = c1w + 512 + 32, *f1w = c2w + 16384 + 32;
     return tc_split_fits(c1w, 512) && tc_split_fits(c2w, 16384) && tc_split_fits(f1w, (size_t)128 * 2048);
@@ -370,8 +404,10 @@ static int dn_tc_prepare(void **state, const float *w, int atoms, cudaStream_t s
     if (cudaMemcpyAsync(st->d_w, h.data(), h.size(), cudaMemcpyHostToDevice, stream) != cudaSuccess) return 1;
     if (cudaStreamSynchronize(stream) != cudaSuccess) return 1;
     st->TW.wc1 = st->d_w; st->TW.wc2 = st->d_w + TDC_W1BYTES; st->TW.wfc = st->TW.wc2 + TDC_WBYTES;
-    if (cudaFuncSetAttribute(k_tdc_conv, cudaFuncAttributeMaxDynamicSharedMemorySize, TDC_SMEM) != cudaSuccess) return 1;
-    if (cudaFuncSetAttribute(k_tdc_fc, cudaFuncAttributeMaxDynamicSharedMemorySize, TDF_SMEM) != cudaSuccess) return 1;
+    if (cudaFuncSetAttribute(k_tdc_conv<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, TDC_SMEM) != cudaSuccess) return 1;
+    if (cudaFuncSetAttribute(k_tdc_conv<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, TDC_SMEM) != cudaSuccess) return 1;
+    if (cudaFuncSetAttribute(k_tdc_fc<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, TDF_SMEM) != cudaSuccess) return 1;
+    if (cudaFuncSetAttribute(k_tdc_fc<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, TDF_SMEM) != cudaSuccess) return 1;
     return 0;
 }
 

@@ -19,7 +19,8 @@ class BatchedEngine:
                  stale_pop=True, rollout_variance=1e3, trace_max=512, overflow_reset=False, dist_bins=50, dist_vmin=0.0, dist_vmax=5000.0,
                  dist_weights=None, path_cache=None):
         mode_id = {"lp": L.MODE_LP, "single": L.MODE_SINGLE, "vanilla": L.MODE_VANILLA, "dist": L.MODE_DIST}[mode] if isinstance(mode, str) else int(mode)
-        eval_id = {"synthetic": L.EVAL_SYNTHETIC, "net": L.EVAL_NET, "net_tc": L.EVAL_NET_TC, "net_fp16": L.EVAL_NET_FP16}[eval_kind] if isinstance(eval_kind, str) else int(eval_kind)
+        eval_id = {"synthetic": L.EVAL_SYNTHETIC, "net": L.EVAL_NET, "net_tc": L.EVAL_NET_TC, "net_fp16": L.EVAL_NET_FP16,
+                   "dist_fp16": L.EVAL_DIST_FP16}[eval_kind] if isinstance(eval_kind, str) else int(eval_kind)
         if tuple(env_args[0]) != (20, 10):
             raise ValueError("only 20x10 boards (SPEC_PYTETRIS.md §1)")
         cfg = L.Config()
