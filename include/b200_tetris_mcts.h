@@ -196,6 +196,12 @@ int b200_distnet_forward(b200_engine *e, const int8_t *states, int k, int atoms,
 /* test aid: the conv stack's output of the tensor-core distributional network (B200_EVAL_NET_TC or B200_EVAL_DIST_FP16; other kinds
  * return B200_ERR_BAD_ARG) on states[k][200]: out[k][2048] in torch flatten order c*64 + y*4 + x, as the tensor cores' fp16 operands hold it */
 int b200_debug_dist_act2(b200_engine *e, const int8_t *states, int k, float *out);
+/* test aid: one layer of a tensor-core network exactly as the next layer reads it, from a forward pass on states[k][200].  dist = 0: the
+ * value network (B200_EVAL_NET_TC or B200_EVAL_NET_FP16), layer 1..3 = act1 [32][18][8], act2 [32][16][6], act3 [32][14][4]; dist = 1: the
+ * distributional network (B200_EVAL_NET_TC or B200_EVAL_DIST_FP16), layer 1..2 = act1 [32][19][7], act2 [32][16][4].  out[k][nt][...] holds
+ * fp16 term s < nt of each element divided by 16 (nt = 2 for net_tc, 1 for the fp16 kinds).  layer 0: the same pass's outputs, out[k][2]
+ * = (v, var) or out[k][atoms] = probabilities. */
+int b200_debug_tc_acts(b200_engine *e, int dist, const int8_t *states, int k, int layer, float *out);
 int b200_export_dist(b200_engine *e, int game, float *node_stats /* [M][5] */, float *node_dist /* [M][bins] */);
 
 /* --- replay samples of the live search (ValueSim.store_nodes, agents/ValueSim.py:122-159): observations with

@@ -33,6 +33,7 @@ import numpy as np
 import torch
 import torch.nn.functional as F
 
+import f16_ref as H
 import f64_ref as R
 
 ACT2_REL = 2.0 ** -10          # c 2^-11, c = 2
@@ -75,20 +76,47 @@ def prob_excess(got, ref, ez):
     return float(np.max(np.abs(np.asarray(got, np.float64) - ref) / (2 * ez * ref + 1e-36)))
 
 
-def _round(t, scale, dtype):
-    return (t * scale).to(dtype).to(torch.float64) / scale
+def _leaky_round(t, scale, dtype, rz=False):
+    """the epilogue on t * scale: fp32 rounding (the fma), x > 0 ? x : 0.01f * x in fp32, rounding to `dtype` (toward zero with rz);
+    over scale"""
+    s = (t * scale).to(torch.float32)
+    s = torch.where(s > 0, s, s * torch.tensor(0.01, dtype=torch.float32))
+    return (H._rz16(s) if rz else s.to(dtype).to(torch.float64)) / scale
+
+
+_round = H._round
+
+
+def emulate_layers(w, states, atoms, dtype=torch.float16, mutant=None):
+    """The conv stack of emulate: [act1, act2] as float64 tensors [n, 32, H, W] (each element an fp16 term / 16); mutant: one of
+    f16_ref.MUTANTS, as there."""
+    p = R.unpack(w, R.dn_shapes(atoms))
+    for k in R.SPLIT_DN:
+        p[k] = _round(p[k], 64.0, dtype, mutant == "rz_weight")
+    if mutant == "no_conv2_block":
+        p["conv2.weight"][:, :16, 0] = 0
+    sa = 8.0 if mutant == "scale8" else 16.0
+    a, out = _pad(states), []
+    with torch.no_grad():
+        for l in (1, 2):
+            wl, bl = p["conv%d.weight" % l], p["conv%d.bias" % l]
+            if mutant == "bias_after":
+                a = F.leaky_relu(_round(F.conv2d(a, wl), sa, dtype) + bl[None, :, None, None], 0.01)
+            else:
+                a = _leaky_round(F.conv2d(a, wl, bl), sa, dtype, mutant == "rz_act")
+            out.append(a)
+    return out
 
 
 def emulate(w, states, atoms, dtype=torch.float16):
-    """The dist_fp16 arithmetic in float64: every conv / fc1 weight (x64) and every conv activation (x16) rounded once to `dtype`
-    (torch.float16 as the device does; torch.bfloat16 to show that the act2 bound tells a coarser format apart), exact sums.
-    -> (probabilities, act2) like f64_ref.distnet and act2 above."""
+    """The dist_fp16 arithmetic in float64: every conv / fc1 weight (x64) and every conv activation (x16, after the epilogue's fp32
+    rounding and fp32 LeakyReLU) rounded once to `dtype` (torch.float16 as the device does; torch.bfloat16 to show that the act2 bound
+    tells a coarser format apart), exact sums.  -> (probabilities, act2) like f64_ref.distnet and act2 above."""
     p = R.unpack(w, R.dn_shapes(atoms))
     for k in R.SPLIT_DN:
         p[k] = _round(p[k], 64.0, dtype)
     with torch.no_grad():
-        a = _round(F.leaky_relu(F.conv2d(_pad(states), p["conv1.weight"], p["conv1.bias"]), 0.01), 16.0, dtype)
-        a2 = _round(F.leaky_relu(F.conv2d(a, p["conv2.weight"], p["conv2.bias"]), 0.01), 16.0, dtype).flatten(1)
+        a2 = emulate_layers(w, states, atoms, dtype)[-1].flatten(1)
         h = F.leaky_relu(a2 @ p["fc1.weight"].T + p["fc1.bias"], 0.01)
         probs = torch.softmax(h @ p["fc_v.weight"].T + p["fc_v.bias"], 1)
     return probs.numpy(), a2.numpy()

@@ -72,23 +72,56 @@ def out_excess(got, ref, sens):
     return float(np.max(np.abs(np.asarray(got, np.float64) - ref) / (OUT_RTOL * np.abs(ref) + sens)))
 
 
-def _round(t, scale, dtype):
-    return (t * scale).to(dtype).to(torch.float64) / scale
+def _rz16(t):
+    """float32 tensor -> its float16 neighbour toward zero (as float64)"""
+    x = t.numpy()
+    h = x.astype(np.float16)
+    over = np.abs(h.astype(np.float32)) > np.abs(x)
+    h[over] = np.nextafter(h[over], np.float16(0))
+    return torch.from_numpy(h.astype(np.float64))
+
+
+def _round(t, scale, dtype, rz=False):
+    """t * scale rounded to fp32 (the epilogue's fma; exact for the weights), then to `dtype` (toward zero with rz), over scale"""
+    s = (t * scale).to(torch.float32)
+    return (_rz16(s) if rz else s.to(dtype).to(torch.float64)) / scale
+
+
+# deliberate defects emulate_layers can apply, for the tests that show a check catches them
+MUTANTS = ("rz_act", "rz_weight", "bias_after", "scale8", "no_conv2_block")
+
+
+def emulate_layers(w, states, dtype=torch.float16, mutant=None):
+    """The conv stack of emulate: [act1, act2, act3] as float64 tensors [n, 32, H, W] (each element an fp16 term / 16).  mutant: one of
+    MUTANTS: activations rounded toward zero, weights rounded toward zero, each bias added after the rounding, activations scaled by 8
+    instead of 16, conv2 without its (dy = 0, input channels 0..15) block of products."""
+    p = R.unpack(w, R.VN_SHAPES)
+    for k in R.SPLIT_VN:
+        p[k] = _round(p[k], 64.0, dtype, mutant == "rz_weight")
+    if mutant == "no_conv2_block":
+        p["conv2.weight"][:, :16, 0] = 0
+    sa = 8.0 if mutant == "scale8" else 16.0
+    a, out = R._x(states, torch.float64), []
+    with torch.no_grad():
+        for l in (1, 2, 3):
+            wl, bl = p["conv%d.weight" % l], p["conv%d.bias" % l]
+            if mutant == "bias_after":
+                a = F.relu(_round(F.conv2d(a, wl), sa, dtype) + bl[None, :, None, None])
+            else:
+                a = F.relu(_round(F.conv2d(a, wl, bl), sa, dtype, mutant == "rz_act"))
+            out.append(a)
+    return out
 
 
 def emulate(w, states, dtype=torch.float16):
-    """The net_fp16 arithmetic in float64: every conv / fc1 weight (x64) and every conv activation (x16) rounded once to `dtype`
-    (torch.float16 as the device does; torch.bfloat16 to show that the bounds tell a coarser format apart), exact sums.
-    -> (v, var, act3) like f64_ref.valuenet."""
+    """The net_fp16 arithmetic in float64: every conv / fc1 weight (x64) and every conv activation (x16, after the epilogue's fp32
+    rounding) rounded once to `dtype` (torch.float16 as the device does; torch.bfloat16 to show that the bounds tell a coarser format
+    apart), exact sums.  -> (v, var, act3) like f64_ref.valuenet."""
     p = R.unpack(w, R.VN_SHAPES)
     for k in R.SPLIT_VN:
         p[k] = _round(p[k], 64.0, dtype)
-    x = R._x(states, torch.float64)
     with torch.no_grad():
-        a = x
-        for l in (1, 2, 3):
-            a = _round(F.relu(F.conv2d(a, p["conv%d.weight" % l], p["conv%d.bias" % l])), 16.0, dtype)
-        act3 = a.flatten(1)
+        act3 = emulate_layers(w, states, dtype)[-1].flatten(1)
         h = F.relu(act3 @ p["fc1.weight"].T + p["fc1.bias"])
         out = torch.sigmoid(h @ p["fc_out.weight"].T + p["fc_out.bias"]) * p["out_ubound"] + p["out_lbound"]
     o = out.numpy()

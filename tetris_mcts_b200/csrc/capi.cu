@@ -6,6 +6,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <string>
 #include <vector>
 
@@ -366,16 +367,20 @@ static int ensure_act3(b200_engine *e, size_t rows) {
     return 0;
 }
 
-// run the network over the request list req[0..*n_req) -> eval_out; device-side count, no host sync
+// run the network over the request list req[0..*n_req) -> eval_out; device-side count, no host sync.  dbg (tensor-core kinds,
+// standalone requests only): run k_tc_conv_dbg instead, which also copies act1 / act2 there (TCC_DBG_BYTES per request)
 static int launch_net(b200_engine *e, const uint2 *req, const int32_t *n_req, const uint32_t *keys, int M, float2 *eval_out,
-                      size_t max_rows) {
+                      size_t max_rows, uint8_t *dbg = nullptr) {
     if (!e->have_weights) return fail(B200_ERR_NO_WEIGHTS, "b200_load_weights was not called");
     if (tc_net(e)) {
         TcState *st = (TcState *)e->tc_state;
         const uint8_t *act3_before = st->d_act3;
         if (tc_ensure_act3(st, max_rows, e->stream)) return fail(B200_ERR_CUDA, "act3 (tensor-core layout) allocation failed");
         if (act3_before && st->d_act3 != act3_before) drop_step_graph(e);   // a larger standalone batch moved the activation buffer
-        {
+        if (dbg) {
+            (e->cfg.eval_kind == B200_EVAL_NET_FP16 ? k_tc_conv_dbg<1> : k_tc_conv_dbg<2>)<<<e->n_sm, TCC_THREADS, TCC_SMEM, e->stream>>>(
+                e->W, st->TW, req, n_req, keys, st->d_act3, (int)st->tiles, dbg);
+        } else {
             PhaseTimer t(e, PH_CONV);
             tc_conv_kernel(e)<<<e->n_sm, TCC_THREADS, TCC_SMEM, e->stream>>>(e->W, st->TW, req, n_req, nullptr, keys, M, st->d_act3, (int)st->tiles,
                                                                              e->timing ? e->A.counters + 16 : nullptr);
@@ -435,7 +440,9 @@ extern "C" int b200_load_dist_weights(b200_engine *e, const float *w, int atoms)
     return B200_OK;
 }
 
-static int launch_distnet_on(b200_engine *e, const uint2 *req, const int32_t *n_req, const uint32_t *keys, int M, float *out, size_t max_rows) {
+// dbg (tensor-core kinds, standalone requests only): run k_tdc_conv_dbg instead, which also copies act1 there (TDC_ASLOT per request)
+static int launch_distnet_on(b200_engine *e, const uint2 *req, const int32_t *n_req, const uint32_t *keys, int M, float *out, size_t max_rows,
+                             uint8_t *dbg = nullptr) {
     if (!e->have_dist_weights) return fail(B200_ERR_NO_WEIGHTS, "b200_load_dist_weights was not called");
     if (dn_tc_net(e)) {
         DnTcState *st = (DnTcState *)e->dn_tc_state;
@@ -443,7 +450,10 @@ static int launch_distnet_on(b200_engine *e, const uint2 *req, const int32_t *n_
         if (dn_tc_ensure_act2(st, max_rows, e->stream, &moved)) return fail(B200_ERR_CUDA, "act2 (tensor-core layout) allocation failed");
         if (moved) drop_step_graph(e);
         const bool one = e->cfg.eval_kind == B200_EVAL_DIST_FP16;
-        {
+        if (dbg) {
+            (one ? k_tdc_conv_dbg<1> : k_tdc_conv_dbg<2>)<<<e->n_sm, TDC_THREADS, TDC_SMEM, e->stream>>>(e->DW, st->TW, req, n_req, keys, st->d_act2,
+                                                                                                       (int)st->tiles, dbg);
+        } else {
             PhaseTimer t(e, PH_CONV);
             (one ? k_tdc_conv<1> : k_tdc_conv<2>)<<<e->n_sm, TDC_THREADS, TDC_SMEM, e->stream>>>(e->DW, st->TW, req, n_req, keys, M, st->d_act2,
                                                                                                (int)st->tiles);
@@ -478,7 +488,7 @@ static int launch_distnet(b200_engine *e) {
 }
 
 // Model.inference of model/model_distributional.py (softmax over atoms): states[k][200] int8 -> dist[k][atoms]
-extern "C" int b200_distnet_forward(b200_engine *e, const int8_t *states, int k, int atoms, float *dist) {
+static int distnet_forward(b200_engine *e, const int8_t *states, int k, int atoms, float *dist, uint8_t *dbg) {
     if (!e || !states || !dist || k < 1 || atoms != e->DW.atoms) return fail(B200_ERR_BAD_ARG, "bad argument (atoms must match the loaded weights)");
     CK(cudaSetDevice(e->cfg.device));
     int8_t *d_states = nullptr; uint32_t *d_keys = nullptr; uint2 *d_req = nullptr; int32_t *d_n = nullptr; float *d_out = nullptr;
@@ -489,7 +499,7 @@ extern "C" int b200_distnet_forward(b200_engine *e, const int8_t *states, int k,
     CK(cudaMemcpyAsync(d_n, &k, 4, cudaMemcpyHostToDevice, e->stream));
     k_states_to_keys<<<(k + 127) / 128, 128, 0, e->stream>>>(d_states, k, d_keys, d_req);
     k_dn_req_rows<<<(k + 127) / 128, 128, 0, e->stream>>>(d_req, k);      // request i -> output row i
-    int rc = launch_distnet_on(e, d_req, d_n, d_keys, 0, d_out, (size_t)k);
+    int rc = launch_distnet_on(e, d_req, d_n, d_keys, 0, d_out, (size_t)k, dbg);
     if (rc == B200_OK) {
         cudaError_t ce = cudaMemcpyAsync(dist, d_out, (size_t)k * atoms * 4, cudaMemcpyDeviceToHost, e->stream);
         if (ce == cudaSuccess) ce = cudaStreamSynchronize(e->stream);
@@ -497,6 +507,9 @@ extern "C" int b200_distnet_forward(b200_engine *e, const int8_t *states, int k,
     }
     cudaStreamSynchronize(e->stream);
     return rc;
+}
+extern "C" int b200_distnet_forward(b200_engine *e, const int8_t *states, int k, int atoms, float *dist) {
+    return distnet_forward(e, states, k, atoms, dist, nullptr);
 }
 
 // ---------------------------------------------------------------------------------------------------- games / roots
@@ -966,7 +979,7 @@ __global__ void k_states_to_keys(const int8_t *states, int k, uint32_t *keys, ui
     req[i] = make_uint2((uint32_t)(i >> 3), (uint32_t)i | ((uint32_t)(i & 7) << 28));
 }
 
-extern "C" int b200_valuenet_forward(b200_engine *e, const int8_t *states, int k, float *v, float *var) {
+static int valuenet_forward(b200_engine *e, const int8_t *states, int k, float *v, float *var, uint8_t *dbg) {
     if (!e || !states || !v || !var || k < 1) return fail(B200_ERR_BAD_ARG, "bad argument");
     if (k >= (1 << 28)) return fail(B200_ERR_BAD_ARG, "k too large");
     CK(cudaSetDevice(e->cfg.device));
@@ -979,7 +992,7 @@ extern "C" int b200_valuenet_forward(b200_engine *e, const int8_t *states, int k
     CK(cudaMemcpyAsync(d_n, &k, 4, cudaMemcpyHostToDevice, e->stream));
     k_states_to_keys<<<(k + 127) / 128, 128, 0, e->stream>>>(d_states, k, d_keys, d_req);
     // keys are addressed as keys[(game * M + obs)]: with game = i/8 we pass M = 0 so that only obs (= i) indexes
-    int rc = launch_net(e, d_req, d_n, d_keys, 0, d_out, kp);
+    int rc = launch_net(e, d_req, d_n, d_keys, 0, d_out, kp, dbg);
     if (rc == B200_OK) {
         std::vector<float2> h(k);
         cudaError_t ce = cudaMemcpyAsync(h.data(), d_out, (size_t)k * 8, cudaMemcpyDeviceToHost, e->stream);
@@ -989,6 +1002,9 @@ extern "C" int b200_valuenet_forward(b200_engine *e, const int8_t *states, int k
     }
     cudaStreamSynchronize(e->stream);
     return rc;
+}
+extern "C" int b200_valuenet_forward(b200_engine *e, const int8_t *states, int k, float *v, float *var) {
+    return valuenet_forward(e, states, k, v, var, nullptr);
 }
 
 // development / test aid: the conv stack's output (flatten input of fc1) in torch order c*56 + y*4 + x, for either path
@@ -1050,6 +1066,70 @@ extern "C" int b200_debug_dist_act2(b200_engine *e, const int8_t *states, int k,
             }
             out[(size_t)r * 2048 + c * 64 + p] = sum / TC_SCALE_A;
         }
+    return B200_OK;
+}
+
+// development / test aid: every layer of the tensor-core networks exactly as the next layer reads it, from one forward pass that runs the
+// conv kernel's DBG instantiation (which also copies the shared-memory activations out) and the production fc kernel
+extern "C" int b200_debug_tc_acts(b200_engine *e, int dist, const int8_t *states, int k, int layer, float *out) {
+    if (!e || !states || !out || k < 1) return fail(B200_ERR_BAD_ARG, "bad argument");
+    if (dist ? !dn_tc_net(e) : !tc_net(e))
+        return fail(B200_ERR_BAD_ARG, "b200_debug_tc_acts reads the tensor-core networks: eval_kind net_tc, net_fp16 (value) or dist_fp16 (distributional)");
+    if (layer < 0 || layer > (dist ? 2 : 3)) return fail(B200_ERR_BAD_ARG, "layer out of range");
+    if (dist ? !e->have_dist_weights : !e->have_weights) return fail(B200_ERR_NO_WEIGHTS, "no weights loaded for this network");
+    const int nt = (e->cfg.eval_kind == B200_EVAL_NET_FP16 || e->cfg.eval_kind == B200_EVAL_DIST_FP16) ? 1 : 2;
+    const size_t slot = dist ? TDC_ASLOT : TCC_DBG_BYTES;
+    uint8_t *d_dbg = nullptr;
+    Scratch tmp;
+    CK(tmp.get(&d_dbg, (size_t)k * slot));
+    std::vector<float> o0((size_t)k * (dist ? e->DW.atoms : 2));
+    int rc;
+    if (dist) rc = distnet_forward(e, states, k, e->DW.atoms, o0.data(), d_dbg);
+    else {
+        std::vector<float> v(k), var(k);
+        rc = valuenet_forward(e, states, k, v.data(), var.data(), d_dbg);
+        for (int r = 0; r < k; ++r) { o0[2 * r] = v[r]; o0[2 * r + 1] = var[r]; }
+    }
+    if (rc) return rc;
+    if (layer == 0) { memcpy(out, o0.data(), o0.size() * 4); return B200_OK; }
+    // out[k][nt][32][H][W]: fp16 term s of channel c at (y, x), divided by TC_SCALE_A
+    int H, Wd;
+    std::vector<uint8_t> h;
+    std::function<size_t(int, int, int, int, int)> off;
+    if (layer == (dist ? 2 : 3)) {                               // the conv stack's output: in HBM, the fc kernel's tile layout
+        const uint8_t *src; size_t tiles; int kch;
+        if (dist) { DnTcState *st = (DnTcState *)e->dn_tc_state; src = st->d_act2; tiles = st->tiles; kch = DACT2_KCHUNKS; H = 16; Wd = 4; }
+        else { TcState *st = (TcState *)e->tc_state; src = st->d_act3; tiles = st->tiles; kch = ACT3_KCHUNKS; H = 14; Wd = 4; }
+        h.resize((size_t)2 * tiles * kch * 2048);
+        CK(cudaMemcpy(h.data(), src, h.size(), cudaMemcpyDeviceToHost));
+        off = [=](int r, int s, int c, int y, int x) {
+            const int kp = (y * 4 + x) * 32 + c;
+            return ((((size_t)s * tiles + (r >> 7)) * kch + (kp >> 3)) * 128 + (r & 127)) * 16 + (kp & 7) * 2;
+        };
+    } else {                                                     // a shared-memory slot copied by the DBG kernel
+        h.resize((size_t)k * slot);
+        CK(cudaMemcpy(h.data(), d_dbg, h.size(), cudaMemcpyDeviceToHost));
+        if (dist) {                                              // act1: [term][chunk 4][152 rows][16 B], row y*8 + x
+            H = 19; Wd = 7;
+            off = [=](int r, int s, int c, int y, int x) { return r * slot + (size_t)s * 4 * TDC_R * 16 + ((c >> 3) * TDC_R + y * 8 + x) * 16 + (c & 7) * 2; };
+        } else if (layer == 1) {                                 // act1: [term][chunk 4][144 rows][16 B], row y*8 + x
+            H = 18; Wd = 8;
+            off = [=](int r, int s, int c, int y, int x) { return r * slot + (size_t)s * 4 * TCC_R * 16 + ((c >> 3) * TCC_R + y * 8 + x) * 16 + (c & 7) * 2; };
+        } else {                                                 // act2: [term, stride TCC_A2SPLIT][chunk 4][98 rows][16 B], row x*16 + y
+            H = 16; Wd = 6;
+            off = [=](int r, int s, int c, int y, int x) {
+                return r * slot + TCC_ASLOT + (size_t)s * TCC_A2SPLIT + ((c >> 3) * TCC_R2 + x * 16 + y) * 16 + (c & 7) * 2;
+            };
+        }
+    }
+    for (int r = 0; r < k; ++r)
+        for (int s = 0; s < nt; ++s)
+            for (int c = 0; c < 32; ++c)
+                for (int y = 0; y < H; ++y)
+                    for (int x = 0; x < Wd; ++x) {
+                        uint16_t hb; memcpy(&hb, &h[off(r, s, c, y, x)], 2);
+                        out[((((size_t)r * nt + s) * 32 + c) * H + y) * Wd + x] = host_half_f(hb) / TC_SCALE_A;
+                    }
     return B200_OK;
 }
 

@@ -79,9 +79,11 @@ __device__ __forceinline__ void issue_dconv2(float (&d)[64], uint32_t a_addr, ui
     }
 }
 
-template <int NT>
-__global__ void __launch_bounds__(TDC_THREADS, 1)
-k_tdc_conv(DistNetWeights W, DnTcWeights TW, const uint2 *req, const int32_t *n_req_ptr, const uint32_t *keys, int M, uint8_t *act2, int n_tiles) {
+// With DBG, each board's act1 slot (which never leaves shared memory) is copied verbatim to dbg + ridx * TDC_ASLOT once conv1's epilogue
+// has finished (b200_debug_tc_acts decodes it).  Only k_tdc_conv_dbg instantiates it.
+template <int NT, bool DBG>
+__device__ __forceinline__ void tdc_conv_body(DistNetWeights W, DnTcWeights TW, const uint2 *req, const int32_t *n_req_ptr, const uint32_t *keys, int M,
+                                              uint8_t *act2, int n_tiles, uint8_t *dbg) {
     extern __shared__ __align__(128) uint8_t smem[];
     float *sB = reinterpret_cast<float *>(smem + TDC_OFF_BIAS);
     const int t = threadIdx.x, wg = t >> 7, wt = t & 127, w = wt >> 5, lane = t & 31;
@@ -185,6 +187,7 @@ k_tdc_conv(DistNetWeights W, DnTcWeights TW, const uint2 *req, const int32_t *n_
         }
         fence_async_smem();
         wg_sync(wg);
+        if constexpr (DBG) copy_slot(dbg + (size_t)ridx * TDC_ASLOT, act, TDC_ASLOT, wt);
         // ---- conv2 (model_distributional.py:22): act1 on the 19x8 grid; epilogue: dx sum + bias + LeakyReLU + split -> act2 in HBM
 #pragma unroll 1
         for (int mt = 0; mt < 2; ++mt) {
@@ -225,6 +228,17 @@ k_tdc_conv(DistNetWeights W, DnTcWeights TW, const uint2 *req, const int32_t *n_
             }
         }
     }
+}
+
+template <int NT>
+__global__ void __launch_bounds__(TDC_THREADS, 1)
+k_tdc_conv(DistNetWeights W, DnTcWeights TW, const uint2 *req, const int32_t *n_req_ptr, const uint32_t *keys, int M, uint8_t *act2, int n_tiles) {
+    tdc_conv_body<NT, false>(W, TW, req, n_req_ptr, keys, M, act2, n_tiles, nullptr);
+}
+template <int NT>
+__global__ void __launch_bounds__(TDC_THREADS, 1)
+k_tdc_conv_dbg(DistNetWeights W, DnTcWeights TW, const uint2 *req, const int32_t *n_req_ptr, const uint32_t *keys, uint8_t *act2, int n_tiles, uint8_t *dbg) {
+    tdc_conv_body<NT, true>(W, TW, req, n_req_ptr, keys, 0, act2, n_tiles, dbg);
 }
 
 // ---------------------------------------------------------------------------------------------------- fc1 + fc_v + softmax
@@ -406,6 +420,8 @@ static int dn_tc_prepare(void **state, const float *w, int atoms, cudaStream_t s
     st->TW.wc1 = st->d_w; st->TW.wc2 = st->d_w + TDC_W1BYTES; st->TW.wfc = st->TW.wc2 + TDC_WBYTES;
     if (cudaFuncSetAttribute(k_tdc_conv<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, TDC_SMEM) != cudaSuccess) return 1;
     if (cudaFuncSetAttribute(k_tdc_conv<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, TDC_SMEM) != cudaSuccess) return 1;
+    if (cudaFuncSetAttribute(k_tdc_conv_dbg<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, TDC_SMEM) != cudaSuccess) return 1;
+    if (cudaFuncSetAttribute(k_tdc_conv_dbg<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, TDC_SMEM) != cudaSuccess) return 1;
     if (cudaFuncSetAttribute(k_tdc_fc<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, TDF_SMEM) != cudaSuccess) return 1;
     if (cudaFuncSetAttribute(k_tdc_fc<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, TDF_SMEM) != cudaSuccess) return 1;
     return 0;

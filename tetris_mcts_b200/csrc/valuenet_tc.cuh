@@ -266,10 +266,16 @@ __device__ __forceinline__ void build_im2col3(uint8_t *im, const uint32_t *tab, 
     }
 }
 
-template <int NT>
-__global__ void __launch_bounds__(TCC_THREADS, 1)
-k_tc_conv(NetWeights W, TcWeights TW, const uint2 *req, const int32_t *n_req_ptr, const int32_t *first_ptr, const uint32_t *keys, int M, uint8_t *act3,
-          int n_tiles, unsigned long long *prof) {
+// Test export of the activations that never leave shared memory: with DBG, each board's act1 and act2 slots are copied verbatim to
+// dbg + ridx * TCC_DBG_BYTES once their epilogue has finished (b200_debug_tc_acts decodes them).  Only k_tc_conv_dbg instantiates it.
+constexpr int TCC_DBG_BYTES = TCC_ASLOT + TCC_A2SLOT;
+__device__ __forceinline__ void copy_slot(uint8_t *dst, const uint8_t *src, int bytes, int wt) {
+    for (int i = wt; i < bytes / 16; i += 128) reinterpret_cast<uint4 *>(dst)[i] = reinterpret_cast<const uint4 *>(src)[i];
+}
+
+template <int NT, bool DBG>
+__device__ __forceinline__ void tc_conv_body(NetWeights W, TcWeights TW, const uint2 *req, const int32_t *n_req_ptr, const int32_t *first_ptr,
+                                             const uint32_t *keys, int M, uint8_t *act3, int n_tiles, unsigned long long *prof, uint8_t *dbg) {
     extern __shared__ __align__(128) uint8_t smem[];
     float *sB = reinterpret_cast<float *>(smem + TCC_OFF_BIAS);
     const int t = threadIdx.x, wg = t >> 7, wt = t & 127, w = wt >> 5, lane = t & 31;
@@ -370,6 +376,7 @@ k_tc_conv(NetWeights W, TcWeights TW, const uint2 *req, const int32_t *n_req_ptr
         fence_async_smem();
         wg_sync(wg);
         prof_t(1);
+        if constexpr (DBG) copy_slot(dbg + (size_t)ridx * TCC_DBG_BYTES, act, TCC_ASLOT, wt);
         // ---- conv2 (model_vv.py:34) on act1 (18x8 grid) -> act2 (column-major, its own buffer: tile 0's outputs reach row 87 of act2
         // while tile 1 still reads act1 rows 64..143)
 #pragma unroll 1
@@ -424,6 +431,7 @@ k_tc_conv(NetWeights W, TcWeights TW, const uint2 *req, const int32_t *n_req_ptr
         fence_async_smem();
         wg_sync(wg);
         prof_t(2);
+        if constexpr (DBG) copy_slot(dbg + (size_t)ridx * TCC_DBG_BYTES + TCC_ASLOT, act2, TCC_A2SLOT, wt);
         // ---- conv3 (:36) on act2: one tile, warp w holds column x = w, lane rows y = 8h + rl; act3 -> HBM
         {
             float d[3][16];
@@ -465,6 +473,18 @@ k_tc_conv(NetWeights W, TcWeights TW, const uint2 *req, const int32_t *n_req_ptr
         prof_t(3);
     }
     if (do_prof) for (int k = 0; k < 4; ++k) atomicAdd(&prof[k], (unsigned long long)pacc[k]);
+}
+
+template <int NT>
+__global__ void __launch_bounds__(TCC_THREADS, 1)
+k_tc_conv(NetWeights W, TcWeights TW, const uint2 *req, const int32_t *n_req_ptr, const int32_t *first_ptr, const uint32_t *keys, int M, uint8_t *act3,
+          int n_tiles, unsigned long long *prof) {
+    tc_conv_body<NT, false>(W, TW, req, n_req_ptr, first_ptr, keys, M, act3, n_tiles, prof, nullptr);
+}
+template <int NT>
+__global__ void __launch_bounds__(TCC_THREADS, 1)
+k_tc_conv_dbg(NetWeights W, TcWeights TW, const uint2 *req, const int32_t *n_req_ptr, const uint32_t *keys, uint8_t *act3, int n_tiles, uint8_t *dbg) {
+    tc_conv_body<NT, true>(W, TW, req, n_req_ptr, nullptr, keys, 0, act3, n_tiles, nullptr, dbg);
 }
 
 // ---------------------------------------------------------------------------------------------------- fc kernel
@@ -649,6 +669,8 @@ static int tc_prepare(void **state, const float *w, cudaStream_t stream) {
     st->TW.wc1 = st->d_w; st->TW.wc2 = st->d_w + TCC_W1BYTES; st->TW.wc3 = st->TW.wc2 + TCC_WBYTES; st->TW.wfc = st->TW.wc3 + TCC_WBYTES;
     if (cudaFuncSetAttribute(k_tc_conv<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, TCC_SMEM) != cudaSuccess) return 1;
     if (cudaFuncSetAttribute(k_tc_conv<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, TCC_SMEM) != cudaSuccess) return 1;
+    if (cudaFuncSetAttribute(k_tc_conv_dbg<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, TCC_SMEM) != cudaSuccess) return 1;
+    if (cudaFuncSetAttribute(k_tc_conv_dbg<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, TCC_SMEM) != cudaSuccess) return 1;
     if (cudaFuncSetAttribute(k_tc_fc<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, TCF_SMEM) != cudaSuccess) return 1;
     if (cudaFuncSetAttribute(k_tc_fc<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, TCF_SMEM) != cudaSuccess) return 1;
     return 0;
