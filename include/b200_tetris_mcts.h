@@ -199,8 +199,9 @@ int b200_debug_dist_act2(b200_engine *e, const int8_t *states, int k, float *out
 /* test aid: one layer of a tensor-core network exactly as the next layer reads it, from a forward pass on states[k][200].  dist = 0: the
  * value network (B200_EVAL_NET_TC or B200_EVAL_NET_FP16), layer 1..3 = act1 [32][18][8], act2 [32][16][6], act3 [32][14][4]; dist = 1: the
  * distributional network (B200_EVAL_NET_TC or B200_EVAL_DIST_FP16), layer 1..2 = act1 [32][19][7], act2 [32][16][4].  out[k][nt][...] holds
- * fp16 term s < nt of each element divided by 16 (nt = 2 for net_tc, 1 for the fp16 kinds).  layer 0: the same pass's outputs, out[k][2]
- * = (v, var) or out[k][atoms] = probabilities. */
+ * fp16 term s < nt of each element divided by 16 (nt = 2 for net_tc, 1 for the fp16 kinds).  layer 4 (value) / 3 (distributional): fc1's
+ * raw fp32 accumulator, out[k][256] / out[k][128] in torch column order (the value before the 2^-10, the bias and the activation).
+ * layer 0: the same pass's outputs, out[k][2] = (v, var) or out[k][atoms] = probabilities. */
 int b200_debug_tc_acts(b200_engine *e, int dist, const int8_t *states, int k, int layer, float *out);
 int b200_export_dist(b200_engine *e, int game, float *node_stats /* [M][5] */, float *node_dist /* [M][bins] */);
 

@@ -302,6 +302,7 @@ extern "C" int b200_engine_get_stream(b200_engine *e, void **cuda_stream_out) {
 static bool tc_net(const b200_engine *e) { return e->cfg.eval_kind == B200_EVAL_NET_TC || e->cfg.eval_kind == B200_EVAL_NET_FP16; }
 static decltype(&k_tc_conv<2>) tc_conv_kernel(const b200_engine *e) { return e->cfg.eval_kind == B200_EVAL_NET_FP16 ? k_tc_conv<1> : k_tc_conv<2>; }
 static decltype(&k_tc_fc<2>) tc_fc_kernel(const b200_engine *e) { return e->cfg.eval_kind == B200_EVAL_NET_FP16 ? k_tc_fc<1> : k_tc_fc<2>; }
+static decltype(&k_tc_fc_dbg<2>) tc_fc_dbg_kernel(const b200_engine *e) { return e->cfg.eval_kind == B200_EVAL_NET_FP16 ? k_tc_fc_dbg<1> : k_tc_fc_dbg<2>; }
 
 extern "C" int b200_load_weights(b200_engine *e, const float *w) {
     if (!e || !w) return fail(B200_ERR_BAD_ARG, "null argument");
@@ -368,9 +369,10 @@ static int ensure_act3(b200_engine *e, size_t rows) {
 }
 
 // run the network over the request list req[0..*n_req) -> eval_out; device-side count, no host sync.  dbg (tensor-core kinds,
-// standalone requests only): run k_tc_conv_dbg instead, which also copies act1 / act2 there (TCC_DBG_BYTES per request)
+// standalone requests only): run k_tc_conv_dbg and k_tc_fc_dbg instead, which also copy act1 / act2 there (TCC_DBG_BYTES per request)
+// and fc1's fp32 accumulator to dbg_fc (256 floats per request)
 static int launch_net(b200_engine *e, const uint2 *req, const int32_t *n_req, const uint32_t *keys, int M, float2 *eval_out,
-                      size_t max_rows, uint8_t *dbg = nullptr) {
+                      size_t max_rows, uint8_t *dbg = nullptr, float *dbg_fc = nullptr) {
     if (!e->have_weights) return fail(B200_ERR_NO_WEIGHTS, "b200_load_weights was not called");
     if (tc_net(e)) {
         TcState *st = (TcState *)e->tc_state;
@@ -385,7 +387,9 @@ static int launch_net(b200_engine *e, const uint2 *req, const int32_t *n_req, co
             tc_conv_kernel(e)<<<e->n_sm, TCC_THREADS, TCC_SMEM, e->stream>>>(e->W, st->TW, req, n_req, nullptr, keys, M, st->d_act3, (int)st->tiles,
                                                                              e->timing ? e->A.counters + 16 : nullptr);
         }
-        {
+        if (dbg) {
+            tc_fc_dbg_kernel(e)<<<e->n_sm, TCF_THREADS, TCF_SMEM, e->stream>>>(e->W, st->TW, st->d_act3, (int)st->tiles, req, n_req, eval_out, dbg_fc);
+        } else {
             PhaseTimer t(e, PH_FC);
             tc_fc_kernel(e)<<<e->n_sm, TCF_THREADS, TCF_SMEM, e->stream>>>(e->W, st->TW, st->d_act3, (int)st->tiles, req, n_req, eval_out);
         }
@@ -440,9 +444,10 @@ extern "C" int b200_load_dist_weights(b200_engine *e, const float *w, int atoms)
     return B200_OK;
 }
 
-// dbg (tensor-core kinds, standalone requests only): run k_tdc_conv_dbg instead, which also copies act1 there (TDC_ASLOT per request)
+// dbg (tensor-core kinds, standalone requests only): run k_tdc_conv_dbg and k_tdc_fc_dbg instead, which also copy act1 there (TDC_ASLOT
+// per request) and fc1's fp32 accumulator to dbg_fc (128 floats per request)
 static int launch_distnet_on(b200_engine *e, const uint2 *req, const int32_t *n_req, const uint32_t *keys, int M, float *out, size_t max_rows,
-                             uint8_t *dbg = nullptr) {
+                             uint8_t *dbg = nullptr, float *dbg_fc = nullptr) {
     if (!e->have_dist_weights) return fail(B200_ERR_NO_WEIGHTS, "b200_load_dist_weights was not called");
     if (dn_tc_net(e)) {
         DnTcState *st = (DnTcState *)e->dn_tc_state;
@@ -458,7 +463,10 @@ static int launch_distnet_on(b200_engine *e, const uint2 *req, const int32_t *n_
             (one ? k_tdc_conv<1> : k_tdc_conv<2>)<<<e->n_sm, TDC_THREADS, TDC_SMEM, e->stream>>>(e->DW, st->TW, req, n_req, keys, M, st->d_act2,
                                                                                                (int)st->tiles);
         }
-        {
+        if (dbg) {
+            (one ? k_tdc_fc_dbg<1> : k_tdc_fc_dbg<2>)<<<e->n_sm, TDF_THREADS, TDF_SMEM, e->stream>>>(e->DW, st->TW, st->d_act2, (int)st->tiles, req, n_req,
+                                                                                                   out, dbg_fc);
+        } else {
             PhaseTimer t(e, PH_FC);
             (one ? k_tdc_fc<1> : k_tdc_fc<2>)<<<e->n_sm, TDF_THREADS, TDF_SMEM, e->stream>>>(e->DW, st->TW, st->d_act2, (int)st->tiles, req, n_req, out);
         }
@@ -488,7 +496,7 @@ static int launch_distnet(b200_engine *e) {
 }
 
 // Model.inference of model/model_distributional.py (softmax over atoms): states[k][200] int8 -> dist[k][atoms]
-static int distnet_forward(b200_engine *e, const int8_t *states, int k, int atoms, float *dist, uint8_t *dbg) {
+static int distnet_forward(b200_engine *e, const int8_t *states, int k, int atoms, float *dist, uint8_t *dbg, float *dbg_fc) {
     if (!e || !states || !dist || k < 1 || atoms != e->DW.atoms) return fail(B200_ERR_BAD_ARG, "bad argument (atoms must match the loaded weights)");
     CK(cudaSetDevice(e->cfg.device));
     int8_t *d_states = nullptr; uint32_t *d_keys = nullptr; uint2 *d_req = nullptr; int32_t *d_n = nullptr; float *d_out = nullptr;
@@ -499,7 +507,7 @@ static int distnet_forward(b200_engine *e, const int8_t *states, int k, int atom
     CK(cudaMemcpyAsync(d_n, &k, 4, cudaMemcpyHostToDevice, e->stream));
     k_states_to_keys<<<(k + 127) / 128, 128, 0, e->stream>>>(d_states, k, d_keys, d_req);
     k_dn_req_rows<<<(k + 127) / 128, 128, 0, e->stream>>>(d_req, k);      // request i -> output row i
-    int rc = launch_distnet_on(e, d_req, d_n, d_keys, 0, d_out, (size_t)k, dbg);
+    int rc = launch_distnet_on(e, d_req, d_n, d_keys, 0, d_out, (size_t)k, dbg, dbg_fc);
     if (rc == B200_OK) {
         cudaError_t ce = cudaMemcpyAsync(dist, d_out, (size_t)k * atoms * 4, cudaMemcpyDeviceToHost, e->stream);
         if (ce == cudaSuccess) ce = cudaStreamSynchronize(e->stream);
@@ -509,7 +517,7 @@ static int distnet_forward(b200_engine *e, const int8_t *states, int k, int atom
     return rc;
 }
 extern "C" int b200_distnet_forward(b200_engine *e, const int8_t *states, int k, int atoms, float *dist) {
-    return distnet_forward(e, states, k, atoms, dist, nullptr);
+    return distnet_forward(e, states, k, atoms, dist, nullptr, nullptr);
 }
 
 // ---------------------------------------------------------------------------------------------------- games / roots
@@ -979,7 +987,7 @@ __global__ void k_states_to_keys(const int8_t *states, int k, uint32_t *keys, ui
     req[i] = make_uint2((uint32_t)(i >> 3), (uint32_t)i | ((uint32_t)(i & 7) << 28));
 }
 
-static int valuenet_forward(b200_engine *e, const int8_t *states, int k, float *v, float *var, uint8_t *dbg) {
+static int valuenet_forward(b200_engine *e, const int8_t *states, int k, float *v, float *var, uint8_t *dbg, float *dbg_fc) {
     if (!e || !states || !v || !var || k < 1) return fail(B200_ERR_BAD_ARG, "bad argument");
     if (k >= (1 << 28)) return fail(B200_ERR_BAD_ARG, "k too large");
     CK(cudaSetDevice(e->cfg.device));
@@ -992,7 +1000,7 @@ static int valuenet_forward(b200_engine *e, const int8_t *states, int k, float *
     CK(cudaMemcpyAsync(d_n, &k, 4, cudaMemcpyHostToDevice, e->stream));
     k_states_to_keys<<<(k + 127) / 128, 128, 0, e->stream>>>(d_states, k, d_keys, d_req);
     // keys are addressed as keys[(game * M + obs)]: with game = i/8 we pass M = 0 so that only obs (= i) indexes
-    int rc = launch_net(e, d_req, d_n, d_keys, 0, d_out, kp, dbg);
+    int rc = launch_net(e, d_req, d_n, d_keys, 0, d_out, kp, dbg, dbg_fc);
     if (rc == B200_OK) {
         std::vector<float2> h(k);
         cudaError_t ce = cudaMemcpyAsync(h.data(), d_out, (size_t)k * 8, cudaMemcpyDeviceToHost, e->stream);
@@ -1004,7 +1012,7 @@ static int valuenet_forward(b200_engine *e, const int8_t *states, int k, float *
     return rc;
 }
 extern "C" int b200_valuenet_forward(b200_engine *e, const int8_t *states, int k, float *v, float *var) {
-    return valuenet_forward(e, states, k, v, var, nullptr);
+    return valuenet_forward(e, states, k, v, var, nullptr, nullptr);
 }
 
 // development / test aid: the conv stack's output (flatten input of fc1) in torch order c*56 + y*4 + x, for either path
@@ -1069,29 +1077,37 @@ extern "C" int b200_debug_dist_act2(b200_engine *e, const int8_t *states, int k,
     return B200_OK;
 }
 
-// development / test aid: every layer of the tensor-core networks exactly as the next layer reads it, from one forward pass that runs the
-// conv kernel's DBG instantiation (which also copies the shared-memory activations out) and the production fc kernel
+// development / test aid: every layer of the tensor-core networks exactly as the next layer reads it, and fc1's fp32 accumulator, from one
+// forward pass that runs the DBG instantiations of the conv kernel (which also copies the shared-memory activations out) and of the fc
+// kernel (which also writes the accumulator out)
 extern "C" int b200_debug_tc_acts(b200_engine *e, int dist, const int8_t *states, int k, int layer, float *out) {
     if (!e || !states || !out || k < 1) return fail(B200_ERR_BAD_ARG, "bad argument");
     if (dist ? !dn_tc_net(e) : !tc_net(e))
         return fail(B200_ERR_BAD_ARG, "b200_debug_tc_acts reads the tensor-core networks: eval_kind net_tc, net_fp16 (value) or dist_fp16 (distributional)");
-    if (layer < 0 || layer > (dist ? 2 : 3)) return fail(B200_ERR_BAD_ARG, "layer out of range");
+    if (layer < 0 || layer > (dist ? 3 : 4)) return fail(B200_ERR_BAD_ARG, "layer out of range");
     if (dist ? !e->have_dist_weights : !e->have_weights) return fail(B200_ERR_NO_WEIGHTS, "no weights loaded for this network");
     const int nt = (e->cfg.eval_kind == B200_EVAL_NET_FP16 || e->cfg.eval_kind == B200_EVAL_DIST_FP16) ? 1 : 2;
     const size_t slot = dist ? TDC_ASLOT : TCC_DBG_BYTES;
+    const int n_fc1 = dist ? 128 : 256;
     uint8_t *d_dbg = nullptr;
+    float *d_fc = nullptr;
     Scratch tmp;
     CK(tmp.get(&d_dbg, (size_t)k * slot));
+    CK(tmp.get(&d_fc, (size_t)k * n_fc1 * 4));
     std::vector<float> o0((size_t)k * (dist ? e->DW.atoms : 2));
     int rc;
-    if (dist) rc = distnet_forward(e, states, k, e->DW.atoms, o0.data(), d_dbg);
+    if (dist) rc = distnet_forward(e, states, k, e->DW.atoms, o0.data(), d_dbg, d_fc);
     else {
         std::vector<float> v(k), var(k);
-        rc = valuenet_forward(e, states, k, v.data(), var.data(), d_dbg);
+        rc = valuenet_forward(e, states, k, v.data(), var.data(), d_dbg, d_fc);
         for (int r = 0; r < k; ++r) { o0[2 * r] = v[r]; o0[2 * r + 1] = var[r]; }
     }
     if (rc) return rc;
     if (layer == 0) { memcpy(out, o0.data(), o0.size() * 4); return B200_OK; }
+    if (layer == (dist ? 3 : 4)) {                               // fc1's accumulator: out[k][n_fc1], as the fc kernel's DBG instantiation wrote it
+        CK(cudaMemcpy(out, d_fc, (size_t)k * n_fc1 * 4, cudaMemcpyDeviceToHost));
+        return B200_OK;
+    }
     // out[k][nt][32][H][W]: fp16 term s of channel c at (y, x), divided by TC_SCALE_A
     int H, Wd;
     std::vector<uint8_t> h;

@@ -258,9 +258,11 @@ static_assert(2 * TDF_STAGES * 8 <= 256, "barrier block overflows into the epilo
 constexpr int TDF_SMEM = TDF_OFF_EPI + (128 + 128 * TDF_ATOMS + TDF_ATOMS + TDF_CONSUMERS * 64 * TDF_HSTRIDE) * 4;
 static_assert(TDF_SMEM <= 227 * 1024, "k_tdc_fc shared memory");
 
-template <int NT>
-__global__ void __launch_bounds__(TDF_THREADS, 1)
-k_tdc_fc(DistNetWeights W, DnTcWeights TW, const uint8_t *act2, int n_tiles_alloc, const uint2 *req, const int32_t *n_req_ptr, float *out) {
+// With DBG, each board's raw fp32 fc1 accumulator (before the 2^-10, the bias and the LeakyReLU) is also written to dbg + ridx * 128, in
+// torch column order (b200_debug_tc_acts returns it).  Only k_tdc_fc_dbg instantiates it.
+template <int NT, bool DBG>
+__device__ __forceinline__ void tdc_fc_body(DistNetWeights W, DnTcWeights TW, const uint8_t *act2, int n_tiles_alloc, const uint2 *req,
+                                            const int32_t *n_req_ptr, float *out, float *dbg) {
     extern __shared__ __align__(128) uint8_t smem[];
     uint64_t *full = reinterpret_cast<uint64_t *>(smem + TDF_OFF_BAR);
     uint64_t *empty = full + TDF_STAGES;
@@ -322,6 +324,18 @@ k_tdc_fc(DistNetWeights W, DnTcWeights TW, const uint8_t *act2, int n_tiles_allo
             }
             wgmma_wait<0>();
             fence_regs(d);
+            if constexpr (DBG) {
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int r = tile * 128 + wg * 64 + 16 * w + 8 * h + rl;
+                    if (r < n_req)
+#pragma unroll
+                        for (int j = 0; j < 16; ++j) {
+                            dbg[(size_t)r * 128 + 8 * j + 2 * qd] = d[4 * j + 2 * h];
+                            dbg[(size_t)r * 128 + 8 * j + 2 * qd + 1] = d[4 * j + 2 * h + 1];
+                        }
+                }
+            }
             if (wt == 0) mbar_arrive(&empty[prev]);
 #pragma unroll
             for (int j = 0; j < 16; ++j)
@@ -362,6 +376,17 @@ k_tdc_fc(DistNetWeights W, DnTcWeights TW, const uint8_t *act2, int n_tiles_allo
             wg_sync(wg);                                 // h is rewritten by the next tile's epilogue
         }
     }
+}
+
+template <int NT>
+__global__ void __launch_bounds__(TDF_THREADS, 1)
+k_tdc_fc(DistNetWeights W, DnTcWeights TW, const uint8_t *act2, int n_tiles_alloc, const uint2 *req, const int32_t *n_req_ptr, float *out) {
+    tdc_fc_body<NT, false>(W, TW, act2, n_tiles_alloc, req, n_req_ptr, out, nullptr);
+}
+template <int NT>
+__global__ void __launch_bounds__(TDF_THREADS, 1)
+k_tdc_fc_dbg(DistNetWeights W, DnTcWeights TW, const uint8_t *act2, int n_tiles_alloc, const uint2 *req, const int32_t *n_req_ptr, float *out, float *dbg) {
+    tdc_fc_body<NT, true>(W, TW, act2, n_tiles_alloc, req, n_req_ptr, out, dbg);
 }
 
 // ---------------------------------------------------------------------------------------------------- host side
@@ -424,6 +449,8 @@ static int dn_tc_prepare(void **state, const float *w, int atoms, cudaStream_t s
     if (cudaFuncSetAttribute(k_tdc_conv_dbg<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, TDC_SMEM) != cudaSuccess) return 1;
     if (cudaFuncSetAttribute(k_tdc_fc<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, TDF_SMEM) != cudaSuccess) return 1;
     if (cudaFuncSetAttribute(k_tdc_fc<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, TDF_SMEM) != cudaSuccess) return 1;
+    if (cudaFuncSetAttribute(k_tdc_fc_dbg<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, TDF_SMEM) != cudaSuccess) return 1;
+    if (cudaFuncSetAttribute(k_tdc_fc_dbg<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, TDF_SMEM) != cudaSuccess) return 1;
     return 0;
 }
 

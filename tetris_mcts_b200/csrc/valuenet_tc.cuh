@@ -502,9 +502,11 @@ static_assert(2 * TCF_STAGES * 8 <= 256, "barrier block overflows into the epilo
 constexpr int TCF_SMEM = TCF_OFF_EPI + (256 * 3 + 8) * 4;
 static_assert(TCF_SMEM <= 227 * 1024, "k_tc_fc shared memory");
 
-template <int NT>
-__global__ void __launch_bounds__(TCF_THREADS, 1)
-k_tc_fc(NetWeights W, TcWeights TW, const uint8_t *act3, int n_tiles_alloc, const uint2 *req, const int32_t *n_req_ptr, float2 *eval_out) {
+// With DBG, each board's raw fp32 fc1 accumulator (before the 2^-10, the bias and the ReLU) is also written to dbg + ridx * 256, in torch
+// column order (b200_debug_tc_acts returns it).  Only k_tc_fc_dbg instantiates it.
+template <int NT, bool DBG>
+__device__ __forceinline__ void tc_fc_body(NetWeights W, TcWeights TW, const uint8_t *act3, int n_tiles_alloc, const uint2 *req, const int32_t *n_req_ptr,
+                                           float2 *eval_out, float *dbg) {
     extern __shared__ __align__(128) uint8_t smem[];
     uint64_t *full = reinterpret_cast<uint64_t *>(smem + TCF_OFF_BAR);     // [stage] operands landed
     uint64_t *empty = full + TCF_STAGES;                                    // [stage] operands consumed (one arrival per consumer warpgroup)
@@ -564,6 +566,18 @@ k_tc_fc(NetWeights W, TcWeights TW, const uint8_t *act3, int n_tiles_alloc, cons
             }
             wgmma_wait<0>();
             fence_regs(d);
+            if constexpr (DBG) {
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int ridx = tile * 128 + wg * 64 + 16 * w + 8 * h + rl;
+                    if (ridx < n_req)
+#pragma unroll
+                        for (int j = 0; j < 32; ++j) {
+                            dbg[(size_t)ridx * 256 + 8 * j + 2 * qd] = d[4 * j + 2 * h];
+                            dbg[(size_t)ridx * 256 + 8 * j + 2 * qd + 1] = d[4 * j + 2 * h + 1];
+                        }
+                }
+            }
             if ((t & 127) == 0) mbar_arrive(&empty[prev]);
             float p0[2] = {0.f, 0.f}, p1[2] = {0.f, 0.f};
 #pragma unroll
@@ -591,6 +605,18 @@ k_tc_fc(NetWeights W, TcWeights TW, const uint8_t *act3, int n_tiles_alloc, cons
             }
         }
     }
+}
+
+template <int NT>
+__global__ void __launch_bounds__(TCF_THREADS, 1)
+k_tc_fc(NetWeights W, TcWeights TW, const uint8_t *act3, int n_tiles_alloc, const uint2 *req, const int32_t *n_req_ptr, float2 *eval_out) {
+    tc_fc_body<NT, false>(W, TW, act3, n_tiles_alloc, req, n_req_ptr, eval_out, nullptr);
+}
+template <int NT>
+__global__ void __launch_bounds__(TCF_THREADS, 1)
+k_tc_fc_dbg(NetWeights W, TcWeights TW, const uint8_t *act3, int n_tiles_alloc, const uint2 *req, const int32_t *n_req_ptr, float2 *eval_out,
+            float *dbg) {
+    tc_fc_body<NT, true>(W, TW, act3, n_tiles_alloc, req, n_req_ptr, eval_out, dbg);
 }
 
 // ---------------------------------------------------------------------------------------------------- host side
@@ -673,6 +699,8 @@ static int tc_prepare(void **state, const float *w, cudaStream_t stream) {
     if (cudaFuncSetAttribute(k_tc_conv_dbg<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, TCC_SMEM) != cudaSuccess) return 1;
     if (cudaFuncSetAttribute(k_tc_fc<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, TCF_SMEM) != cudaSuccess) return 1;
     if (cudaFuncSetAttribute(k_tc_fc<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, TCF_SMEM) != cudaSuccess) return 1;
+    if (cudaFuncSetAttribute(k_tc_fc_dbg<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, TCF_SMEM) != cudaSuccess) return 1;
+    if (cudaFuncSetAttribute(k_tc_fc_dbg<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, TCF_SMEM) != cudaSuccess) return 1;
     return 0;
 }
 
