@@ -260,6 +260,13 @@ int b200_trainer_set_weights(b200_trainer *t, const float *weights);            
 int b200_trainer_get_state(b200_trainer *t, float *exp_avg, float *exp_avg_sq, int64_t *step);   /* optimizer.state_dict(); step -1 = no state yet */
 int b200_trainer_set_state(b200_trainer *t, const float *exp_avg, const float *exp_avg_sq, int64_t step);   /* load_state_dict; step < 0 = reset_optimizer */
 int b200_trainer_get_grads(b200_trainer *t, float *grads_out);                                   /* p.grad of the last step, state_dict order (478338 floats) */
+/* test aid: a copy of one batch buffer as the last step / loss / step_rows_dev / grad_rows_dev left it, rows [0, n_rows) (fp32, row-major;
+ * conv activations and their gradients NHWC [n][pixel][32], im2col buffers [n][pixel][ci*9 + ky*3 + kx]).  which: "x0" [200], "value",
+ * "variance", "weight" [1], "col1" [144*9], "a1" [144*32], "col2" [96*288], "a2" [96*32], "col3" [56*288], "a3" [56*32], "flat" [1792]
+ * (torch flatten order), "h" [256], "pred" [2], "lossv" [1], "dz" [2], "dh" [256], "dflat" [1792], "dc3" [56*32], "dcol3" [56*288],
+ * "da2" [96*32], "dcol2" [96*288], "da1" [144*32]; or "d_sumsq": the last step's 10 per-tensor gradient sums of squares (double, n_rows
+ * ignored).  Launches no kernel.  B200_ERR_BAD_ARG for an unknown name or n_rows outside [0, max_batch]. */
+int b200_trainer_debug_buffer(b200_trainer *t, const char *which, int n_rows, void *out);
 /* Model_VV._loss under no_grad on one chunk (Model.compute_loss, model/model.py:52-83): mean and population std of (weight *) logl; pred_out NULL or [n][2] */
 int b200_trainer_loss(b200_trainer *t, const int8_t *states, const float *value, const float *variance, const float *weight, int n,
                       int weighted, double *loss, double *loss_std, float *pred_out);

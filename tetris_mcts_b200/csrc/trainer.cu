@@ -899,6 +899,27 @@ extern "C" int b200_trainer_get_grads(b200_trainer *t, float *grads_out) {      
     return B200_OK;
 }
 
+// test aid: one batch buffer as the last step / loss / step_rows_dev / grad_rows_dev left it, rows [0, n_rows) (a copy, no kernel)
+extern "C" int b200_trainer_debug_buffer(b200_trainer *t, const char *which, int n_rows, void *out) {
+    if (!t || !which || !out || n_rows < 0 || n_rows > t->max_batch) return tfail(B200_ERR_BAD_ARG, "trainer: bad argument (0 <= n_rows <= max_batch)");
+    const struct { const char *name; const float *p; size_t row; } bufs[] = {
+        {"x0", t->x0, 200}, {"value", t->value, 1}, {"variance", t->variance, 1}, {"weight", t->weight, 1},
+        {"col1", t->col1, 144 * 9}, {"a1", t->a1, 144 * 32}, {"col2", t->col2, 96 * 288}, {"a2", t->a2, 96 * 32},
+        {"col3", t->col3, 56 * 288}, {"a3", t->a3, 56 * 32}, {"flat", t->flat, 1792}, {"h", t->h, 256}, {"pred", t->pred, 2},
+        {"lossv", t->lossv, 1}, {"dz", t->dz, 2}, {"dh", t->dh, 256}, {"dflat", t->dflat, 1792}, {"dc3", t->dc3, 56 * 32},
+        {"dcol3", t->dcol3, 56 * 288}, {"da2", t->da2, 96 * 32}, {"dcol2", t->dcol2, 96 * 288}, {"da1", t->da1, 144 * 32}};
+    const void *src = nullptr;
+    size_t bytes = 0;
+    if (!strcmp(which, "d_sumsq")) { src = t->d_sumsq; bytes = N_TENSORS * sizeof(double); }
+    for (const auto &b : bufs)
+        if (!strcmp(which, b.name)) { src = b.p; bytes = (size_t)n_rows * b.row * sizeof(float); }
+    if (!src) return tfail(B200_ERR_BAD_ARG, std::string("trainer: unknown buffer ") + which);
+    TCK(cudaSetDevice(t->device));
+    if (bytes) TCK(cudaMemcpyAsync(out, src, bytes, cudaMemcpyDeviceToHost, t->stream));
+    TCK(cudaStreamSynchronize(t->stream));
+    return B200_OK;
+}
+
 // Model_VV._loss under torch.no_grad (one chunk of Model.compute_loss, model/model.py:52-83); pred_out (may be NULL): [n][2] = (v, var)
 extern "C" int b200_trainer_loss(b200_trainer *t, const int8_t *states, const float *value, const float *variance, const float *weight, int n,
                                  int weighted, double *loss, double *loss_std, float *pred_out) {

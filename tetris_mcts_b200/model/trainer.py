@@ -13,6 +13,10 @@ from .. import _lib as L
 N_TRAIN = 478338            # trainable floats (state_dict order without out_ubound / out_lbound)
 GRAD_VEC = N_TRAIN + 3      # doubles of one data-parallel gradient slice: the fp64 gradient, then the slice's loss {count, mean, M2}
 KINDS = {"fp64": 0, "tc": 1}  # B200_TRAIN_FP64, B200_TRAIN_TC
+# floats per batch row of each buffer b200_trainer_debug_buffer reads (include/b200_tetris_mcts.h)
+DEBUG_ROWS = {"x0": 200, "value": 1, "variance": 1, "weight": 1, "col1": 144 * 9, "a1": 144 * 32, "col2": 96 * 288, "a2": 96 * 32,
+              "col3": 56 * 288, "a3": 56 * 32, "flat": 1792, "h": 256, "pred": 2, "lossv": 1, "dz": 2, "dh": 256, "dflat": 1792,
+              "dc3": 56 * 32, "dcol3": 56 * 288, "da2": 96 * 32, "dcol2": 96 * 288, "da1": 144 * 32}
 P = C.c_void_p
 _sig_done = False
 
@@ -42,6 +46,7 @@ def _lib():
         lib.b200_trainer_grad_rows_dev.argtypes = [P, P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_uint64, C.c_int64, C.c_float, C.c_int, P]
         lib.b200_trainer_apply_grads_dev.argtypes = [P, P, C.c_int, C.c_double, C.c_int]
         lib.b200_trainer_read_log.argtypes = [P, C.c_int, P]
+        lib.b200_trainer_debug_buffer.argtypes = [P, C.c_char_p, C.c_int, P]
         _sig_done = True
     return lib
 
@@ -135,6 +140,16 @@ class Trainer:
         g = np.zeros(N_TRAIN, np.float32)
         _check(_lib().b200_trainer_get_grads(self.h, L.ptr(g)))
         return g
+
+    def debug_buffer(self, name, n):
+        """test aid: batch buffer `name` (DEBUG_ROWS) as the last step / loss / step_rows_dev / grad_rows_dev left it, rows [0, n) ->
+        float32 [n, row]; "d_sumsq": the last step's per-tensor gradient sums of squares, float64 [10]"""
+        if name == "d_sumsq":
+            out = np.zeros(10, np.float64)
+        else:
+            out = np.zeros((max(int(n), 0), DEBUG_ROWS.get(name, 1)), np.float32)
+        _check(_lib().b200_trainer_debug_buffer(self.h, name.encode(), int(n), L.ptr(out)))
+        return out
 
     def loss(self, batch, weighted=False, want_pred=False):
         """Model_VV._loss under no_grad on one chunk: (mean, population std[, pred (n,2)])"""
