@@ -34,7 +34,10 @@ enum { B200_MODE_LP = 0,        /* agents/ValueSimLP.py:13-70 */
        B200_MODE_VANILLA = 2,   /* agents/Vanilla.py:17-64 */
        B200_MODE_DIST = 3 };    /* agents/core_distributional.py:82-124 driven as agents/DistValueSimOnline.py:36-75 sketches */
 enum { B200_EVAL_SYNTHETIC = 0, /* test evaluator (hash of the observation), shared with the CPU oracle */
-       B200_EVAL_NET = 1,       /* model/model_vv.py Model_VV.inference, fp32 CUDA cores */
+       B200_EVAL_NET = 1,       /* model/model_vv.py Model_VV.inference, fp32 CUDA cores.  Takes finite weights of any size, so a sum can
+                                   overflow fp32 to +-inf, and inf - inf gives NaN.  The value network's ReLU is fmaxf, and fmaxf(NaN, 0)
+                                   is 0 where torch's relu keeps the NaN: such a board gets finite (and wrong) v and var where the fp32
+                                   reference returns NaN.  The distributional network's LeakyReLU keeps NaN (DESIGN §5). */
        B200_EVAL_NET_TC = 2,    /* same network on wgmma tensor cores (fp16 x 2 operand split, 3 products per product); in B200_MODE_DIST:
                                    model/model_distributional.py on tensor cores (csrc/distnet_tc.cuh) instead of the fp32 CUDA-core kernels */
        B200_EVAL_NET_FP16 = 3,  /* same weights and tensor-core kernels as B200_EVAL_NET_TC with ONE fp16 term per operand and one product per
@@ -203,6 +206,13 @@ int b200_debug_dist_act2(b200_engine *e, const int8_t *states, int k, float *out
  * raw fp32 accumulator, out[k][256] / out[k][128] in torch column order (the value before the 2^-10, the bias and the activation).
  * layer 0: the same pass's outputs, out[k][2] = (v, var) or out[k][atoms] = probabilities. */
 int b200_debug_tc_acts(b200_engine *e, int dist, const int8_t *states, int k, int layer, float *out);
+/* test aid: every stage of an fp32 CUDA-core network (B200_EVAL_NET only; other kinds, dist not 0 / 1 or a layer outside 0..4 return
+ * B200_ERR_BAD_ARG, a network without weights B200_ERR_NO_WEIGHTS) exactly as the kernels computed it, from one forward pass on
+ * states[k][200].  dist = 0, the value network: layer 0 = (v, var) out[k][2], 1 = act1 [32][18][8], 2 = act2 [32][16][6], 3 = act3
+ * [32][14][4] (the production buffer fc1 reads), 4 = fc1's fp32 accumulator out[k][256] in torch column order (before the bias and the
+ * ReLU).  dist = 1, the distributional network: layer 0 = probabilities out[k][atoms], 1 = act1 [32][19][7], 2 = act2 [32][16][4] (the
+ * production buffer), 3 = fc1's accumulator out[k][128] (bias included, before the LeakyReLU), 4 = the logits out[k][atoms]. */
+int b200_debug_net_acts(b200_engine *e, int dist, const int8_t *states, int k, int layer, float *out);
 int b200_export_dist(b200_engine *e, int game, float *node_stats /* [M][5] */, float *node_dist /* [M][bins] */);
 
 /* --- replay samples of the live search (ValueSim.store_nodes, agents/ValueSim.py:122-159): observations with

@@ -94,6 +94,7 @@ def lib():
         L.b200_distnet_forward.argtypes = [P, P, C.c_int, C.c_int, P]
         L.b200_debug_dist_act2.argtypes = [P, P, C.c_int, P]
         L.b200_debug_tc_acts.argtypes = [P, C.c_int, P, C.c_int, C.c_int, P]
+        L.b200_debug_net_acts.argtypes = [P, C.c_int, P, C.c_int, C.c_int, P]
         L.b200_export_dist.argtypes = [P, C.c_int, P, P]
         L.b200_dist_shift_distribution.argtypes = [P, C.c_int, C.c_double, C.c_double, C.c_double, P]
         L.b200_dist_mean_variance.argtypes = [P, C.c_int, C.c_double, C.c_double, P, P]

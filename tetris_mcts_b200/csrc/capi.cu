@@ -351,6 +351,7 @@ extern "C" int b200_load_weights(b200_engine *e, const float *w) {
     e->W.wfc1 = e->W.b1 + 96; e->W.bfc1 = e->W.wfc1 + (size_t)1792 * 256; e->W.wout = e->W.bfc1 + 256;
     e->W.bout = e->W.wout + 512; e->W.ub = e->W.bout + 2; e->W.lb = e->W.bout + 4;
     CK(cudaFuncSetAttribute(k_vn_conv, cudaFuncAttributeMaxDynamicSharedMemorySize, VN_SMEM_BYTES));
+    CK(cudaFuncSetAttribute(k_vn_conv_dbg, cudaFuncAttributeMaxDynamicSharedMemorySize, VN_SMEM_BYTES));
     {
         int rc = tc_prepare(&e->tc_state, w, e->stream);
         if (rc) return fail(B200_ERR_CUDA, "tensor-core weight preparation failed");
@@ -368,9 +369,9 @@ static int ensure_act3(b200_engine *e, size_t rows) {
     return 0;
 }
 
-// run the network over the request list req[0..*n_req) -> eval_out; device-side count, no host sync.  dbg (tensor-core kinds,
-// standalone requests only): run k_tc_conv_dbg and k_tc_fc_dbg instead, which also copy act1 / act2 there (TCC_DBG_BYTES per request)
-// and fc1's fp32 accumulator to dbg_fc (256 floats per request)
+// run the network over the request list req[0..*n_req) -> eval_out; device-side count, no host sync.  dbg (standalone requests only):
+// run the DBG instantiations instead, which also copy act1 / act2 there (tensor-core kinds: k_tc_conv_dbg, TCC_DBG_BYTES per request;
+// net: k_vn_conv_dbg, VN_DBG_FLOATS floats per request) and fc1's fp32 accumulator to dbg_fc (256 floats per request)
 static int launch_net(b200_engine *e, const uint2 *req, const int32_t *n_req, const uint32_t *keys, int M, float2 *eval_out,
                       size_t max_rows, uint8_t *dbg = nullptr, float *dbg_fc = nullptr) {
     if (!e->have_weights) return fail(B200_ERR_NO_WEIGHTS, "b200_load_weights was not called");
@@ -400,6 +401,12 @@ static int launch_net(b200_engine *e, const uint2 *req, const int32_t *n_req, co
         const float *act3_before = e->d_act3;
         if (ensure_act3(e, max_rows)) return B200_ERR_CUDA;
         if (act3_before && e->d_act3 != act3_before) drop_step_graph(e);
+    }
+    if (dbg) {
+        k_vn_conv_dbg<<<e->n_sm, VN_THREADS, VN_SMEM_BYTES, e->stream>>>(e->W, req, n_req, keys, M, e->d_act3, reinterpret_cast<float *>(dbg));
+        k_vn_fc_dbg<<<e->n_sm * 2, FC_THREADS, 0, e->stream>>>(e->W, e->d_act3, req, n_req, eval_out, dbg_fc);
+        CK(cudaGetLastError());
+        return B200_OK;
     }
     {
         PhaseTimer t(e, PH_CONV);
@@ -438,16 +445,19 @@ extern "C" int b200_load_dist_weights(b200_engine *e, const float *w, int atoms)
     e->DW = dn_pointers(e->d_dnw, atoms);
     CK(cudaFuncSetAttribute(k_dn_conv, cudaFuncAttributeMaxDynamicSharedMemorySize, DN_CONV_SMEM));
     CK(cudaFuncSetAttribute(k_dn_fc, cudaFuncAttributeMaxDynamicSharedMemorySize, DN_FC_SMEM));
+    CK(cudaFuncSetAttribute(k_dn_conv_dbg, cudaFuncAttributeMaxDynamicSharedMemorySize, DN_CONV_SMEM));
+    CK(cudaFuncSetAttribute(k_dn_fc_dbg, cudaFuncAttributeMaxDynamicSharedMemorySize, DN_FC_SMEM));
     if (dn_tc_prepare(&e->dn_tc_state, w, atoms, e->stream)) return fail(B200_ERR_CUDA, "tensor-core weight preparation (distributional network) failed");
     e->have_dist_weights = true;
     drop_step_graph(e);
     return B200_OK;
 }
 
-// dbg (tensor-core kinds, standalone requests only): run k_tdc_conv_dbg and k_tdc_fc_dbg instead, which also copy act1 there (TDC_ASLOT
-// per request) and fc1's fp32 accumulator to dbg_fc (128 floats per request)
+// dbg (standalone requests only): run the DBG instantiations instead, which also copy act1 there (tensor-core kinds: k_tdc_conv_dbg,
+// TDC_ASLOT per request; net: k_dn_conv_dbg, DN_DBG_A1 floats per request) and fc1's fp32 accumulator to dbg_fc (128 floats per
+// request); net's k_dn_fc_dbg also copies the logits to dbg_lg (atoms floats per request)
 static int launch_distnet_on(b200_engine *e, const uint2 *req, const int32_t *n_req, const uint32_t *keys, int M, float *out, size_t max_rows,
-                             uint8_t *dbg = nullptr, float *dbg_fc = nullptr) {
+                             uint8_t *dbg = nullptr, float *dbg_fc = nullptr, float *dbg_lg = nullptr) {
     if (!e->have_dist_weights) return fail(B200_ERR_NO_WEIGHTS, "b200_load_dist_weights was not called");
     if (dn_tc_net(e)) {
         DnTcState *st = (DnTcState *)e->dn_tc_state;
@@ -480,6 +490,12 @@ static int launch_distnet_on(b200_engine *e, const uint2 *req, const int32_t *n_
         e->dn_rows = max_rows;
         if (had) drop_step_graph(e);
     }
+    if (dbg) {
+        k_dn_conv_dbg<<<e->n_sm * 2, DN_THREADS, DN_CONV_SMEM, e->stream>>>(e->DW, req, n_req, keys, M, e->d_dn_act, reinterpret_cast<float *>(dbg));
+        k_dn_fc_dbg<<<e->n_sm, DN_THREADS, DN_FC_SMEM, e->stream>>>(e->DW, e->d_dn_act, req, n_req, out, dbg_fc, dbg_lg);
+        CK(cudaGetLastError());
+        return B200_OK;
+    }
     {
         PhaseTimer t(e, PH_CONV);
         k_dn_conv<<<e->n_sm * 2, DN_THREADS, DN_CONV_SMEM, e->stream>>>(e->DW, req, n_req, keys, M, e->d_dn_act);
@@ -496,7 +512,8 @@ static int launch_distnet(b200_engine *e) {
 }
 
 // Model.inference of model/model_distributional.py (softmax over atoms): states[k][200] int8 -> dist[k][atoms]
-static int distnet_forward(b200_engine *e, const int8_t *states, int k, int atoms, float *dist, uint8_t *dbg, float *dbg_fc) {
+static int distnet_forward(b200_engine *e, const int8_t *states, int k, int atoms, float *dist, uint8_t *dbg, float *dbg_fc,
+                           float *dbg_lg = nullptr) {
     if (!e || !states || !dist || k < 1 || atoms != e->DW.atoms) return fail(B200_ERR_BAD_ARG, "bad argument (atoms must match the loaded weights)");
     CK(cudaSetDevice(e->cfg.device));
     int8_t *d_states = nullptr; uint32_t *d_keys = nullptr; uint2 *d_req = nullptr; int32_t *d_n = nullptr; float *d_out = nullptr;
@@ -507,7 +524,7 @@ static int distnet_forward(b200_engine *e, const int8_t *states, int k, int atom
     CK(cudaMemcpyAsync(d_n, &k, 4, cudaMemcpyHostToDevice, e->stream));
     k_states_to_keys<<<(k + 127) / 128, 128, 0, e->stream>>>(d_states, k, d_keys, d_req);
     k_dn_req_rows<<<(k + 127) / 128, 128, 0, e->stream>>>(d_req, k);      // request i -> output row i
-    int rc = launch_distnet_on(e, d_req, d_n, d_keys, 0, d_out, (size_t)k, dbg, dbg_fc);
+    int rc = launch_distnet_on(e, d_req, d_n, d_keys, 0, d_out, (size_t)k, dbg, dbg_fc, dbg_lg);
     if (rc == B200_OK) {
         cudaError_t ce = cudaMemcpyAsync(dist, d_out, (size_t)k * atoms * 4, cudaMemcpyDeviceToHost, e->stream);
         if (ce == cudaSuccess) ce = cudaStreamSynchronize(e->stream);
@@ -1146,6 +1163,56 @@ extern "C" int b200_debug_tc_acts(b200_engine *e, int dist, const int8_t *states
                         uint16_t hb; memcpy(&hb, &h[off(r, s, c, y, x)], 2);
                         out[((((size_t)r * nt + s) * 32 + c) * H + y) * Wd + x] = host_half_f(hb) / TC_SCALE_A;
                     }
+    return B200_OK;
+}
+
+// development / test aid: every stage of the fp32 CUDA-core networks (eval_kind net) exactly as the kernels computed it, from one forward
+// pass that runs the DBG instantiations k_vn_conv_dbg / k_vn_fc_dbg or k_dn_conv_dbg / k_dn_fc_dbg
+extern "C" int b200_debug_net_acts(b200_engine *e, int dist, const int8_t *states, int k, int layer, float *out) {
+    if (!e || !states || !out || k < 1) return fail(B200_ERR_BAD_ARG, "bad argument");
+    if (e->cfg.eval_kind != B200_EVAL_NET) return fail(B200_ERR_BAD_ARG, "b200_debug_net_acts reads the fp32 CUDA-core networks: eval_kind net");
+    if (dist != 0 && dist != 1) return fail(B200_ERR_BAD_ARG, "dist must be 0 (value network) or 1 (distributional network)");
+    if (layer < 0 || layer > 4) return fail(B200_ERR_BAD_ARG, "layer out of range");
+    if (dist ? !e->have_dist_weights : !e->have_weights) return fail(B200_ERR_NO_WEIGHTS, "no weights loaded for this network");
+    const int atoms = e->DW.atoms;
+    const size_t slot = dist ? DN_DBG_A1 : VN_DBG_FLOATS, n_fc1 = dist ? 128 : 256;
+    float *d_dbg = nullptr, *d_fc = nullptr, *d_lg = nullptr;
+    Scratch tmp;
+    CK(tmp.get(&d_dbg, (size_t)k * slot * 4));
+    CK(tmp.get(&d_fc, (size_t)k * n_fc1 * 4));
+    if (dist) CK(tmp.get(&d_lg, (size_t)k * atoms * 4));
+    std::vector<float> o0((size_t)k * (dist ? atoms : 2));
+    int rc;
+    if (dist) rc = distnet_forward(e, states, k, atoms, o0.data(), reinterpret_cast<uint8_t *>(d_dbg), d_fc, d_lg);
+    else {
+        std::vector<float> v(k), var(k);
+        rc = valuenet_forward(e, states, k, v.data(), var.data(), reinterpret_cast<uint8_t *>(d_dbg), d_fc);
+        for (int r = 0; r < k; ++r) { o0[2 * r] = v[r]; o0[2 * r + 1] = var[r]; }
+    }
+    if (rc) return rc;
+    if (layer == 0) { memcpy(out, o0.data(), o0.size() * 4); return B200_OK; }
+    const float *src = nullptr;        // layers already in their output layout: copied as they are
+    size_t n = 0;
+    if (dist) {
+        if (layer == 1) { src = d_dbg; n = (size_t)k * DN_DBG_A1; }                  // act1 [32][19][7]
+        else if (layer == 2) { src = e->d_dn_act; n = (size_t)k * 2048; }        // act2 [32][16][4], the production buffer
+        else if (layer == 3) { src = d_fc; n = (size_t)k * 128; }                // fc1, bias included, before the LeakyReLU
+        else { src = d_lg; n = (size_t)k * atoms; }                              // logits
+    } else if (layer == 4) { src = d_fc; n = (size_t)k * 256; }                  // fc1's accumulator, before the bias and the ReLU
+    if (src) { CK(cudaMemcpy(out, src, n * 4, cudaMemcpyDeviceToHost)); return B200_OK; }
+    if (layer == 3) {                                                            // act3 [32][14][4] from the production buffer
+        std::vector<float> h((size_t)k * 1792);
+        CK(cudaMemcpy(h.data(), e->d_act3, h.size() * 4, cudaMemcpyDeviceToHost));
+        for (int r = 0; r < k; ++r)
+            for (int y = 0; y < 14; ++y)
+                for (int c = 0; c < 32; ++c)
+                    for (int x = 0; x < 4; ++x) out[(size_t)r * 1792 + c * 56 + y * 4 + x] = h[(size_t)r * 1792 + (y * 32 + c) * 4 + x];
+        return B200_OK;
+    }
+    std::vector<float> h((size_t)k * VN_DBG_FLOATS);                             // act1 [32][18][8] | act2 [32][16][6] per board
+    CK(cudaMemcpy(h.data(), d_dbg, h.size() * 4, cudaMemcpyDeviceToHost));
+    const int off = layer == 1 ? 0 : VN_DBG_A1, len = layer == 1 ? VN_DBG_A1 : VN_DBG_FLOATS - VN_DBG_A1;
+    for (int r = 0; r < k; ++r) memcpy(out + (size_t)r * len, h.data() + (size_t)r * VN_DBG_FLOATS + off, (size_t)len * 4);
     return B200_OK;
 }
 

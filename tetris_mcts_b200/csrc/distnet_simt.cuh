@@ -59,9 +59,13 @@ __global__ void k_dn_req_rows(uint2 *req, int k) {   // standalone inference: re
     if (i < k) req[i] = make_uint2((uint32_t)i, (uint32_t)i);
 }
 
-// conv stack: persistent CTAs, one board per pass; act2 [request][2048] in NCHW flatten order
-__global__ void __launch_bounds__(DN_THREADS) k_dn_conv(DistNetWeights W, const uint2 *req, const int32_t *n_req_ptr, const uint32_t *keys, int M,
-                                                       float *act) {
+// conv stack: persistent CTAs, one board per pass; act2 [request][2048] in NCHW flatten order.  With DBG, each board's act1 [32][19][7] is
+// also copied to dbg + ridx * DN_DBG_A1 once conv1 has finished (b200_debug_net_acts returns it).  Only k_dn_conv_dbg instantiates it.
+constexpr int DN_DBG_A1 = 32 * 133;
+
+template <bool DBG>
+__device__ __forceinline__ void dn_conv_body(DistNetWeights W, const uint2 *req, const int32_t *n_req_ptr, const uint32_t *keys, int M, float *act,
+                                             float *dbg) {
     extern __shared__ __align__(16) float sm[];
     float *sW2 = sm, *sW1 = sW2 + 512 * 32, *sB = sW1 + 16 * 32, *sIn = sB + 64, *sA1 = sIn + 220;   // sA1 [32][136] (19x7 = 133 used)
     const int t = threadIdx.x;
@@ -102,6 +106,9 @@ __global__ void __launch_bounds__(DN_THREADS) k_dn_conv(DistNetWeights W, const 
             for (int j = 0; j < 8; ++j) sA1[(cq * 8 + j) * 136 + pix] = leaky(acc[j]);
         }
         __syncthreads();
+        if constexpr (DBG) {   // sA1 stays unchanged until the next board's first __syncthreads
+            for (int i = t; i < DN_DBG_A1; i += DN_THREADS) dbg[(size_t)ridx * DN_DBG_A1 + i] = sA1[(i / 133) * 136 + i % 133];
+        }
         {   // conv2: thread = (pixel of 16x4, 8-cout chunk): 64 x 4 = 256 threads
             const int cq = t >> 6, pix = t & 63, y = pix >> 2, x = pix & 3;
             float acc[8];
@@ -125,8 +132,21 @@ __global__ void __launch_bounds__(DN_THREADS) k_dn_conv(DistNetWeights W, const 
     }
 }
 
-// fc1 + LeakyReLU + fc_v + softmax; DN_FC_ROWS boards per CTA pass; output row = req.x (the game) * atoms
-__global__ void __launch_bounds__(DN_THREADS) k_dn_fc(DistNetWeights W, const float *act, const uint2 *req, const int32_t *n_req_ptr, float *out) {
+__global__ void __launch_bounds__(DN_THREADS) k_dn_conv(DistNetWeights W, const uint2 *req, const int32_t *n_req_ptr, const uint32_t *keys, int M,
+                                                       float *act) {
+    dn_conv_body<false>(W, req, n_req_ptr, keys, M, act, nullptr);
+}
+__global__ void __launch_bounds__(DN_THREADS) k_dn_conv_dbg(DistNetWeights W, const uint2 *req, const int32_t *n_req_ptr, const uint32_t *keys,
+                                                           int M, float *act, float *dbg) {
+    dn_conv_body<true>(W, req, n_req_ptr, keys, M, act, dbg);
+}
+
+// fc1 + LeakyReLU + fc_v + softmax; DN_FC_ROWS boards per CTA pass; output row = req.x (the game) * atoms.  With DBG, each row's fc1
+// accumulator (bias included, before the LeakyReLU) is also written to dbg_fc + ridx * 128, and its logits (before the softmax overwrites
+// them) to dbg_lg + ridx * atoms (b200_debug_net_acts returns both).  Only k_dn_fc_dbg instantiates it.
+template <bool DBG>
+__device__ __forceinline__ void dn_fc_body(DistNetWeights W, const float *act, const uint2 *req, const int32_t *n_req_ptr, float *out, float *dbg_fc,
+                                           float *dbg_lg) {
     extern __shared__ __align__(16) float sm[];
     float *sA = sm, *sH = sA + DN_FC_ROWS * 2048, *sL = sH + DN_FC_ROWS * 128;
     const int t = threadIdx.x, n_req = *n_req_ptr, atoms = W.atoms;
@@ -145,6 +165,11 @@ __global__ void __launch_bounds__(DN_THREADS) k_dn_fc(DistNetWeights W, const fl
             }
 #pragma unroll
             for (int r = 0; r < 4; ++r) sH[(r0 + r) * 128 + n] = leaky(acc[r]);
+            if constexpr (DBG) {
+#pragma unroll
+                for (int r = 0; r < 4; ++r)
+                    if (r0 + r < rows) dbg_fc[(size_t)(base + r0 + r) * 128 + n] = acc[r];
+            }
         }
         __syncthreads();
         for (int task = t; task < rows * atoms; task += DN_THREADS) {     // fc_v logits
@@ -152,6 +177,7 @@ __global__ void __launch_bounds__(DN_THREADS) k_dn_fc(DistNetWeights W, const fl
             float acc = W.bfv[a];
             for (int k = 0; k < 128; ++k) acc = fmaf(sH[r * 128 + k], W.wfv[(size_t)k * atoms + a], acc);
             sL[r * 64 + a] = acc;
+            if constexpr (DBG) dbg_lg[(size_t)(base + r) * atoms + a] = acc;
         }
         __syncthreads();
         if (t < rows) {                                                    // softmax (F.softmax(x, 1), model_distributional.py:47-50)
@@ -163,6 +189,14 @@ __global__ void __launch_bounds__(DN_THREADS) k_dn_fc(DistNetWeights W, const fl
             for (int a = 0; a < atoms; ++a) dst[a] = sL[t * 64 + a] / sum;
         }
     }
+}
+
+__global__ void __launch_bounds__(DN_THREADS) k_dn_fc(DistNetWeights W, const float *act, const uint2 *req, const int32_t *n_req_ptr, float *out) {
+    dn_fc_body<false>(W, act, req, n_req_ptr, out, nullptr, nullptr);
+}
+__global__ void __launch_bounds__(DN_THREADS) k_dn_fc_dbg(DistNetWeights W, const float *act, const uint2 *req, const int32_t *n_req_ptr, float *out,
+                                                         float *dbg_fc, float *dbg_lg) {
+    dn_fc_body<true>(W, act, req, n_req_ptr, out, dbg_fc, dbg_lg);
 }
 
 }  // namespace b200

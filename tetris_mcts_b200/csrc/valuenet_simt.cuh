@@ -6,9 +6,11 @@
 //               resident in shared memory.  Output: act3[request][1792] in HBM, K order (y*32 + c)*4 + x.
 //   k_vn_fc   : act3 [R,1792] x W1' [1792,256] (+bias, ReLU) -> fc_out (2 dot products) -> sigmoid -> affine,
 //               64x256 output tile per CTA so the whole hidden vector of a row stays in the CTA.
-// Arithmetic is plain fp32 FMA with fp32 accumulation, the same precision class as the reference's torch CPU
-// path; results agree with it to ~1e-6 relative (tests use rtol 1e-5).  This is the bit-faithful baseline the
-// tensor-core path (valuenet_tc.cuh) is checked against.
+// Arithmetic is plain fp32 in a fixed order: fmaf chains, IEEE adds and divisions, a fixed shuffle tree and an explicit
+// __fmul_rn / __fadd_rn affine.  So every activation, fc1 accumulator and logit is one fp32 value, bit for bit the
+// restatement of tests/f32_net_ref.py from the previous stage, and each output lies within the few fp32 values that expf's
+// 2 ulp admit (tests/test_gpu_net_layers.py, which reads every stage back through the DBG instantiations and
+// b200_debug_net_acts).  This is the bit-faithful baseline the tensor-core path (valuenet_tc.cuh) is checked against.
 #pragma once
 #include "search_dev.cuh"
 
@@ -29,8 +31,14 @@ constexpr int VN_THREADS = 256;
 constexpr int VN_SMEM_FLOATS = 9216 * 2 + 288 + 96 + VN_TB * 200 + 32 * VN_TB * 18 * 8 + 32 * VN_TB * 16 * 8;
 constexpr int VN_SMEM_BYTES = VN_SMEM_FLOATS * 4;
 
-__global__ void __launch_bounds__(VN_THREADS, 1)
-k_vn_conv(NetWeights W, const uint2 *req, const int32_t *n_req_ptr, const uint32_t *keys, int M, float *act3) {
+// Test export of the activations that never leave shared memory: with DBG, each board's act1 [32][18][8] and act2 [32][16][6] are
+// copied to dbg + ridx * VN_DBG_FLOATS in [c][y][x] order once conv2 has finished (b200_debug_net_acts returns them).  Only k_vn_conv_dbg
+// instantiates it.
+constexpr int VN_DBG_A1 = 32 * 18 * 8, VN_DBG_FLOATS = VN_DBG_A1 + 32 * 16 * 6;
+
+template <bool DBG>
+__device__ __forceinline__ void vn_conv_body(NetWeights W, const uint2 *req, const int32_t *n_req_ptr, const uint32_t *keys, int M, float *act3,
+                                             float *dbg) {
     extern __shared__ __align__(16) float sm[];
     float *sW2 = sm;                       // 9216
     float *sW3 = sW2 + 9216;               // 9216
@@ -123,6 +131,21 @@ k_vn_conv(NetWeights W, const uint2 *req, const int32_t *n_req_ptr, const uint32
             }
         }
         __syncthreads();
+        if constexpr (DBG) {   // sA1 and sA2 stay unchanged until the next tile's first __syncthreads
+            for (int i = t; i < VN_TB * VN_DBG_FLOATS; i += VN_THREADS) {
+                const int b = i / VN_DBG_FLOATS, e = i - b * VN_DBG_FLOATS, ridx = tile * VN_TB + b;
+                if (ridx >= n_req) continue;
+                float v;
+                if (e < VN_DBG_A1) {
+                    const int c = e / 144, y = (e >> 3) % 18, x = e & 7;
+                    v = sA1[(x >> 2) * A1P + ((c * (VN_TB * 18) + b * 18 + y) * 4 + (x & 3))];
+                } else {
+                    const int e2 = e - VN_DBG_A1, c = e2 / 96, y = (e2 / 6) % 16, x = e2 % 6;
+                    v = sA2[(x >> 2) * A2P + ((c * (VN_TB * 16) + b * 16 + y) * 4 + (x & 3))];
+                }
+                dbg[(size_t)ridx * VN_DBG_FLOATS + e] = v;
+            }
+        }
         // ---- conv3 (32->32, 16x6 -> 14x4) + ReLU: thread = (cout group, board, output row < 14), 4 px x 8 cout
         {
             const int cg = t >> 6, by = t & 63, b = by >> 4, y = by & 15;
@@ -161,11 +184,23 @@ k_vn_conv(NetWeights W, const uint2 *req, const int32_t *n_req_ptr, const uint32
     }
 }
 
+__global__ void __launch_bounds__(VN_THREADS, 1)
+k_vn_conv(NetWeights W, const uint2 *req, const int32_t *n_req_ptr, const uint32_t *keys, int M, float *act3) {
+    vn_conv_body<false>(W, req, n_req_ptr, keys, M, act3, nullptr);
+}
+__global__ void __launch_bounds__(VN_THREADS, 1)
+k_vn_conv_dbg(NetWeights W, const uint2 *req, const int32_t *n_req_ptr, const uint32_t *keys, int M, float *act3, float *dbg) {
+    vn_conv_body<true>(W, req, n_req_ptr, keys, M, act3, dbg);
+}
+
 // ---------------------------------------------------------------------------------------------------- fc1 + head
 constexpr int FC_BM = 64, FC_BN = 256, FC_BK = 16, FC_THREADS = 256;
 
-__global__ void __launch_bounds__(FC_THREADS)
-k_vn_fc(NetWeights W, const float *act3, const uint2 *req, const int32_t *n_req_ptr, float2 *eval_out) {
+// With DBG, each row's fc1 accumulator (before the bias and the ReLU) is also written to dbg + ridx * 256 in torch column order
+// (b200_debug_net_acts returns it).  Only k_vn_fc_dbg instantiates it.
+template <bool DBG>
+__device__ __forceinline__ void vn_fc_body(NetWeights W, const float *act3, const uint2 *req, const int32_t *n_req_ptr, float2 *eval_out,
+                                           float *dbg) {
     __shared__ __align__(16) float sA[2][FC_BK][FC_BM];     // transposed: [k][row]
     __shared__ __align__(16) float sBm[2][FC_BK][FC_BN];
     const int n_req = *n_req_ptr;
@@ -221,6 +256,15 @@ k_vn_fc(NetWeights W, const float *act3, const uint2 *req, const int32_t *n_req_
             int col = (j < 4) ? tx * 4 + j : 128 + tx * 4 + (j - 4);
             bias[j] = W.bfc1[col]; wo0[j] = W.wout[col]; wo1[j] = W.wout[256 + col];
         }
+        if constexpr (DBG) {
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+                const int r = row0 + ty * 8 + i;
+                if (r < n_req)
+#pragma unroll
+                    for (int j = 0; j < 8; ++j) dbg[(size_t)r * 256 + ((j < 4) ? tx * 4 + j : 128 + tx * 4 + (j - 4))] = acc[i][j];
+            }
+        }
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
             float p0 = 0.f, p1 = 0.f;
@@ -245,6 +289,15 @@ k_vn_fc(NetWeights W, const float *act3, const uint2 *req, const int32_t *n_req_
         }
         __syncthreads();
     }
+}
+
+__global__ void __launch_bounds__(FC_THREADS)
+k_vn_fc(NetWeights W, const float *act3, const uint2 *req, const int32_t *n_req_ptr, float2 *eval_out) {
+    vn_fc_body<false>(W, act3, req, n_req_ptr, eval_out, nullptr);
+}
+__global__ void __launch_bounds__(FC_THREADS)
+k_vn_fc_dbg(NetWeights W, const float *act3, const uint2 *req, const int32_t *n_req_ptr, float2 *eval_out, float *dbg) {
+    vn_fc_body<true>(W, act3, req, n_req_ptr, eval_out, dbg);
 }
 
 }  // namespace b200
