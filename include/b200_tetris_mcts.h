@@ -257,10 +257,25 @@ int b200_trainer_create(int device, const float *weights, int max_batch, b200_tr
  *                    summed in a fixed order).  Loss, gradient norm and each gradient tensor stay within 1e-5 (relative, resp. of the
  *                    tensor's norm) of float64 arithmetic; fp32's exponent range is kept, so small gradients do not flush.  Bit-
  *                    reproducible run to run, and train_rows_dev stays bit-identical to step_rows_dev fed the same indices, as for fp64.
- * Weights and Yogi state mean the same in both kinds, so a checkpoint of one kind loads into the other.
+ *   B200_TRAIN_TF32  the same GEMMs on tensor cores with one tf32 term per operand (rna_tf32(x), |x - rna_tf32(x)| <= 2^-11 |x|): one
+ *                    wgmma per k8 instead of three, and the tc kind's accumulation (32-k tiles, round-to-nearest chunk sums over <= 2048 k,
+ *                    fp64 partials).  Per element: the exact products of the rounded operands, summed within tc's accumulation bound.
+ *                    Against float64: each GEMM output lies within 2^-10 (two operand roundings of 2^-11) of its |term| sum plus tc's
+ *                    accumulation (~1e-5), once per product on a result's path: the loss and loss_std stay within 4 * 2^-10 (four
+ *                    forward products), the gradient norm within 8 * 2^-10.  Gradient elements sum over pixels whose terms cancel and
+ *                    see the forward error through GaussianLL's mean - pred, so their bound is that error propagated through the
+ *                    head and the backward pass in absolute values (tests/test_gpu_trainer_tf32.py error_bound; measured up to a few
+ *                    percent of a tensor's norm, against 1e-5 for tc).  The convolutions are implicit GEMMs: conv1-3 gather their A operand from the NHWC activations (k =
+ *                    ci*9 + ky*3 + kx), the conv weight gradients gather col^T the same way, and the input gradients of conv3 / conv2 are
+ *                    one GEMM each, da[b][y][x][ci] = (act > 0) * sum over k = (ky*3 + kx)*32 + co (ascending, K = 288; taps outside
+ *                    the output gradient are zero terms) of dY[b][y-ky][x-kx][co] * W[co][ci][ky][kx].  So a tf32 trainer has no
+ *                    col1 / col2 / col3 / dcol3 / dcol2 buffers (355 392 B per sample of max_batch), and b200_trainer_debug_buffer
+ *                    returns B200_ERR_BAD_ARG for those names.  Bit-reproducible, train_rows_dev == step_rows_dev, as the other kinds.
+ * Weights and Yogi state mean the same in every kind, so a checkpoint of one kind loads into the others.
  * b200_trainer_create_kind returns B200_ERR_BAD_ARG for an unknown kind. */
 #define B200_TRAIN_FP64 0
 #define B200_TRAIN_TC 1
+#define B200_TRAIN_TF32 2
 int b200_trainer_create_kind(int device, const float *weights, int max_batch, int kind, b200_trainer **out);
 int b200_trainer_destroy(b200_trainer *t);
 int b200_trainer_set_hyper(b200_trainer *t, double lr, double beta1, double beta2, double eps, double weight_decay);   /* Yogi(...) model_vv.py:132 */
@@ -275,7 +290,8 @@ int b200_trainer_get_grads(b200_trainer *t, float *grads_out);                  
  * "variance", "weight" [1], "col1" [144*9], "a1" [144*32], "col2" [96*288], "a2" [96*32], "col3" [56*288], "a3" [56*32], "flat" [1792]
  * (torch flatten order), "h" [256], "pred" [2], "lossv" [1], "dz" [2], "dh" [256], "dflat" [1792], "dc3" [56*32], "dcol3" [56*288],
  * "da2" [96*32], "dcol2" [96*288], "da1" [144*32]; or "d_sumsq": the last step's 10 per-tensor gradient sums of squares (double, n_rows
- * ignored).  Launches no kernel.  B200_ERR_BAD_ARG for an unknown name or n_rows outside [0, max_batch]. */
+ * ignored).  Launches no kernel.  B200_ERR_BAD_ARG for an unknown name or n_rows outside [0, max_batch], and on a B200_TRAIN_TF32 trainer
+ * for "col1", "col2", "col3", "dcol3" and "dcol2" (not allocated: its convolutions read the activations directly). */
 int b200_trainer_debug_buffer(b200_trainer *t, const char *which, int n_rows, void *out);
 /* Model_VV._loss under no_grad on one chunk (Model.compute_loss, model/model.py:52-83): mean and population std of (weight *) logl; pred_out NULL or [n][2] */
 int b200_trainer_loss(b200_trainer *t, const int8_t *states, const float *value, const float *variance, const float *weight, int n,

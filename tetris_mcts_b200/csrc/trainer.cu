@@ -43,6 +43,21 @@
 //     inference split (valuenet_tc.cuh); tests hold loss, gradient norm and each gradient tensor to 1e-5 of float64 autograd.
 //   - determinism: the chunking depends on the shapes alone and no reduction uses atomics: the tc kind is bit-reproducible run to run and
 //     b200_trainer_train_rows_dev stays bit-identical to b200_trainer_step_rows_dev fed the same indices.
+// B200_TRAIN_TF32 runs the same GEMMs through k_gemm_tf32 with one tf32 term per operand (one wgmma per k8, a third of the tc kind's):
+//   - operands: x -> rna_tf32(x), |x - rna_tf32(x)| <= 2^-11 |x| (2^-137 absolute below fp32's normal range); the product of two
+//     rounded operands (11 x 11 significant bits) is exact in the fp32 accumulator.
+//   - reductions: the tc kind's structure unchanged (one wgmma chain per 32-wide k tile, round-to-nearest FADD into the chunk accumulator,
+//     tc_k_per_split's k ranges, fp64 partials, k_finish), so per element a result is the exact sum of the rounded products within the
+//     tc accumulation bound (32 instead of 96 truncating adds per tile), independent of the batch size.
+//   - against float64: each GEMM output is within 2^-10 of its |term| sum from the two operand roundings, plus the accumulation; summed
+//     to first order over the products on a result's path this holds the loss within 4 * 2^-10 and the gradient norm within 8 * 2^-10;
+//     a gradient element is held to that error carried through the head (GaussianLL's mean - pred can cancel) and the backward pass in
+//     absolute values (tests/test_gpu_trainer_tf32.py).  TF32 with one term is also what torch uses for the reference's conv layers on
+//     Hopper by default (cudnn.allow_tf32).
+//   - implicit im2col: the conv forward GEMMs gather A from the NHWC activations (k = ci*9 + ky*3 + kx), the conv weight gradients gather
+//     col^T the same way, and the input gradients of conv3 / conv2 are one GEMM each writing da2 / da1 directly (k = (ky*3 + kx)*32 + co,
+//     K = 288, taps outside dY are zero terms, ReLU mask in the epilogue): no col1-3 / dcol3 / dcol2 buffers and no k_col2im_relu.
+//   - determinism: as the tc kind.
 #include <cuda_runtime.h>
 #include <cmath>
 #include <cstdio>
@@ -267,6 +282,125 @@ __global__ void __launch_bounds__(128) k_gemm_tc(const float *__restrict__ A, co
                     float v = a;
                     if (bias) v = v + bias[n];
                     if (relu) v = fmaxf(v, 0.f);
+                    Cdirect[o] = v;
+                } else {
+                    Cp[o] = (double)a;
+                }
+            }
+}
+
+// ------------------------------------------------------------------------------------------------ GEMM on tensor cores (one tf32 term, the tf32 kind)
+// k_gemm_tc with one term per operand: each fp32 operand is stored as rna_tf32(x) and each k8 step is one wgmma; the k tiles, the FADD
+// chunk accumulator, the k ranges (tc_k_per_split), the fp64 partials and the epilogue are k_gemm_tc's.  The operands are read through
+// the accessor AOP / BOP names, so a convolution needs no im2col or col2im buffer:
+//   OP_N, OP_T   A stored [M][K] / [K][M], B stored [K][N] / [N][K] (k_gemm's TA / TB)
+//   OP_CONV      A[m][k] = im2col(act)[m][k]: m = (b, y, x) an output pixel of the valid 3x3 conv of act [B][H][W][C] (NHWC),
+//                k = ci*9 + ky*3 + kx (k_im2col's order)
+//   OP_CONV_T    A[m][k] = im2col(act)[k][m] (a conv weight gradient's col^T)
+//   OP_DGRAD     A[m][k] = dY[b][yy - ky][xx - kx][co] for the input pixel m = (b, yy, xx) of a conv whose output gradient dY is
+//                [B][H-2][W-2][32]; k = (ky*3 + kx)*32 + co, so each 32-wide k tile is one tap; 0 where the tap falls outside dY
+//   OP_DGRAD_W   B[k][n] = Wt[co][n][ky][kx] with OP_DGRAD's k (the layer's weight [32][C*9])
+// H, W, C: the conv input's geometry, compile-time so that the index divisions are multiplications.  mask (one k range only): the output
+// is mask[m][n] > 0 ? sum : 0 (the ReLU of the layer below, as k_col2im_relu).
+enum { OP_N = 0, OP_T = 1, OP_CONV = 2, OP_CONV_T = 3, OP_DGRAD = 4, OP_DGRAD_W = 5 };
+
+template <int H, int W, int C>
+__device__ __forceinline__ float im2col_at(const float *__restrict__ act, int pix, int k) {
+    constexpr int OH = H - 2, OW = W - 2;
+    const int b = pix / (OH * OW), r = pix - b * (OH * OW), y = r / OW, x = r - y * OW;
+    const int ci = k / 9, tap = k - ci * 9, ky = tap / 3, kx = tap - ky * 3;
+    return act[(((size_t)b * H + y + ky) * W + x + kx) * C + ci];
+}
+template <int H, int W>
+__device__ __forceinline__ float dgrad_at(const float *__restrict__ dy, int pix, int k) {
+    constexpr int OH = H - 2, OW = W - 2;
+    const int b = pix / (H * W), r = pix - b * (H * W), yy = r / W, xx = r - yy * W;
+    const int tap = k >> 5, ky = tap / 3, y = yy - ky, x = xx - (tap - ky * 3);
+    return (y >= 0 && y < OH && x >= 0 && x < OW) ? dy[(((size_t)b * OH + y) * OW + x) * 32 + (k & 31)] : 0.f;
+}
+
+template <int AOP, int BOP, int BN, int H, int W, int C>
+__global__ void __launch_bounds__(128) k_gemm_tf32(const float *__restrict__ A, const float *__restrict__ B, double *__restrict__ Cpart,
+                                                   int M, int N, int K, int k_per_split, float *__restrict__ Cdirect, const float *__restrict__ bias,
+                                                   int relu, int ct, const float *__restrict__ mask) {
+    static_assert(BN == 32 || BN == 64, "wgmma_tf32 covers N = 32 and 64");
+    constexpr int NA = TG_BM * TG_BK / 128, NB = BN * TG_BK / 128, KC = TG_BK / 4;
+    constexpr bool AM = AOP == OP_T || AOP == OP_CONV_T, BK = BOP == OP_T || BOP == OP_DGRAD_W;    // a warp's loads run along m / along k
+    __shared__ __align__(128) float sA[KC][TG_BM][4];        // [k chunk][row][4 k]
+    __shared__ __align__(128) float sB[KC][BN][4];
+    const int tid = threadIdx.x;
+    const int m0 = blockIdx.y * TG_BM, n0 = blockIdx.x * BN;
+    const int kb = blockIdx.z * k_per_split, ke = min(K, kb + k_per_split);
+    auto a_at = [&](int i, int &mm, int &kk) { const int e = i * 128 + tid; if (AM) { mm = e & 63; kk = e >> 6; } else { kk = e & 31; mm = e >> 5; } };
+    auto b_at = [&](int i, int &nn, int &kk) { const int e = i * 128 + tid; if (BK) { kk = e & 31; nn = e >> 5; } else { nn = e % BN; kk = e / BN; } };
+    auto a_val = [&](int m, int k) -> float {
+        if constexpr (AOP == OP_N) return A[(size_t)m * K + k];
+        else if constexpr (AOP == OP_T) return A[(size_t)k * M + m];
+        else if constexpr (AOP == OP_CONV) return im2col_at<H, W, C>(A, m, k);
+        else if constexpr (AOP == OP_CONV_T) return im2col_at<H, W, C>(A, k, m);
+        else return dgrad_at<H, W>(A, m, k);
+    };
+    auto b_val = [&](int k, int n) -> float {
+        if constexpr (BOP == OP_N) return B[(size_t)k * N + n];
+        else if constexpr (BOP == OP_T) return B[(size_t)n * K + k];
+        else return B[(size_t)(k & 31) * (C * 9) + n * 9 + (k >> 5)];
+    };
+    float ra[NA], rb[NB];
+    auto load = [&](int k0) {
+#pragma unroll
+        for (int i = 0; i < NA; ++i) {
+            int mm, kk; a_at(i, mm, kk);
+            const int k = k0 + kk, m = m0 + mm;
+            ra[i] = (k < ke && m < M) ? a_val(m, k) : 0.f;
+        }
+#pragma unroll
+        for (int i = 0; i < NB; ++i) {
+            int nn, kk; b_at(i, nn, kk);
+            const int k = k0 + kk, n = n0 + nn;
+            rb[i] = (k < ke && n < N) ? b_val(k, n) : 0.f;
+        }
+    };
+    float d[BN / 2], acc[BN / 2];                          // d: this k tile's sum (tensor core), acc: the chunk's sum (FADD, round to nearest)
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) { d[i] = 0.f; acc[i] = 0.f; }
+    const uint32_t sa = b200::smem_u32(&sA[0][0][0]), sb = b200::smem_u32(&sB[0][0][0]);
+    load(kb);
+    for (int k0 = kb; k0 < ke; k0 += TG_BK) {
+        __syncthreads();                                   // the previous tile's wgmmas are complete (every thread waited on them)
+#pragma unroll
+        for (int i = 0; i < NA; ++i) { int mm, kk; a_at(i, mm, kk); sA[kk >> 2][mm][kk & 3] = tf32_rna(ra[i]); }
+#pragma unroll
+        for (int i = 0; i < NB; ++i) { int nn, kk; b_at(i, nn, kk); sB[kk >> 2][nn][kk & 3] = tf32_rna(rb[i]); }
+        b200::fence_async_smem();
+        __syncthreads();
+        b200::wgmma_fence();
+#pragma unroll
+        for (int s = 0; s < TG_BK / 8; ++s)
+            wgmma_tf32(d, b200::gmma_desc(sa + s * 2 * TG_BM * 16, TG_BM * 16, 128), b200::gmma_desc(sb + s * 2 * BN * 16, BN * 16, 128), s ? 1u : 0u);
+        b200::wgmma_commit();
+        if (k0 + TG_BK < ke) load(k0 + TG_BK);            // next tile's global loads overlap this tile's MMAs
+        b200::wgmma_wait<0>();
+        b200::fence_regs(d);
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[i] += d[i];
+    }
+    const int w = tid >> 5, lane = tid & 31, qd = lane & 3, rl = lane >> 2;
+    double *Cp = Cdirect ? nullptr : Cpart + (size_t)blockIdx.z * M * N;
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int m = m0 + 16 * w + 8 * h + rl, n = n0 + 8 * j + 2 * qd + e;
+                if (m >= M || n >= N) continue;
+                const size_t o = ct ? (size_t)n * M + m : (size_t)m * N + n;
+                const float a = acc[4 * j + 2 * h + e];
+                if (Cdirect) {                             // one k range: bias / ReLU / mask here (no partial-sum buffer)
+                    float v = a;
+                    if (bias) v = v + bias[n];
+                    if (relu) v = fmaxf(v, 0.f);
+                    if (mask) v = mask[o] > 0.f ? v : 0.f;
                     Cdirect[o] = v;
                 } else {
                     Cp[o] = (double)a;
@@ -652,6 +786,25 @@ int gemm_tc(b200_trainer *t, const float *A, const float *B, float *C, int M, in
     return 0;
 }
 
+// gemm_tc's launch for k_gemm_tf32 (same k ranges); mask: the ReLU mask of an input gradient, which needs a single k range
+template <int AOP, int BOP, int BN, int H = 0, int W = 0, int C = 0>
+int gemm_tf32(b200_trainer *t, const float *A, const float *B, float *Cm, int M, int N, int K, const float *bias, int relu, int ct = 0,
+              double *out64 = nullptr, const float *mask = nullptr) {
+    const int kps = tc_k_per_split(M, N, K, BN), splits = (K + kps - 1) / kps;
+    dim3 grid((N + BN - 1) / BN, (M + TG_BM - 1) / TG_BM, splits);
+    if (splits == 1) {
+        if (out64) k_gemm_tf32<AOP, BOP, BN, H, W, C><<<grid, 128, 0, t->stream>>>(A, B, out64, M, N, K, kps, nullptr, nullptr, 0, ct, nullptr);
+        else k_gemm_tf32<AOP, BOP, BN, H, W, C><<<grid, 128, 0, t->stream>>>(A, B, nullptr, M, N, K, kps, Cm, bias, relu, ct, mask);
+        return 0;
+    }
+    if (mask) return tfail(B200_ERR_BAD_ARG, "trainer: a masked product needs one k range");
+    if ((size_t)splits * M * N > t->part_elems) return tfail(B200_ERR_BAD_ARG, "trainer: partial-sum buffer too small");
+    k_gemm_tf32<AOP, BOP, BN, H, W, C><<<grid, 128, 0, t->stream>>>(A, B, t->part, M, N, K, kps, nullptr, nullptr, 0, ct, nullptr);
+    if (out64) k_finish<double><<<nblk((size_t)M * N), 256, 0, t->stream>>>(t->part, splits, (size_t)M * N, ct ? M : N, nullptr, 0, out64);
+    else k_finish<float><<<nblk((size_t)M * N), 256, 0, t->stream>>>(t->part, splits, (size_t)M * N, ct ? M : N, bias, relu, Cm);
+    return 0;
+}
+
 // the partial-sum buffer of the tc kind at max_batch: the conv / fc1 weight gradients in TG_KCHUNK chunks, or the small-grid bound above
 size_t tc_part_elems(int max_batch) {
     const size_t B = (size_t)max_batch;
@@ -667,7 +820,23 @@ size_t tc_part_elems(int max_batch) {
 template <bool TA, bool TB, int BN>
 int mm(b200_trainer *t, const float *A, const float *B, float *C, int M, int N, int K, const float *bias, int relu, double *out64 = nullptr) {
     if (t->kind == B200_TRAIN_TC) return gemm_tc<TA, TB, BN>(t, A, B, C, M, N, K, bias, relu, 0, out64);
+    if (t->kind == B200_TRAIN_TF32) return gemm_tf32<TA ? OP_T : OP_N, TB ? OP_T : OP_N, BN>(t, A, B, C, M, N, K, bias, relu, 0, out64);
     return gemm<TA, TB>(t, A, B, C, M, N, K, bias, relu, out64);
+}
+// The tf32 kind's convolution of act [B][H][W][C] -> out [B][H-2][W-2][32] (+ bias, ReLU), its weight gradient dW[32][C*9] (computed as
+// dW^T = col^T dout, stored transposed, like the tc kind's) and, when din, its input gradient din [B][H][W][C] masked by act > 0, each one
+// k_gemm_tf32 reading act / dout directly
+template <int H, int W, int C>
+int conv_fwd_tf32(b200_trainer *t, const float *act, const float *Wt, const float *bias, float *out, int B) {
+    return gemm_tf32<OP_CONV, OP_T, 32, H, W, C>(t, act, Wt, out, B * (H - 2) * (W - 2), 32, C * 9, bias, 1);
+}
+template <int H, int W, int C>
+int conv_back_tf32(b200_trainer *t, const float *act, const float *dout, const float *Wt, float *dW, double *dW64, float *din, int B) {
+    int rc = gemm_tf32<OP_CONV_T, OP_N, 32, H, W, C>(t, act, dout, dW, C * 9, 32, B * (H - 2) * (W - 2), nullptr, 0, 1, dW64);
+    if constexpr (C == 32) {                           // OP_DGRAD's k order takes 32 channels per tap (conv1 needs no input gradient)
+        if (din) rc |= gemm_tf32<OP_DGRAD, OP_DGRAD_W, 32, H, W, C>(t, dout, Wt, din, B * H * W, 32, 9 * 32, nullptr, 0, 0, nullptr, act);
+    }
+    return rc;
 }
 // conv weight gradient dW[32][Kc] = dout^T [32 x P] . col [P x Kc]; the tc kind computes dW^T = col^T dout (32 output columns) and stores
 // it transposed
@@ -684,6 +853,13 @@ void colsum(b200_trainer *t, const float *X, int M, int N, float *out, double *o
 int forward(b200_trainer *t, int B) {
     float *W = t->w;
     int rc = 0;
+    if (t->kind == B200_TRAIN_TF32) {                                                                // implicit im2col
+        rc |= conv_fwd_tf32<20, 10, 1>(t, t->x0, W + O_C1W, W + O_C1B, t->a1, B);
+        rc |= conv_fwd_tf32<18, 8, 32>(t, t->a1, W + O_C2W, W + O_C2B, t->a2, B);
+        rc |= conv_fwd_tf32<16, 6, 32>(t, t->a2, W + O_C3W, W + O_C3B, t->a3, B);
+        k_nhwc_to_flat<<<nblk((size_t)B * 1792), 256, 0, t->stream>>>(t->a3, B, t->flat);
+        return rc | mm<false, true, 64>(t, t->flat, W + O_F1W, t->h, B, 256, 1792, W + O_F1B, 1);
+    }
     k_im2col<<<nblk((size_t)B * 144 * 9), 256, 0, t->stream>>>(t->x0, B, 20, 10, 1, t->col1);
     rc |= mm<false, true, 32>(t, t->col1, W + O_C1W, t->a1, B * 144, 32, 9, W + O_C1B, 1);        // model_vv.py:32-33
     k_im2col<<<nblk((size_t)B * 96 * 288), 256, 0, t->stream>>>(t->a1, B, 18, 8, 32, t->col2);
@@ -733,6 +909,15 @@ int backward(b200_trainer *t, int B, double *g64 = nullptr) {
     colsum(t, t->dh, B, 256, G + O_F1B, G64(O_F1B));
     rc |= mm<false, false, 64>(t, t->dh, W + O_F1W, t->dflat, B, 1792, 256, nullptr, 0);
     k_flat_to_nhwc_relu<<<nblk((size_t)B * 1792), 256, 0, t->stream>>>(t->dflat, t->flat, B, t->dc3);   // ReLU after conv3 (act3)
+    if (t->kind == B200_TRAIN_TF32) {                  // implicit im2col and input gradients (no col / dcol buffers, no col2im)
+        rc |= conv_back_tf32<16, 6, 32>(t, t->a2, t->dc3, W + O_C3W, G + O_C3W, G64(O_C3W), t->da2, B);
+        colsum(t, t->dc3, B * 56, 32, G + O_C3B, G64(O_C3B));
+        rc |= conv_back_tf32<18, 8, 32>(t, t->a1, t->da2, W + O_C2W, G + O_C2W, G64(O_C2W), t->da1, B);
+        colsum(t, t->da2, B * 96, 32, G + O_C2B, G64(O_C2B));
+        rc |= conv_back_tf32<20, 10, 1>(t, t->x0, t->da1, W + O_C1W, G + O_C1W, G64(O_C1W), nullptr, B);
+        colsum(t, t->da1, B * 144, 32, G + O_C1B, G64(O_C1B));
+        return rc;
+    }
     // conv3
     rc |= conv_wgrad(t, t->dc3, t->col3, G + O_C3W, 288, B * 56, G64(O_C3W));
     colsum(t, t->dc3, B * 56, 32, G + O_C3B, G64(O_C3B));
@@ -803,7 +988,8 @@ extern "C" int b200_trainer_create(int device, const float *weights, int max_bat
 
 extern "C" int b200_trainer_create_kind(int device, const float *weights, int max_batch, int kind, b200_trainer **out) {
     if (!weights || !out || max_batch < 1 || max_batch > 65536) return tfail(B200_ERR_BAD_ARG, "trainer: bad argument (1 <= max_batch <= 65536)");
-    if (kind != B200_TRAIN_FP64 && kind != B200_TRAIN_TC) return tfail(B200_ERR_BAD_ARG, "trainer: unknown kind (B200_TRAIN_FP64 or B200_TRAIN_TC)");
+    if (kind != B200_TRAIN_FP64 && kind != B200_TRAIN_TC && kind != B200_TRAIN_TF32)
+        return tfail(B200_ERR_BAD_ARG, "trainer: unknown kind (B200_TRAIN_FP64, B200_TRAIN_TC or B200_TRAIN_TF32)");
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return tfail(B200_ERR_CUDA, "no CUDA device: this library has no CPU path");
     TCK(cudaSetDevice(device));
@@ -817,14 +1003,18 @@ extern "C" int b200_trainer_create_kind(int device, const float *weights, int ma
     rc |= talloc(t, &t->d_toff, N_TENSORS + 1); rc |= talloc(t, &t->d_sumsq, N_TENSORS); rc |= talloc(t, &t->d_lossstat, 2);
     rc |= talloc(t, &t->d_states, B * 200); rc |= talloc(t, &t->d_idx, B);
     rc |= talloc(t, &t->x0, B * 200); rc |= talloc(t, &t->value, B); rc |= talloc(t, &t->variance, B); rc |= talloc(t, &t->weight, B);
-    rc |= talloc(t, &t->col1, B * 144 * 9); rc |= talloc(t, &t->a1, B * 144 * 32); rc |= talloc(t, &t->col2, B * 96 * 288); rc |= talloc(t, &t->a2, B * 96 * 32);
-    rc |= talloc(t, &t->col3, B * 56 * 288); rc |= talloc(t, &t->a3, B * 56 * 32); rc |= talloc(t, &t->flat, B * 1792); rc |= talloc(t, &t->h, B * 256);
+    if (kind != B200_TRAIN_TF32) {                     // the tf32 kind's convolutions read the activations directly (null pointers here)
+        rc |= talloc(t, &t->col1, B * 144 * 9); rc |= talloc(t, &t->col2, B * 96 * 288); rc |= talloc(t, &t->col3, B * 56 * 288);
+        rc |= talloc(t, &t->dcol3, B * 56 * 288); rc |= talloc(t, &t->dcol2, B * 96 * 288);
+    }
+    rc |= talloc(t, &t->a1, B * 144 * 32); rc |= talloc(t, &t->a2, B * 96 * 32);
+    rc |= talloc(t, &t->a3, B * 56 * 32); rc |= talloc(t, &t->flat, B * 1792); rc |= talloc(t, &t->h, B * 256);
     rc |= talloc(t, &t->pred, B * 2); rc |= talloc(t, &t->lossv, B); rc |= talloc(t, &t->dz, B * 2);
-    rc |= talloc(t, &t->dh, B * 256); rc |= talloc(t, &t->dflat, B * 1792); rc |= talloc(t, &t->dc3, B * 56 * 32); rc |= talloc(t, &t->dcol3, B * 56 * 288);
-    rc |= talloc(t, &t->da2, B * 96 * 32); rc |= talloc(t, &t->dcol2, B * 96 * 288); rc |= talloc(t, &t->da1, B * 144 * 32);
+    rc |= talloc(t, &t->dh, B * 256); rc |= talloc(t, &t->dflat, B * 1792); rc |= talloc(t, &t->dc3, B * 56 * 32);
+    rc |= talloc(t, &t->da2, B * 96 * 32); rc |= talloc(t, &t->da1, B * 144 * 32);
     // split-k partial sums (fp64): fp64 kind: only the weight-gradient products are split; the largest is fc1 (256 x 1792) with <= 8 k
-    // ranges.  tc kind: tc_part_elems.
-    t->part_elems = kind == B200_TRAIN_TC ? tc_part_elems(max_batch) : (size_t)8 * 256 * 1792;
+    // ranges.  tc and tf32 kinds: tc_part_elems (the same k ranges).
+    t->part_elems = kind != B200_TRAIN_FP64 ? tc_part_elems(max_batch) : (size_t)8 * 256 * 1792;
     rc |= talloc(t, &t->part, t->part_elems);
     rc |= talloc(t, &t->d_coef, 1); rc |= talloc(t, &t->d_pmax, 2 * STATS_CTAS); rc |= talloc(t, &t->d_psum, STATS_CTAS);
     rc |= talloc(t, &t->d_max2, 2); rc |= talloc(t, &t->d_dsum, 1);
@@ -912,7 +1102,10 @@ extern "C" int b200_trainer_debug_buffer(b200_trainer *t, const char *which, int
     size_t bytes = 0;
     if (!strcmp(which, "d_sumsq")) { src = t->d_sumsq; bytes = N_TENSORS * sizeof(double); }
     for (const auto &b : bufs)
-        if (!strcmp(which, b.name)) { src = b.p; bytes = (size_t)n_rows * b.row * sizeof(float); }
+        if (!strcmp(which, b.name)) {
+            if (!b.p) return tfail(B200_ERR_BAD_ARG, std::string("trainer: a tf32 trainer has no buffer ") + which + " (implicit im2col)");
+            src = b.p; bytes = (size_t)n_rows * b.row * sizeof(float);
+        }
     if (!src) return tfail(B200_ERR_BAD_ARG, std::string("trainer: unknown buffer ") + which);
     TCK(cudaSetDevice(t->device));
     if (bytes) TCK(cudaMemcpyAsync(out, src, bytes, cudaMemcpyDeviceToHost, t->stream));

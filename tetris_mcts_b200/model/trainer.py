@@ -3,7 +3,9 @@ reference's value network — Model_VV._loss (model/model_vv.py:136-153, Gaussia
 (model/yogi.py:39-90) — entirely on the GPU.  No CPU path: without the library / a device the calls raise.
 
 kind: "fp64" runs the contractions on CUDA cores with fp64 accumulation (the reference kind); "tc" runs them on Hopper tensor cores with
-the 3xTF32 split (trainer.cu header, include/b200_tetris_mcts.h B200_TRAIN_TC).  Weights and optimiser state are the same in both kinds."""
+the 3xTF32 split (trainer.cu header, include/b200_tetris_mcts.h B200_TRAIN_TC); "tf32" on tensor cores with one tf32 term per operand and
+implicit-im2col convolutions (B200_TRAIN_TF32: faster, ~1e-3 instead of 1e-5 of float64).  Weights and optimiser state are the same in
+every kind.  A tf32 trainer has no col* / dcol* buffers (NO_BUFFERS); debug_buffer refuses those names."""
 import ctypes as C
 
 import numpy as np
@@ -12,11 +14,12 @@ from .. import _lib as L
 
 N_TRAIN = 478338            # trainable floats (state_dict order without out_ubound / out_lbound)
 GRAD_VEC = N_TRAIN + 3      # doubles of one data-parallel gradient slice: the fp64 gradient, then the slice's loss {count, mean, M2}
-KINDS = {"fp64": 0, "tc": 1}  # B200_TRAIN_FP64, B200_TRAIN_TC
+KINDS = {"fp64": 0, "tc": 1, "tf32": 2}  # B200_TRAIN_FP64, B200_TRAIN_TC, B200_TRAIN_TF32
 # floats per batch row of each buffer b200_trainer_debug_buffer reads (include/b200_tetris_mcts.h)
 DEBUG_ROWS = {"x0": 200, "value": 1, "variance": 1, "weight": 1, "col1": 144 * 9, "a1": 144 * 32, "col2": 96 * 288, "a2": 96 * 32,
               "col3": 56 * 288, "a3": 56 * 32, "flat": 1792, "h": 256, "pred": 2, "lossv": 1, "dz": 2, "dh": 256, "dflat": 1792,
               "dc3": 56 * 32, "dcol3": 56 * 288, "da2": 96 * 32, "dcol2": 96 * 288, "da1": 144 * 32}
+NO_BUFFERS = {"tf32": ("col1", "col2", "col3", "dcol3", "dcol2")}    # the buffers a trainer of that kind does not allocate
 P = C.c_void_p
 _sig_done = False
 

@@ -234,8 +234,9 @@ def parse_args(argv=None):
     p.add_argument('--memory_growth_rate', default=5000, type=int, help='rows the training threshold grows by per training (policy 3)')
     p.add_argument('--train_batch_size', default=1024, type=int, help='training batch size (--online)')
     p.add_argument('--train_max_iters', default=50000, type=int, help='most optimiser steps per training (--online; early stopping usually ends it)')
-    p.add_argument('--train_kind', default='fp64', choices=('fp64', 'tc'),
-                   help='trainer GEMMs (--online): fp64 CUDA cores, or tc = Hopper tensor cores with the 3xTF32 split')
+    p.add_argument('--train_kind', default='fp64', choices=('fp64', 'tc', 'tf32'),
+                   help='trainer GEMMs (--online): fp64 CUDA cores, tc = Hopper tensor cores with the 3xTF32 split, or tf32 = one tf32 '
+                        'term per operand with implicit-im2col convolutions (fastest, ~1e-3 of float64)')
     p.add_argument('--eval_kind', default='net_tc', choices=('net_tc', 'net_fp16'),
                    help='value network of the search (not Vanilla): net_tc = tensor cores within 1e-5 of fp32, net_fp16 = one fp16 product per '
                         'product, about a third of the tensor-core work (DESIGN §5).  --online trains in fp32 / fp64 either way')
