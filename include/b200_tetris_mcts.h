@@ -47,7 +47,7 @@ enum { B200_EVAL_SYNTHETIC = 0, /* test evaluator (hash of the observation), sha
                                    2^-11 relative plus two ill-conditioned cases); the search on those outputs is exact.  Same weight
                                    limits as B200_EVAL_NET_TC.  Not available in B200_MODE_DIST (b200_engine_create returns
                                    B200_ERR_BAD_ARG) nor for b200_load_dist_weights. */
-       B200_EVAL_DIST_FP16 = 4 };/* model/model_distributional.py on the tensor-core kernels of B200_EVAL_NET_TC in B200_MODE_DIST, with ONE
+       B200_EVAL_DIST_FP16 = 4, /* model/model_distributional.py on the tensor-core kernels of B200_EVAL_NET_TC in B200_MODE_DIST, with ONE
                                    fp16 term per operand and one product per product (about 1/3 of the MMA work).  Every conv activation
                                    and conv / fc1 weight is rounded to fp16 (2^-11 relative), so the probabilities are NOT within 1e-5 of
                                    the fp32 network: DESIGN §5 states the bounds (act2 per element within 2^-10 of the board's largest
@@ -55,6 +55,10 @@ enum { B200_EVAL_SYNTHETIC = 0, /* test evaluator (hash of the observation), sha
                                    only in B200_MODE_DIST (b200_engine_create returns B200_ERR_BAD_ARG otherwise: net_fp16 is the value
                                    network's one-term kind); b200_load_weights returns B200_ERR_BAD_ARG (no value network);
                                    b200_load_dist_weights takes the weight limits of B200_EVAL_NET_TC. */
+       B200_EVAL_EXTERNAL = 5 }; /* the caller's evaluator (OnlineMCTSAgent(..., evaluator=, evaluation_type=0), agents/cppmodule/agent.cpp:
+                                   423-436; ValueSimLP.mcts' self.model.inference, agents/ValueSimLP.py:55-60): each simulation step is driven
+                                   with b200_ext_step_begin / b200_ext_step_end below.  B200_MODE_LP, B200_MODE_SINGLE and B200_MODE_DIST
+                                   (b200_engine_create returns B200_ERR_BAD_ARG in B200_MODE_VANILLA, whose evaluator is the rollout). */
 
 typedef struct b200_engine b200_engine;
 
@@ -126,6 +130,32 @@ int b200_set_path_cache(b200_engine *e, int on);
 
 /* --- TreeAgent.mcts (agents/ValueSimLP.py:13, ValueSim.py:52, Vanilla.py:17): `sims` simulations on every game */
 int b200_run_sims(b200_engine *e, int sims);
+
+/* --- the caller's evaluator (B200_EVAL_EXTERNAL): one simulation step of every game in two halves around the caller's network.
+ *   b200_ext_capacity: max_rows = the most rows one step hands out (7 * n_games in B200_MODE_LP, n_games otherwise); out_cols = 2 (v, var),
+ *     or dist_bins in B200_MODE_DIST.
+ *   b200_ext_step_begin: select + expand and the collections of one step (the code b200_run_sims runs), then this step's evaluation
+ *     requests as boards: boards_dev (DEVICE) [max_rows][200] = NCHW [n,1,20,10] in {-1, 0, 1} as Model_VV.inference sees them (the
+ *     board bits, the four falling-piece cells -1), int8 (B200_BOARD_INT8) or float32 (B200_BOARD_F32); ids_dev (DEVICE, may be NULL)
+ *     [max_rows] = game * 8 + slot of each row (slot = child index in LP, 7 = the leaf itself).  Rows are in ascending (game, slot) order,
+ *     so the batch is a function of the search state alone, not of the order the device queued the requests in.  Synchronises the
+ *     engine's stream and returns *n_rows (0 is possible, e.g. when every leaf is a game over).  In LP the rows are the unique children
+ *     whose observation has no statistics yet; the reference also evaluates the others and discards those outputs (core.h:303-381), so
+ *     the results are the same.
+ *   b200_ext_step_end: out_dev (DEVICE) [n_rows][out_cols] fp32 row-major (stored as they are, NaN included), then the backup.
+ *     Asynchronous on the engine's stream, like b200_run_sims: order the evaluator's work against b200_engine_get_stream.
+ *   Between the two a step is open: a second step_begin, and b200_run_sims, b200_play_move, b200_update_root, b200_set_games,
+ *   b200_env_step, b200_remove_nodes, b200_set_path_cache, b200_engine_set_stream and the b200_replay_* calls return B200_ERR_BAD_ARG;
+ *   step_end without an open step too.  Reading calls (b200_export_game, b200_export_dist, b200_get_stats, b200_counters, b200_status)
+ *   work as usual.  An external engine returns B200_ERR_BAD_ARG from b200_run_sims, b200_play_move, b200_load_weights,
+ *   b200_load_dist_weights, b200_valuenet_forward, b200_distnet_forward and the b200_debug_* network readers; b200_set_deep_lane is
+ *   ignored; counter 12 is the longest trace since the engine was created (only b200_run_sims resets it).  The kernels of the split
+ *   count under phase 6 of b200_phase_ms. */
+#define B200_BOARD_INT8 0
+#define B200_BOARD_F32 1
+int b200_ext_capacity(b200_engine *e, int32_t *max_rows, int32_t *out_cols);
+int b200_ext_step_begin(b200_engine *e, void *boards_dev, int board_dtype, int32_t *ids_dev, int32_t *n_rows);
+int b200_ext_step_end(b200_engine *e, const float *out_dev);
 
 /* --- TreeAgent.compute_stats / get_action (agents/agent.py:153-185): stats[n][3][7], action[n] */
 int b200_get_stats(b200_engine *e, float *stats, int32_t *action);

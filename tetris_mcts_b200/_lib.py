@@ -14,7 +14,8 @@ N_ACTIONS = 7
 N_WEIGHTS = 478342
 
 MODE_LP, MODE_SINGLE, MODE_VANILLA, MODE_DIST = 0, 1, 2, 3
-EVAL_SYNTHETIC, EVAL_NET, EVAL_NET_TC, EVAL_NET_FP16, EVAL_DIST_FP16 = 0, 1, 2, 3, 4
+EVAL_SYNTHETIC, EVAL_NET, EVAL_NET_TC, EVAL_NET_FP16, EVAL_DIST_FP16, EVAL_EXTERNAL = 0, 1, 2, 3, 4, 5
+BOARD_INT8, BOARD_F32 = 0, 1
 ERR_NAMES = {1: "BAD_ARG", 2: "CUDA", 3: "ARENA_FULL", 4: "TRACE_FULL", 5: "NO_WEIGHTS"}
 
 
@@ -100,6 +101,9 @@ def lib():
         L.b200_dist_mean_variance.argtypes = [P, C.c_int, C.c_double, C.c_double, P, P]
         L.b200_dist_select_trace.argtypes = [C.c_int, P, P, C.c_int, C.c_int, P, P, C.c_int, P]
         L.b200_dist_backup_trace.argtypes = [P, C.c_int, P, P, C.c_int, C.c_int, C.c_double, P, C.c_double, C.c_double]
+        L.b200_ext_capacity.argtypes = [P, P, P]
+        L.b200_ext_step_begin.argtypes = [P, P, C.c_int, P, P]
+        L.b200_ext_step_end.argtypes = [P, P]
         _lib = L
     return _lib
 

@@ -5,6 +5,7 @@ the search loop it sketches (:36-75) is driven here on the reference's distribut
 getattr(module, 'DistValueSimOnline') (play.py:82), so the class is exported under both names."""
 import numpy as np
 
+from .. import _lib as L
 from .agent import TreeAgent
 
 
@@ -28,7 +29,7 @@ class DistValueSim(TreeAgent):
         kwargs.pop("min_visit", None)
         self.atoms, self.vrange = atoms, (vmin, vmax)
         super().__init__(max_nodes=100000, low=5, eval_kind=kwargs.pop("eval_kind", "net"), **kwargs)
-        if self._eng.eval_kind != 0:
+        if self._eng.eval_kind not in (L.EVAL_SYNTHETIC, L.EVAL_EXTERNAL):
             self._eng.load_dist_weights(init_dist_weights(0, atoms) if dist_weights is None else dist_weights, atoms)
 
     def _engine_kwargs(self):

@@ -15,7 +15,9 @@ class ValueSim(TreeAgent):
     def __init__(self, online=True, memory_size=500000, min_visits_to_store=10, gamma=0.999, memory_growth_rate=5000, weights=None,
                  train_kind="fp64", **kwargs):
         kwargs.pop("max_nodes", None)
-        if weights is None:
+        if kwargs.get("evaluator") is not None and online and not kwargs.get("benchmark", False):
+            raise ValueError("online=True trains the engine's Model_VV weights on the device, not the caller's evaluator: pass online=False")
+        if weights is None and kwargs.get("evaluator") is None:
             # ValueSim.py:42-44: self.model = Model(); self.model.load(); self.model.training(False).  Model.load (model/model.py:163-174)
             # reads ./pytorch_model/model_checkpoint when it exists and otherwise keeps the default-initialised network.
             weights = load_checkpoint_weights()

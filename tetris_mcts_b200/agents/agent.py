@@ -55,7 +55,12 @@ class TreeAgent(Agent):                                          # agents/agent.
     _mode = "lp"
 
     def __init__(self, sims=100, max_nodes=500000, env=None, env_args=None, node_saver=None, projection=True, min_visits=30,
-                 gamma=0.999, low=1, eval_kind="net_tc", weights=None, device=0, overflow_reset=False, **kwargs):
+                 gamma=0.999, low=1, eval_kind="net_tc", weights=None, device=0, overflow_reset=False, evaluator=None,
+                 evaluator_on_device=False, **kwargs):
+        """evaluator: the reference's evaluator callback (OnlineMCTSAgent(..., evaluator=, evaluation_type=0), agents/ValueSimC.py;
+        ValueSimLP's self.model.inference): the engine then runs eval_kind "external" and mcts() hands every simulation step's boards to
+        it.  evaluator_on_device=False: int8 ndarray [n,1,20,10] in, [v (n,1), var (n,1)] or [probs (n, atoms)] out (Model_VV.inference
+        as it is); True: a torch tensor on the engine's device in, torch float32 out (BatchedEngine.run_sims)."""
         super().__init__(**kwargs)
         if not projection:
             raise NotImplementedError("only projection=True is live in the reference (SURVEY N4)")
@@ -63,6 +68,9 @@ class TreeAgent(Agent):                                          # agents/agent.
         self.env, self.env_args = env, env_args if env_args is not None else ((20, 10), 1, 0, 0)
         self.episode, self.min_visits, self.node_saver, self.projection = 0, min_visits, node_saver, projection
         self.gamma = gamma
+        self._evaluator, self._evaluator_on_device = evaluator, bool(evaluator_on_device)
+        if evaluator is not None:
+            eval_kind, weights = "external", None
         self.stats = np.zeros((3, self.n_actions), np.float32)
         self._eng = BatchedEngine(1, max_nodes=self.max_nodes, mode=self._mode, gamma=gamma, low=low, eval_kind=eval_kind, weights=weights,
                                   env_args=self.env_args, device=device, overflow_reset=overflow_reset, **self._engine_kwargs())
@@ -108,7 +116,7 @@ class TreeAgent(Agent):                                          # agents/agent.
 
     def mcts(self, root_index=None, sims=None):                   # agents/agent.py:132 (overridden per agent type)
         self._snap = None
-        self._eng.run_sims(self.sims if sims is None else sims)
+        self._eng.run_sims(self.sims if sims is None else sims, evaluator=self._evaluator, host=not self._evaluator_on_device)
 
     def play(self):                                               # agents/agent.py:147-151
         self.mcts(None, self.sims)

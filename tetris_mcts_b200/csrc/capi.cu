@@ -18,6 +18,7 @@
 #include "replay_policy.cuh"
 #include "valuenet_tc.cuh"
 #include "distnet_tc.cuh"
+#include "ext_eval.cuh"
 
 using namespace b200;
 
@@ -74,7 +75,23 @@ struct b200_engine {
     int gc_pool_main = 0;          // collection scratch sets of the main k_gc launch; DEEP_GC_BLOCKS more follow for the deep lane's
     cudaGraphExec_t step_exec = nullptr; bool step_graph_failed = false;
     uint64_t step_launches[PH_N] = {0};
+    // caller-supplied evaluator (B200_EVAL_EXTERNAL): k_ext_order's marks and ordered rows; ext_open between b200_ext_step_begin and _end
+    int32_t *d_ext_mark = nullptr, *d_ext_n = nullptr; uint2 *d_ext_rows = nullptr;
+    bool ext_open = false; int32_t ext_rows = 0;
 };
+
+static bool ext_kind(const b200_engine *e) { return e->cfg.eval_kind == B200_EVAL_EXTERNAL; }
+// the calls an external engine has no use for (it has no network of its own, and its steps need the caller's outputs)
+static int ext_refuse(const b200_engine *e, const char *fn) {
+    return fail(B200_ERR_BAD_ARG, std::string(fn) + ": eval_kind external has no built-in network; drive the search with "
+                                  "b200_ext_step_begin / b200_ext_step_end");
+}
+// the calls that change the trees, the games or the engine's stream, while a step is open between b200_ext_step_begin and _end
+static int step_open(const b200_engine *e, const char *fn) {
+    return fail(B200_ERR_BAD_ARG, std::string(fn) + ": a simulation step is open; finish it with b200_ext_step_end first");
+}
+#define REFUSE_IF_EXT(e, fn) do { if (ext_kind(e)) return ext_refuse(e, fn); } while (0)
+#define REFUSE_IF_OPEN(e, fn) do { if ((e)->ext_open) return step_open(e, fn); } while (0)
 
 // kernel arguments of the captured step changed (weights, replay memory, ...): capture again at the next run_sims
 static void drop_step_graph(b200_engine *e) {
@@ -182,6 +199,8 @@ extern "C" int b200_engine_create(const b200_config *cfg, b200_engine **out) {
         return fail(B200_ERR_BAD_ARG, "distributional mode needs 2 <= dist_bins <= 64 and dist_vmax > dist_vmin");
     if (cfg->mode == MODE_DIST && cfg->eval_kind == B200_EVAL_NET_FP16)
         return fail(B200_ERR_BAD_ARG, "eval_kind net_fp16 has no distributional network: use net_tc or net in B200_MODE_DIST");
+    if (cfg->mode == MODE_VANILLA && cfg->eval_kind == B200_EVAL_EXTERNAL)
+        return fail(B200_ERR_BAD_ARG, "eval_kind external needs B200_MODE_LP, B200_MODE_SINGLE or B200_MODE_DIST (Vanilla evaluates by rollout)");
     if (cfg->mode != MODE_DIST && cfg->eval_kind == B200_EVAL_DIST_FP16)
         return fail(B200_ERR_BAD_ARG, "eval_kind dist_fp16 is the distributional network's one-term form and needs B200_MODE_DIST: "
                                       "use net_fp16 for the value network");
@@ -232,6 +251,9 @@ extern "C" int b200_engine_create(const b200_config *cfg, b200_engine **out) {
         A.dist_bins = cfg->dist_bins; A.dist_vmin = cfg->dist_vmin; A.dist_vmax = cfg->dist_vmax;
         rc |= dalloc(e, &A.nstat, GM * NSTAT_WORDS); rc |= dalloc(e, &A.ndist, GM * (size_t)A.dist_bins); rc |= dalloc(e, &A.dist_eval, G * (size_t)A.dist_bins);
     }
+    if (cfg->eval_kind == B200_EVAL_EXTERNAL) {
+        rc |= dalloc(e, &e->d_ext_mark, G * 8); rc |= dalloc(e, &e->d_ext_rows, G * 8); rc |= dalloc(e, &e->d_ext_n, 1);
+    }
     rc |= dalloc(e, &e->d_default_rec, REC_WORDS);
     rc |= dalloc(e, &e->d_stats, G * 21); rc |= dalloc(e, &e->d_action, G);
     e->d_game_stats = A.counters + 8;
@@ -279,6 +301,7 @@ extern "C" int b200_engine_destroy(b200_engine *e) {
 // simulation step is dropped and re-captured on the new stream.  The caller keeps ownership of its stream and must keep it alive.
 extern "C" int b200_engine_set_stream(b200_engine *e, void *cuda_stream) {
     if (!e) return fail(B200_ERR_BAD_ARG, "null engine");
+    REFUSE_IF_OPEN(e, "b200_engine_set_stream");
     CK(cudaSetDevice(e->cfg.device));
     CK(cudaStreamSynchronize(e->stream));
     if (e->stream1) CK(cudaStreamSynchronize(e->stream1));
@@ -306,6 +329,7 @@ static decltype(&k_tc_fc_dbg<2>) tc_fc_dbg_kernel(const b200_engine *e) { return
 
 extern "C" int b200_load_weights(b200_engine *e, const float *w) {
     if (!e || !w) return fail(B200_ERR_BAD_ARG, "null argument");
+    REFUSE_IF_EXT(e, "b200_load_weights");
     if (e->cfg.eval_kind == B200_EVAL_DIST_FP16) return fail(B200_ERR_BAD_ARG, "eval_kind dist_fp16 has no value network (use net_fp16)");
     if (tc_net(e) && !tc_weights_fit(w))
         return fail(B200_ERR_BAD_ARG, e->cfg.eval_kind == B200_EVAL_NET_TC
@@ -428,6 +452,7 @@ static bool dn_tc_net(const b200_engine *e) { return e->cfg.eval_kind == B200_EV
 
 extern "C" int b200_load_dist_weights(b200_engine *e, const float *w, int atoms) {
     if (!e || !w || atoms < 2 || atoms > 64) return fail(B200_ERR_BAD_ARG, "bad argument");
+    REFUSE_IF_EXT(e, "b200_load_dist_weights");
     if (e->cfg.eval_kind == B200_EVAL_NET_FP16) return fail(B200_ERR_BAD_ARG, "eval_kind net_fp16 has no distributional network");
     CK(cudaSetDevice(e->cfg.device));
     if (e->A.mode == MODE_DIST && atoms != e->A.dist_bins) return fail(B200_ERR_BAD_ARG, "atoms must equal dist_bins");
@@ -534,6 +559,7 @@ static int distnet_forward(b200_engine *e, const int8_t *states, int k, int atom
     return rc;
 }
 extern "C" int b200_distnet_forward(b200_engine *e, const int8_t *states, int k, int atoms, float *dist) {
+    if (e) REFUSE_IF_EXT(e, "b200_distnet_forward");
     return distnet_forward(e, states, k, atoms, dist, nullptr, nullptr);
 }
 
@@ -556,6 +582,7 @@ static int check_status(b200_engine *e) {   // cheap: max over the status array 
 // TreeAgent.remove_nodes() (agents/agent.py:246-257) for every game with fewer than min_free free node slots, as ONE batched k_gc
 extern "C" int b200_remove_nodes(b200_engine *e, int min_free) {
     if (!e || min_free < 0) return fail(B200_ERR_BAD_ARG, "bad argument");
+    REFUSE_IF_OPEN(e, "b200_remove_nodes");
     CK(cudaSetDevice(e->cfg.device));
     {
         PhaseTimer t(e, PH_GC);
@@ -576,6 +603,7 @@ extern "C" int b200_set_gc_headroom(b200_engine *e, int min_free) {
 // Path cache (search_dev.cuh "path cache"): scheduling/memory-traffic only, no effect on any result.  LP mode, max_nodes <= 65536.
 extern "C" int b200_set_path_cache(b200_engine *e, int on) {
     if (!e) return fail(B200_ERR_BAD_ARG, "null engine");
+    REFUSE_IF_OPEN(e, "b200_set_path_cache");
     CK(cudaSetDevice(e->cfg.device));
     if (on) {
         if (e->A.mode != MODE_LP) return fail(B200_ERR_BAD_ARG, "the path cache serves B200_MODE_LP (its coherence rules rest on the LP backup)");
@@ -639,10 +667,14 @@ static int update_root_impl(b200_engine *e, int auto_reset, bool headroom_collec
     return B200_OK;
 }
 
-extern "C" int b200_update_root(b200_engine *e, int auto_reset) { return update_root_impl(e, auto_reset, true); }
+extern "C" int b200_update_root(b200_engine *e, int auto_reset) {
+    if (e) REFUSE_IF_OPEN(e, "b200_update_root");
+    return update_root_impl(e, auto_reset, true);
+}
 
 extern "C" int b200_set_games(b200_engine *e, const uint32_t *recs) {
     if (!e || !recs) return fail(B200_ERR_BAD_ARG, "null argument");
+    REFUSE_IF_OPEN(e, "b200_set_games");
     CK(cudaSetDevice(e->cfg.device));
     CK(cudaMemcpyAsync(e->A.cur, recs, (size_t)e->A.G * REC_WORDS * 4, cudaMemcpyHostToDevice, e->stream));
     int rc = update_root_impl(e, 0, false);   // handing the games over is not a move: the driver's between-moves collection (b200_set_gc_headroom) is not due here
@@ -721,11 +753,11 @@ static int enqueue_step_lanes(b200_engine *e) {
     return B200_OK;
 }
 
-// One simulation step of every game: select+expand -> (collect garbage, resume) -> evaluate -> backup.
-static int enqueue_step(b200_engine *e) {
+// The first half of a simulation step (one lane): select+expand, then the collections the step needs and the expansions they held up.
+// Leaves the step's evaluation requests in A.req[0 .. *A.n_req).
+static int step_select(b200_engine *e) {
     const Arena &A = e->A;
     const int G = A.G;
-    if (deep_lane_on(e)) return enqueue_step_lanes(e);
     CK(cudaMemsetAsync(A.n_req, 0, 2 * sizeof(int32_t), e->stream));
     {
         PhaseTimer t(e, PH_SELECT);
@@ -738,6 +770,24 @@ static int enqueue_step(b200_engine *e) {
         k_gc<<<gc_blocks(e), GC_THREADS, 0, e->stream>>>(A);
         k_expand_resume<<<blocks_groups(G), TPB, 0, e->stream>>>(A);
     }
+    return B200_OK;
+}
+
+// The second half: back every game's evaluated leaf up its trace (the evaluator's outputs are in A.eval_out / A.dist_eval / A.rollout_val).
+static void step_backup(b200_engine *e) {
+    const Arena &A = e->A;
+    PhaseTimer t(e, PH_BACKUP);
+    if (A.mode == MODE_DIST) k_dist_backup<<<(A.G + 3) / 4, 128, 0, e->stream>>>(A);
+    else k_backup<<<(A.G + 3) / 4, 128, backup_smem(A), e->stream>>>(A, backup_bitmap_words(A));
+}
+
+// One simulation step of every game: select+expand -> (collect garbage, resume) -> evaluate -> backup.
+static int enqueue_step(b200_engine *e) {
+    const Arena &A = e->A;
+    const int G = A.G;
+    if (deep_lane_on(e)) return enqueue_step_lanes(e);
+    int rc = step_select(e);
+    if (rc) return rc;
     if (A.mode == MODE_VANILLA) {
         PhaseTimer t(e, PH_ROLLOUT);
         k_rollout<<<(G + 63) / 64, 64, 0, e->stream>>>(A);
@@ -746,21 +796,17 @@ static int enqueue_step(b200_engine *e) {
             PhaseTimer t(e, PH_SYNTH);
             k_eval_synthetic_dist<<<(G + 127) / 128, 128, 0, e->stream>>>(A);
         } else {
-            int rc = launch_distnet(e);
+            rc = launch_distnet(e);
             if (rc) return rc;
         }
     } else if (e->cfg.eval_kind == B200_EVAL_SYNTHETIC) {
         PhaseTimer t(e, PH_SYNTH);
         k_eval_synthetic<<<(G * 7 + 255) / 256 < 1184 ? (G * 7 + 255) / 256 : 1184, 256, 0, e->stream>>>(A);
     } else {
-        int rc = launch_net(e, A.req, A.n_req, A.key, A.M, A.eval_out, (size_t)G * (A.mode == MODE_LP ? 7 : 1));
+        rc = launch_net(e, A.req, A.n_req, A.key, A.M, A.eval_out, (size_t)G * (A.mode == MODE_LP ? 7 : 1));
         if (rc) return rc;
     }
-    {
-        PhaseTimer t(e, PH_BACKUP);
-        if (A.mode == MODE_DIST) k_dist_backup<<<(G + 3) / 4, 128, 0, e->stream>>>(A);
-        else k_backup<<<(G + 3) / 4, 128, backup_smem(A), e->stream>>>(A, backup_bitmap_words(A));
-    }
+    step_backup(e);
     return B200_OK;
 }
 
@@ -785,6 +831,7 @@ static void capture_step(b200_engine *e) {
 
 extern "C" int b200_run_sims(b200_engine *e, int sims) {
     if (!e || sims < 0) return fail(B200_ERR_BAD_ARG, "bad argument");
+    REFUSE_IF_EXT(e, "b200_run_sims");
     CK(cudaSetDevice(e->cfg.device));
     const Arena &A = e->A;
     const bool need_net = A.mode != MODE_VANILLA && e->cfg.eval_kind != B200_EVAL_SYNTHETIC;
@@ -806,6 +853,61 @@ extern "C" int b200_run_sims(b200_engine *e, int sims) {
     return B200_OK;
 }
 
+// ---------------------------------------------------------------------------------------------------- caller-supplied evaluator
+extern "C" int b200_ext_capacity(b200_engine *e, int32_t *max_rows, int32_t *out_cols) {
+    if (!e || !max_rows || !out_cols) return fail(B200_ERR_BAD_ARG, "null argument");
+    if (!ext_kind(e)) return fail(B200_ERR_BAD_ARG, "b200_ext_capacity: the engine's eval_kind is not external");
+    *max_rows = e->A.G * (e->A.mode == MODE_LP ? 7 : 1);
+    *out_cols = e->A.mode == MODE_DIST ? e->A.dist_bins : 2;
+    return B200_OK;
+}
+
+// The first half of one simulation step (the same code as b200_run_sims'), then this step's requests in (game, slot) order as boards.
+extern "C" int b200_ext_step_begin(b200_engine *e, void *boards_dev, int board_dtype, int32_t *ids_dev, int32_t *n_rows) {
+    if (!e || !boards_dev || !n_rows || (board_dtype != B200_BOARD_INT8 && board_dtype != B200_BOARD_F32))
+        return fail(B200_ERR_BAD_ARG, "bad argument (boards_dev and n_rows non-NULL, board_dtype B200_BOARD_INT8 or B200_BOARD_F32)");
+    if (!ext_kind(e)) return fail(B200_ERR_BAD_ARG, "b200_ext_step_begin: the engine's eval_kind is not external (use b200_run_sims)");
+    if (e->ext_open) return fail(B200_ERR_BAD_ARG, "b200_ext_step_begin: a step is already open; finish it with b200_ext_step_end");
+    CK(cudaSetDevice(e->cfg.device));
+    const Arena &A = e->A;
+    int rc = step_select(e);
+    if (rc) return rc;
+    {
+        PhaseTimer t(e, PH_MISC);
+        const int grid = e->n_sm * 4;
+        k_ext_order<<<1, EXT_ORDER_THREADS, 0, e->stream>>>(A, e->d_ext_mark, e->d_ext_rows, e->d_ext_n);
+        if (board_dtype == B200_BOARD_INT8) k_ext_boards<int8_t><<<grid, 256, 0, e->stream>>>(A, e->d_ext_rows, e->d_ext_n, (int8_t *)boards_dev, ids_dev);
+        else k_ext_boards<float><<<grid, 256, 0, e->stream>>>(A, e->d_ext_rows, e->d_ext_n, (float *)boards_dev, ids_dev);
+    }
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(&e->ext_rows, e->d_ext_n, sizeof(int32_t), cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaStreamSynchronize(e->stream));
+    e->ext_open = true;
+    *n_rows = e->ext_rows;
+    return B200_OK;
+}
+
+// The caller's outputs into the evaluator slots, then the backup: the second half of the step b200_ext_step_begin opened.  Asynchronous.
+extern "C" int b200_ext_step_end(b200_engine *e, const float *out_dev) {
+    if (!e) return fail(B200_ERR_BAD_ARG, "null engine");
+    if (!ext_kind(e)) return fail(B200_ERR_BAD_ARG, "b200_ext_step_end: the engine's eval_kind is not external");
+    if (!e->ext_open) return fail(B200_ERR_BAD_ARG, "b200_ext_step_end: no step is open (call b200_ext_step_begin first)");
+    if (!out_dev && e->ext_rows > 0) return fail(B200_ERR_BAD_ARG, "b200_ext_step_end: out_dev is NULL");
+    CK(cudaSetDevice(e->cfg.device));
+    const Arena &A = e->A;
+    if (e->ext_rows > 0) {
+        PhaseTimer t(e, PH_MISC);
+        const int cols = A.mode == MODE_DIST ? A.dist_bins : 2;
+        const long long work = (long long)e->ext_rows * cols;
+        const int grid = (int)std::min<long long>((work + 255) / 256, (long long)e->n_sm * 4);
+        k_ext_scatter<<<grid, 256, 0, e->stream>>>(A, e->d_ext_rows, e->d_ext_n, out_dev, cols);
+    }
+    step_backup(e);
+    CK(cudaGetLastError());
+    e->ext_open = false;
+    return B200_OK;
+}
+
 extern "C" int b200_get_stats(b200_engine *e, float *stats, int32_t *action) {
     if (!e) return fail(B200_ERR_BAD_ARG, "null engine");
     CK(cudaSetDevice(e->cfg.device));
@@ -821,6 +923,7 @@ extern "C" int b200_get_stats(b200_engine *e, float *stats, int32_t *action) {
 
 extern "C" int b200_env_step(b200_engine *e, const int32_t *actions) {
     if (!e) return fail(B200_ERR_BAD_ARG, "null engine");
+    REFUSE_IF_OPEN(e, "b200_env_step");
     CK(cudaSetDevice(e->cfg.device));
     if (actions) CK(cudaMemcpyAsync(e->d_action, actions, (size_t)e->A.G * 4, cudaMemcpyHostToDevice, e->stream));
     {
@@ -832,6 +935,7 @@ extern "C" int b200_env_step(b200_engine *e, const int32_t *actions) {
 }
 
 extern "C" int b200_play_move(b200_engine *e, int sims, int auto_reset, int32_t *actions_out, float *stats_out) {
+    if (e) REFUSE_IF_EXT(e, "b200_play_move");
     int rc = b200_run_sims(e, sims);
     if (rc) return rc;
     rc = b200_get_stats(e, stats_out, actions_out);
@@ -1029,11 +1133,13 @@ static int valuenet_forward(b200_engine *e, const int8_t *states, int k, float *
     return rc;
 }
 extern "C" int b200_valuenet_forward(b200_engine *e, const int8_t *states, int k, float *v, float *var) {
+    if (e) REFUSE_IF_EXT(e, "b200_valuenet_forward");
     return valuenet_forward(e, states, k, v, var, nullptr, nullptr);
 }
 
 // development / test aid: the conv stack's output (flatten input of fc1) in torch order c*56 + y*4 + x, for either path
 extern "C" int b200_debug_act3(b200_engine *e, const int8_t *states, int k, float *out) {
+    if (e) REFUSE_IF_EXT(e, "b200_debug_act3");
     if (!e || !states || !out || k < 1) return fail(B200_ERR_BAD_ARG, "bad argument");
     std::vector<float> v(k), var(k);
     int rc = b200_valuenet_forward(e, states, k, v.data(), var.data());   // leaves act3 of these k boards in the scratch buffers
@@ -1069,6 +1175,7 @@ extern "C" int b200_debug_act3(b200_engine *e, const int8_t *states, int k, floa
 // development / test aid: the distributional conv stack's output (flatten input of fc1) in torch order c*64 + y*4 + x, read back from the
 // tensor-core kernels' act2 (net_tc: both fp16 terms, dist_fp16: the one it writes)
 extern "C" int b200_debug_dist_act2(b200_engine *e, const int8_t *states, int k, float *out) {
+    if (e) REFUSE_IF_EXT(e, "b200_debug_dist_act2");
     if (!e || !states || !out || k < 1) return fail(B200_ERR_BAD_ARG, "bad argument");
     if (!dn_tc_net(e)) return fail(B200_ERR_BAD_ARG, "b200_debug_dist_act2 reads the tensor-core distributional network: eval_kind net_tc or dist_fp16");
     if (!e->have_dist_weights) return fail(B200_ERR_NO_WEIGHTS, "b200_load_dist_weights was not called");
@@ -1098,6 +1205,7 @@ extern "C" int b200_debug_dist_act2(b200_engine *e, const int8_t *states, int k,
 // forward pass that runs the DBG instantiations of the conv kernel (which also copies the shared-memory activations out) and of the fc
 // kernel (which also writes the accumulator out)
 extern "C" int b200_debug_tc_acts(b200_engine *e, int dist, const int8_t *states, int k, int layer, float *out) {
+    if (e) REFUSE_IF_EXT(e, "b200_debug_tc_acts");
     if (!e || !states || !out || k < 1) return fail(B200_ERR_BAD_ARG, "bad argument");
     if (dist ? !dn_tc_net(e) : !tc_net(e))
         return fail(B200_ERR_BAD_ARG, "b200_debug_tc_acts reads the tensor-core networks: eval_kind net_tc, net_fp16 (value) or dist_fp16 (distributional)");
@@ -1169,6 +1277,7 @@ extern "C" int b200_debug_tc_acts(b200_engine *e, int dist, const int8_t *states
 // development / test aid: every stage of the fp32 CUDA-core networks (eval_kind net) exactly as the kernels computed it, from one forward
 // pass that runs the DBG instantiations k_vn_conv_dbg / k_vn_fc_dbg or k_dn_conv_dbg / k_dn_fc_dbg
 extern "C" int b200_debug_net_acts(b200_engine *e, int dist, const int8_t *states, int k, int layer, float *out) {
+    if (e) REFUSE_IF_EXT(e, "b200_debug_net_acts");
     if (!e || !states || !out || k < 1) return fail(B200_ERR_BAD_ARG, "bad argument");
     if (e->cfg.eval_kind != B200_EVAL_NET) return fail(B200_ERR_BAD_ARG, "b200_debug_net_acts reads the fp32 CUDA-core networks: eval_kind net");
     if (dist != 0 && dist != 1) return fail(B200_ERR_BAD_ARG, "dist must be 0 (value network) or 1 (distributional network)");
@@ -1476,6 +1585,7 @@ __global__ void k_collect_samples(Arena A, int min_visits, uint8_t *out, int cap
 
 // Online replay memory (agents/ValueSim.py:14-37, agent.cpp:588-617): allocate `capacity` rows; k_gc appends to it.
 extern "C" int b200_replay_enable(b200_engine *e, int min_visits, int capacity) {
+    if (e) REFUSE_IF_OPEN(e, "b200_replay_enable");
     if (!e || capacity < 1 || min_visits < 0) return fail(B200_ERR_BAD_ARG, "bad argument");
     CK(cudaSetDevice(e->cfg.device));
     if (e->A.replay) return fail(B200_ERR_BAD_ARG, "replay memory already enabled");
@@ -1493,6 +1603,7 @@ extern "C" int b200_replay_enable(b200_engine *e, int min_visits, int capacity) 
 // Hand the stored rows to the trainer / the all-gather: copies min(count, capacity) rows to out_dev (DEVICE) and empties the memory
 // (memory_index = 0 after training, ValueSim.py:183 / agent.cpp:700).
 extern "C" int b200_replay_drain_dev(b200_engine *e, void *out_dev, int capacity, int32_t *count_out) {
+    if (e) REFUSE_IF_OPEN(e, "b200_replay_drain_dev");
     if (!e || !out_dev || !count_out || !e->A.replay) return fail(B200_ERR_BAD_ARG, "replay memory not enabled / bad argument");
     CK(cudaSetDevice(e->cfg.device));
     int32_t n = 0;
@@ -1555,6 +1666,7 @@ static int rp_compact(b200_engine *e, const std::vector<uint8_t> &keep, int lo, 
 
 // OnlineMCTSAgent(accumulation_policy, episodes_per_train, memory_growth_rate) agent.cpp:588-617; memory_size / min_visit = b200_replay_enable's
 extern "C" int b200_replay_policy(b200_engine *e, int policy, int episodes_per_train, int memory_growth_rate) {
+    if (e) REFUSE_IF_OPEN(e, "b200_replay_policy");
     if (!e || !e->A.replay || policy < 0 || policy > 3 || episodes_per_train < 1 || memory_growth_rate < 0) return fail(B200_ERR_BAD_ARG, "replay memory not enabled / bad policy");
     CK(cudaSetDevice(e->cfg.device));
     ReplayPolicy fresh;
@@ -1610,6 +1722,7 @@ static int rp_random_trimming(b200_engine *e, double fraction) {
 // (agent.cpp:69,279-280: games finished so far).  *train_now = the reference would call train(m_state, m_value, m_variance, m_visit, memory_index)
 // now: drain the first *memory_index rows (b200_replay_peek_dev), train, then b200_replay_policy_trained().
 extern "C" int b200_replay_policy_step(b200_engine *e, int64_t current_episode, int32_t *train_now, int32_t *memory_index) {
+    if (e) REFUSE_IF_OPEN(e, "b200_replay_policy_step");
     if (!e || !train_now || !memory_index || e->rp.policy < 0) return fail(B200_ERR_BAD_ARG, "no replay policy configured");
     CK(cudaSetDevice(e->cfg.device));
     ReplayPolicy &P = e->rp;
@@ -1669,6 +1782,7 @@ extern "C" int b200_replay_policy_step(b200_engine *e, int64_t current_episode, 
 
 // after train(...): ++n_trains; memory_index = 0; last_training_episode = current_episode (agent.cpp:697-701)
 extern "C" int b200_replay_policy_trained(b200_engine *e, int64_t current_episode) {
+    if (e) REFUSE_IF_OPEN(e, "b200_replay_policy_trained");
     if (!e || e->rp.policy < 0) return fail(B200_ERR_BAD_ARG, "no replay policy configured");
     CK(cudaSetDevice(e->cfg.device));
     e->rp.n_trains += 1;
@@ -1680,6 +1794,7 @@ extern "C" int b200_replay_policy_trained(b200_engine *e, int64_t current_episod
 // Append n rows (HOST, 212 bytes each, the format k_gc stores) to the memory exactly as a collection would: in order, until the memory is full
 // (agent.cpp:817).  Seeds the memory from a dump file (ValueSim.py:176-177) or from another process; the policy tests script collections with it.
 extern "C" int b200_replay_append(b200_engine *e, const uint8_t *rows, int n) {
+    if (e) REFUSE_IF_OPEN(e, "b200_replay_append");
     if (!e || !e->A.replay || (n > 0 && !rows) || n < 0) return fail(B200_ERR_BAD_ARG, "replay memory not enabled / bad argument");
     CK(cudaSetDevice(e->cfg.device));
     int32_t count = 0;
@@ -1693,6 +1808,7 @@ extern "C" int b200_replay_append(b200_engine *e, const uint8_t *rows, int n) {
 
 // b200_replay_append from a DEVICE buffer: rank 0 of a data-parallel run appends the rows the other ranks' collections stored this move
 extern "C" int b200_replay_append_dev(b200_engine *e, const void *rows, int n) {
+    if (e) REFUSE_IF_OPEN(e, "b200_replay_append_dev");
     if (!e || !e->A.replay || (n > 0 && !rows) || n < 0) return fail(B200_ERR_BAD_ARG, "replay memory not enabled / bad argument");
     CK(cudaSetDevice(e->cfg.device));
     int32_t count = 0;
@@ -1706,6 +1822,7 @@ extern "C" int b200_replay_append_dev(b200_engine *e, const void *rows, int n) {
 
 // the first n rows of the memory, copied to a DEVICE buffer without emptying it (the arrays the reference hands to train(): m_state ... [:memory_index])
 extern "C" int b200_replay_peek_dev(b200_engine *e, void *out_dev, int n) {
+    if (e) REFUSE_IF_OPEN(e, "b200_replay_peek_dev");
     if (!e || !out_dev || n < 0 || !e->A.replay || n > e->replay_alloc) return fail(B200_ERR_BAD_ARG, "bad argument");
     CK(cudaSetDevice(e->cfg.device));
     if (n > 0) CK(cudaMemcpyAsync(out_dev, e->A.replay, (size_t)n * 212, cudaMemcpyDeviceToDevice, e->stream));

@@ -20,7 +20,7 @@ class BatchedEngine:
                  dist_weights=None, path_cache=None):
         mode_id = {"lp": L.MODE_LP, "single": L.MODE_SINGLE, "vanilla": L.MODE_VANILLA, "dist": L.MODE_DIST}[mode] if isinstance(mode, str) else int(mode)
         eval_id = {"synthetic": L.EVAL_SYNTHETIC, "net": L.EVAL_NET, "net_tc": L.EVAL_NET_TC, "net_fp16": L.EVAL_NET_FP16,
-                   "dist_fp16": L.EVAL_DIST_FP16}[eval_kind] if isinstance(eval_kind, str) else int(eval_kind)
+                   "dist_fp16": L.EVAL_DIST_FP16, "external": L.EVAL_EXTERNAL}[eval_kind] if isinstance(eval_kind, str) else int(eval_kind)
         if tuple(env_args[0]) != (20, 10):
             raise ValueError("only 20x10 boards (SPEC_PYTETRIS.md §1)")
         cfg = L.Config()
@@ -38,6 +38,7 @@ class BatchedEngine:
         self.n_games, self.max_nodes, self.mode, self.eval_kind = int(n_games), int(max_nodes), mode_id, eval_id
         self.h = L.P()
         self.path_cache = False
+        self._ext = None                      # eval_kind external: the board and output buffers and the stream the evaluator runs on
         L.check(L.lib().b200_engine_create(C.byref(cfg), C.byref(self.h)))
         if weights is not None:
             self.load_weights(weights)
@@ -123,8 +124,17 @@ class BatchedEngine:
     def update_root(self, auto_reset=False):
         L.check(L.lib().b200_update_root(self.h, int(auto_reset)))
 
-    def run_sims(self, sims):
-        L.check(L.lib().b200_run_sims(self.h, int(sims)))
+    def run_sims(self, sims, evaluator=None, board_dtype="float32", host=False):
+        """`sims` simulation steps of every game.  evaluator (eval_kind "external" only) evaluates each step's boards:
+        host=False: evaluator(boards) gets a torch tensor [n,1,20,10] (board_dtype "float32" or "int8") on the engine's device, called on
+        the engine's stream, and returns (v, var) each [n] or [n,1] (in mode "dist": [n, atoms], or a list of one such), float32 on that
+        device; the outputs go to the engine without a host round trip.  host=True: the reference's callback, evaluator(int8 ndarray
+        [n,1,20,10]) -> [v (n,1), var (n,1)] or [probs (n, atoms)] as numpy float32 (Model_VV.inference as it is)."""
+        if evaluator is None:
+            L.check(L.lib().b200_run_sims(self.h, int(sims)))
+            return
+        for _ in range(int(sims)):
+            self._ext_step(evaluator, "int8" if host else board_dtype, host)
 
     def get_stats(self):
         stats = np.zeros((self.n_games, 3, L.N_ACTIONS), np.float32)
@@ -136,8 +146,16 @@ class BatchedEngine:
         a = None if actions is None else np.ascontiguousarray(actions, np.int32)
         L.check(L.lib().b200_env_step(self.h, L.ptr(a)))
 
-    def play_move(self, sims, auto_reset=True, want_stats=True):
-        """One move of play.py:118-177 for every game. Returns (actions, stats)."""
+    def play_move(self, sims, auto_reset=True, want_stats=True, evaluator=None, board_dtype="float32", host=False):
+        """One move of play.py:118-177 for every game. Returns (actions, stats).  evaluator / board_dtype / host: see run_sims (eval_kind
+        "external"); the move is then run_sims, get_stats, env_step, update_root, as b200_play_move does it."""
+        if evaluator is not None:
+            self.run_sims(sims, evaluator, board_dtype, host)
+            stats, actions = self.get_stats()
+            self.env_step(None)
+            self.update_root(auto_reset)
+            self.sync()
+            return actions, (stats if want_stats else None)
         actions = np.zeros(self.n_games, np.int32)
         stats = np.zeros((self.n_games, 3, L.N_ACTIONS), np.float32) if want_stats else None
         L.check(L.lib().b200_play_move(self.h, int(sims), int(auto_reset), L.ptr(actions), L.ptr(stats)))
@@ -162,6 +180,8 @@ class BatchedEngine:
         attribute (torch.cuda.Stream), or None for a private stream again.  The caller keeps the stream alive."""
         handle = 0 if stream is None else int(getattr(stream, "cuda_stream", stream))
         L.check(L.lib().b200_engine_set_stream(self.h, C.c_void_p(handle)))
+        if self._ext is not None:
+            self._ext["stream"] = None
 
     def get_stream(self):
         """The cudaStream_t (int) the engine issues its work on — e.g. torch.cuda.ExternalStream(engine.get_stream())."""
@@ -228,6 +248,59 @@ class BatchedEngine:
         L.check(L.lib().b200_valuenet_forward(self.h, L.ptr(s), len(s), L.ptr(v), L.ptr(var)))
         return v, var
 
+    # ------------------------------------------------------------------ the caller's evaluator (eval_kind "external")
+    def ext_capacity(self):
+        """(max_rows, out_cols): the most boards one step hands out (7 * n_games in LP, n_games otherwise) and the outputs per board
+        (2 = v, var; dist_bins in mode "dist")."""
+        rows, cols = np.zeros(1, np.int32), np.zeros(1, np.int32)
+        L.check(L.lib().b200_ext_capacity(self.h, L.ptr(rows), L.ptr(cols)))
+        return int(rows[0]), int(cols[0])
+
+    def ext_step_begin(self, boards, board_dtype="float32", ids=None):
+        """First half of one simulation step: boards (a DEVICE tensor or pointer of max_rows * 200 elements) receive this step's boards in
+        ascending (game, slot) order; ids (optional, int32 DEVICE) = game * 8 + slot of each row.  Synchronises; returns n_rows."""
+        n = np.zeros(1, np.int32)
+        L.check(L.lib().b200_ext_step_begin(self.h, C.c_void_p(_dev_ptr(boards)), _BOARD_DTYPES[board_dtype],
+                                            None if ids is None else C.c_void_p(_dev_ptr(ids)), L.ptr(n)))
+        return int(n[0])
+
+    def ext_step_end(self, out):
+        """Second half: out (a DEVICE fp32 tensor or pointer, [n_rows][out_cols] row-major) into the search, then the backup (asynchronous)."""
+        L.check(L.lib().b200_ext_step_end(self.h, C.c_void_p(_dev_ptr(out))))
+
+    def _ext_buffers(self, board_dtype):
+        import torch
+        if self._ext is None:
+            rows, cols = self.ext_capacity()
+            dev = torch.device("cuda", int(self.cfg.device))
+            self._ext = dict(rows=rows, cols=cols, device=dev, boards={}, stream=None,
+                             out=torch.empty((rows, cols), dtype=torch.float32, device=dev))
+        ext = self._ext
+        if board_dtype not in ext["boards"]:
+            ext["boards"][board_dtype] = torch.empty((ext["rows"], 1, 20, 10), dtype=getattr(torch, board_dtype), device=ext["device"])
+        if ext["stream"] is None:
+            ext["stream"] = torch.cuda.ExternalStream(self.get_stream(), device=ext["device"])
+        return ext
+
+    def _ext_step(self, evaluator, board_dtype, host):
+        """One simulation step through the caller's evaluator.  An output of the wrong form raises ValueError before anything is submitted:
+        the step stays open, and ext_step_end with correct outputs completes it."""
+        import torch
+        ext = self._ext_buffers(board_dtype)
+        boards, out = ext["boards"][board_dtype], ext["out"]
+        n = self.ext_step_begin(boards, board_dtype)
+        if n:
+            dist = self.mode == L.MODE_DIST
+            with torch.cuda.stream(ext["stream"]):
+                if host:
+                    parts = ext_output_parts(evaluator(boards[:n].cpu().numpy()), n, ext["cols"], dist, host=True)
+                    parts = [torch.from_numpy(p) for p in parts]
+                else:
+                    parts = ext_output_parts(evaluator(boards[:n]), n, ext["cols"], dist, device=ext["device"])
+                for j, p in enumerate(parts):
+                    out[:n, j:j + p.shape[1]].copy_(p)
+        self.ext_step_end(out)
+
     def replay_enable(self, min_visits=25, capacity=500000):
         """ValueSim(online=True) replay memory (agents/ValueSim.py:14-37; min_visits_to_store=25 for ValueSimLP.py:11)."""
         L.check(L.lib().b200_replay_enable(self.h, int(min_visits), int(capacity)))
@@ -267,3 +340,41 @@ class BatchedEngine:
         cnt = np.zeros(1, np.int32)
         L.check(L.lib().b200_collect_samples_dev(self.h, int(min_visits), C.c_void_p(int(dev_ptr)), int(capacity), L.ptr(cnt)))
         return int(cnt[0])
+
+
+_BOARD_DTYPES = {"int8": L.BOARD_INT8, "float32": L.BOARD_F32}
+
+
+def _dev_ptr(x):
+    return int(x.data_ptr()) if hasattr(x, "data_ptr") else int(x)
+
+
+def ext_output_parts(res, n, cols, dist, host=False, device=None):
+    """An evaluator's return value for n boards -> the column blocks of the [n, cols] output, each 2-D: value modes (v, var), each of shape
+    (n,) or (n,1) -> [(n,1), (n,1)]; mode dist (n, cols), or a list / tuple of one such (Model_Dist.inference's return) -> [(n, cols)].
+    host: numpy float32 arrays; otherwise torch float32 tensors on `device`.  Anything else raises ValueError."""
+    if dist:
+        if isinstance(res, (list, tuple)):
+            if len(res) != 1:
+                raise ValueError("a distributional evaluator returns probs (n, atoms) or [probs]; got a sequence of %d" % len(res))
+            res = res[0]
+        parts, shapes = [res], [(n, cols)]
+    else:
+        if not isinstance(res, (list, tuple)) or len(res) != 2:
+            raise ValueError("a value evaluator returns (v, var); got %r" % (type(res).__name__,))
+        parts, shapes = list(res), [(n,), (n, 1)]
+    out = []
+    for p in parts:
+        if host:
+            if not isinstance(p, np.ndarray) or p.dtype != np.float32:
+                raise ValueError("a host evaluator returns numpy float32 arrays; got %r" % (getattr(p, "dtype", type(p).__name__),))
+        else:
+            import torch
+            if not isinstance(p, torch.Tensor) or p.dtype != torch.float32 or p.device != device:
+                raise ValueError("a device evaluator returns torch float32 tensors on %s; got %s" % (
+                    device, (p.dtype, p.device) if isinstance(p, torch.Tensor) else type(p).__name__))
+        shape = tuple(p.shape)
+        if shape not in shapes:
+            raise ValueError("evaluator output of shape %s for %d boards; expected %s" % (shape, n, " or ".join(map(str, shapes))))
+        out.append(p.reshape(n, -1))
+    return out

@@ -14,6 +14,10 @@ rows (Model_VV.train_rows), saved to ./pytorch_model/model_checkpoint and swappe
 
   python -m tetris_mcts_b200.play_batched --agent_type ValueSimLP --mcts_sims 100 --ngames 1000 --n_parallel 4096 --endless
   torchrun --nproc-per-node 8 -m tetris_mcts_b200.play_batched --agent_type ValueSimLP --online --n_parallel 32768 --endless
+  python -m tetris_mcts_b200.play_batched --agent_type ValueSimLP --evaluator mynets:make_evaluator --n_parallel 4096 --endless
+
+--evaluator MODULE:FACTORY searches with the caller's network instead of the built-in one: FACTORY(device) returns a device evaluator
+(BatchedEngine.run_sims: a torch tensor [n,1,20,10] of boards in, (v, var) out), and the engine runs eval_kind "external".
 
 Flags are play.py's (play.py:46-70) plus --n_parallel / --max_nodes / --device / --watch / --seed and the online agent's memory and training
 settings.  One "episode" is one finished game of any of the parallel games; episodes are numbered in the order (move, game index) they end."""
@@ -94,8 +98,13 @@ def run(args, out=sys.stdout, timing=None):
     device = args.device if world == 1 else D.env_world()[1]
     mode, gamma, low = MODES[args.agent_type]
     env_args = ((20, 10), args.app, args.tetris_scoring, args.tetris_randomizer)           # play.py:75
-    weights = None
-    if mode != "vanilla":
+    weights, evaluator = None, None
+    if args.evaluator:
+        import importlib
+        import torch
+        module, factory = args.evaluator.split(":", 1)
+        evaluator = getattr(importlib.import_module(module), factory)(torch.device("cuda", device))
+    elif mode != "vanilla":
         from .model.model_vv import init_weights, load_checkpoint_weights
         if rank == 0:
             weights = load_checkpoint_weights()                                             # agents/ValueSim.py:42-44
@@ -107,7 +116,7 @@ def run(args, out=sys.stdout, timing=None):
             weights = init_weights(0)
     # k_init_arena seeds game g's search stream with seed + 0x9E3779B9 * (g + 1): offset by the shard's first global index
     eng = BatchedEngine(hi - lo, max_nodes=args.max_nodes, mode=mode, gamma=gamma, low=low,
-                        eval_kind=args.eval_kind if mode != "vanilla" else "synthetic", weights=weights, env_args=env_args,
+                        eval_kind="external" if evaluator else (args.eval_kind if mode != "vanilla" else "synthetic"), weights=weights, env_args=env_args,
                         seed=(args.seed + 0x9E3779B9 * lo) & 0xFFFFFFFF, device=device, overflow_reset=True)
     eng.set_games(PT.new_games(hi - lo, env_args, D.shard_seeds(args.seed, args.n_parallel, rank, world)))
     eng.set_gc_headroom(args.max_nodes * 5 // 32)
@@ -137,7 +146,8 @@ def run(args, out=sys.stdout, timing=None):
             if status:
                 status.update(eng.get_games()[args.watch - lo])
             before = eng.get_games() if saver else None
-            actions, stats = eng.play_move(args.mcts_sims, auto_reset=True, want_stats=saver is not None)   # agent.play(); game.play(action); agent.update_root(game); reset
+            actions, stats = eng.play_move(args.mcts_sims, auto_reset=True, want_stats=saver is not None,
+                                           evaluator=evaluator)   # agent.play(); game.play(action); agent.update_root(game); reset
             if saver:
                 saver.add_rows(rows_from_move(before, actions, stats, args.cycle, episode_of))
             moves += 1
@@ -240,10 +250,20 @@ def parse_args(argv=None):
     p.add_argument('--eval_kind', default='net_tc', choices=('net_tc', 'net_fp16'),
                    help='value network of the search (not Vanilla): net_tc = tensor cores within 1e-5 of fp32, net_fp16 = one fp16 product per '
                         'product, about a third of the tensor-core work (DESIGN §5).  --online trains in fp32 / fp64 either way')
+    p.add_argument('--evaluator', default=None, metavar='MODULE:FACTORY',
+                   help='search with the caller\'s network: FACTORY(device) returns a device evaluator (boards [n,1,20,10] -> (v, var)); '
+                        'the engine runs eval_kind external.  Not with --online (the trainer trains the built-in network) nor Vanilla')
     p.add_argument('--max_moves', default=0, type=int)
     p.add_argument('--dist_backend', default='nccl', choices=('nccl', 'gloo'),
                    help='under torchrun: collectives over NCCL (one GPU per rank), or gloo through the host (several ranks may share a GPU)')
-    return p.parse_args(argv)
+    args = p.parse_args(argv)
+    if args.evaluator and args.online:
+        p.error('--evaluator cannot be combined with --online: the online trainer trains the built-in Model_VV weights')
+    if args.evaluator and args.agent_type == 'Vanilla':
+        p.error('--evaluator cannot be combined with --agent_type Vanilla: Vanilla evaluates leaves by random rollout')
+    if args.evaluator and ':' not in args.evaluator:
+        p.error('--evaluator takes MODULE:FACTORY')
+    return args
 
 
 def main(argv=None, out=sys.stdout):
