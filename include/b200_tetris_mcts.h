@@ -207,6 +207,8 @@ int b200_backup_trace_obs_LP(const int32_t *trace, int D, int32_t *visit, float 
                              const int32_t *n_to_o, const float *score, const uint8_t *end, int M,
                              const int32_t *c_nodes, const int32_t *c_obs, int k, const float *v, const float *var,
                              double gamma, int mixture, int averaged);
+/* test aid: the walk's z(n) for n[count] (host table below 65536, evaluated on the device above; DESIGN §3 states the exact range) */
+int b200_debug_ztab(const int32_t *n, int count, float *out);
 int b200_get_unique_child_obs(int index, const int32_t *child, const float *score, const int32_t *n_to_o, int M,
                               int32_t *c_nodes, int32_t *c_obs, int32_t *k_out);
 int b200_get_all_childs(int index, const int32_t *child, int M, uint8_t *mark);
@@ -243,6 +245,16 @@ int b200_debug_tc_acts(b200_engine *e, int dist, const int8_t *states, int k, in
  * ReLU).  dist = 1, the distributional network: layer 0 = probabilities out[k][atoms], 1 = act1 [32][19][7], 2 = act2 [32][16][4] (the
  * production buffer), 3 = fc1's accumulator out[k][128] (bias included, before the LeakyReLU), 4 = the logits out[k][atoms]. */
 int b200_debug_net_acts(b200_engine *e, int dist, const int8_t *states, int k, int layer, float *out);
+/* test aid: the production backup (k_backup, launched as b200_run_sims launches it) on a tree in the reference's layout (agents/agent.py:58-88),
+ * on a one-game engine of mode lp, single or vanilla (others, or more games, return B200_ERR_BAD_ARG).  child[M][7], n_to_o[M], score[M] per
+ * node; visit / value / variance / end[M] per observation (the first three updated in place); trace[D] (D <= trace_max); leaf_kind 0 = terminal,
+ * 1 = expanded; eval_out[8][2] = (value, variance) per child slot (LP) or of the leaf in slot 7 (single); rollout_val (vanilla).  Overwrites
+ * the engine's tree of game 0 with the given one.  With the path cache on (and only then) pc_len points to the number of entries the walk left
+ * valid (<= D - 1 after an expansion, <= D at a terminal leaf); they are filled from the given arena as the walk stores them, and pc_len, the
+ * own records pc_own[D][4], the child ids pc_sib[D][8], the entries pc_ent[D][8][4] and pc_var[D][8] come back as the backup left them. */
+int b200_debug_backup(b200_engine *e, int M, const int32_t *child, const int32_t *n_to_o, const float *score, int32_t *visit, float *value,
+                      float *variance, const uint8_t *end, const int32_t *trace, int D, int leaf_kind, const float *eval_out, float rollout_val,
+                      int32_t *pc_len, int32_t *pc_own, uint16_t *pc_sib, int32_t *pc_ent, int32_t *pc_var);
 int b200_export_dist(b200_engine *e, int game, float *node_stats /* [M][5] */, float *node_dist /* [M][bins] */);
 
 /* --- replay samples of the live search (ValueSim.store_nodes, agents/ValueSim.py:122-159): observations with

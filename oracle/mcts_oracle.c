@@ -18,6 +18,11 @@ double mo_norm_quantile(double t) {
     return 10 * log(1 - log(-log(alpha) / l2) / l22) / l41;
 }
 
+/* core.h:93's bound coefficient for many n at once: mo_norm_quantile narrowed to float, as the engine's host table holds it */
+void mo_norm_quantile_f32(const int32_t *n, int count, float *out) {
+    for (int i = 0; i < count; ++i) out[i] = (float)mo_norm_quantile((double)n[i]);
+}
+
 /* ------------------------------------------------------------------ core.h:111-144 */
 int mo_unique_child_obs(int index, const int32_t *child, const float *score, const int32_t *n2o,
                         int32_t *c_nodes, int32_t *c_obs) {

@@ -21,6 +21,7 @@ extern "C" {
 typedef uint32_t (*mo_rand_fn)(void *ctx); /* stands in for libc rand() of core.h:62,76 */
 
 double mo_norm_quantile(double t);                                             /* special.h:26-33 */
+void mo_norm_quantile_f32(const int32_t *n, int count, float *out);            /* (float)mo_norm_quantile(n[i]) */
 int mo_unique_child_obs(int index, const int32_t *child, const float *score, const int32_t *n2o,
                         int32_t *c_nodes, int32_t *c_obs);                     /* core.h:111-144 */
 int mo_policy_clt(const int32_t *nodes, const int32_t *visit, const float *value, const float *variance, int k); /* core.h:83-105 */

@@ -58,6 +58,7 @@ def _p(a):
 def _sig(L):
     L.mo_norm_quantile.restype = C.c_double
     L.mo_norm_quantile.argtypes = [C.c_double]
+    L.mo_norm_quantile_f32.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
     L.mo_agent_create.restype = C.c_void_p
     L.mo_agent_create.argtypes = [C.POINTER(MoConfig), C.c_int, C.c_int, C.c_int]
     L.mo_agent_destroy.argtypes = [C.c_void_p]
@@ -164,6 +165,14 @@ def obskey_to_state(key):
 
 
 # ----------------------------------------------------------------------------- core twins
+def norm_quantile_f32(n):
+    """z(n) of policy_clt (special.h:26-33 narrowed to float, core.h:93) with the host libm, for an int32 array of n."""
+    n = np.ascontiguousarray(n, np.int32)
+    out = np.empty(len(n), np.float32)
+    lib().mo_norm_quantile_f32(_p(n), len(n), _p(out))
+    return out
+
+
 def select_trace_obs(index, child, visit, value, variance, score, n2o, low, max_trace=512, rng_state=None):
     """rng_state: uint32[1] array -> check_low draws come from xorshift32 on it (as in the device twin);
     None -> libc rand() like the reference (core.h:76)."""

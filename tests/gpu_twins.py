@@ -45,3 +45,31 @@ def get_all_childs(index, child):
     mark = np.zeros(child.shape[0], np.uint8)
     L.check(L.lib().b200_get_all_childs(int(index), L.ptr(child), child.shape[0], L.ptr(mark)))
     return set(np.nonzero(mark)[0].tolist())
+
+
+def debug_backup(eng, c, pc_len=None):
+    """The production k_backup on case c (tests/backup_edges.py layout) through b200_debug_backup on the one-game engine `eng`.
+    Returns (visit, value, variance) and, with pc_len given (the path cache on), a dict of what the backup left in the cache."""
+    visit, value, variance = c["visit"].copy(), c["value"].copy(), c["variance"].copy()
+    child = np.ascontiguousarray(c["child"], np.int32)
+    M, D = child.shape[0], len(c["trace"])
+    ev = np.ascontiguousarray(c["ev"], np.float32)
+    pc = None
+    if pc_len is not None:
+        pc = dict(pc_len=np.array([pc_len], np.int32), own=np.zeros((D, 4), np.int32), sib=np.zeros((D, 8), np.uint16),
+                  ent=np.zeros((D, 8, 4), np.int32), var=np.zeros((D, 8), np.int32))
+    g = pc or {}
+    L.check(L.lib().b200_debug_backup(eng.h, M, L.ptr(child), L.ptr(np.ascontiguousarray(c["n2o"], np.int32)),
+                                      L.ptr(np.ascontiguousarray(c["score"], np.float32)), L.ptr(visit), L.ptr(value), L.ptr(variance),
+                                      L.ptr(np.ascontiguousarray(c["end"], np.uint8)), L.ptr(np.ascontiguousarray(c["trace"], np.int32)), D,
+                                      int(c["kind"]), L.ptr(ev), float(c["rollout"]), L.ptr(g.get("pc_len")), L.ptr(g.get("own")),
+                                      L.ptr(g.get("sib")), L.ptr(g.get("ent")), L.ptr(g.get("var"))))
+    return (visit, value, variance), pc
+
+
+def ztab(n):
+    """The walk's z(n) on the device (search_dev.cuh ztab) for an int32 array of n."""
+    n = np.ascontiguousarray(n, np.int32)
+    out = np.empty(len(n), np.float32)
+    L.check(L.lib().b200_debug_ztab(L.ptr(n), len(n), L.ptr(out)))
+    return out

@@ -1373,6 +1373,101 @@ extern "C" int b200_tetris_state(const uint32_t *recs, int8_t *out, int n) {
     return env_stream_op(const_cast<uint32_t *>(recs), nullptr, out, n);
 }
 
+// development / test aid: the production k_backup (through step_backup, the launch run_sims uses) on a tree given in the reference's layout
+// (agents/agent.py:58-88), on game 0 of a one-game engine.  The game's row (c / o / s from child, n_to_o, score; the link words by
+// finish_expansion), stat (visit / value / variance / end per observation), trace, trace_meta (own observation | pick << 28, own score; the
+// pick = the first slot holding the next level's observation), leaf_kind and the evaluator outputs (eval_out[8][2] per slot, rollout_val)
+// are written as a walk and an evaluation would leave them; visit / value / variance come back in place.  With the path cache on, pc_len
+// (in: the entries the walk left valid, <= D - 1 after an expansion, <= D at a terminal leaf) is filled from the pre-backup arena by the
+// walk's own store (k_debug_pc_fill) and returned with the entries: pc_own[D][4], pc_sib[D][8], pc_ent[D][8][4] ({link word, val, visit,
+// root}; slot 7 {0, own score, own observation, node}), pc_var[D][8].
+extern "C" int b200_debug_backup(b200_engine *e, int M, const int32_t *child, const int32_t *n_to_o, const float *score, int32_t *visit,
+                                 float *value, float *variance, const uint8_t *end, const int32_t *trace, int D, int leaf_kind,
+                                 const float *eval_out, float rollout_val, int32_t *pc_len, int32_t *pc_own, uint16_t *pc_sib,
+                                 int32_t *pc_ent, int32_t *pc_var) {
+    if (!e || !child || !n_to_o || !score || !visit || !value || !variance || !end || !trace || !eval_out) return fail(B200_ERR_BAD_ARG, "bad argument");
+    REFUSE_IF_OPEN(e, "b200_debug_backup");
+    Arena &A = e->A;
+    if (A.G != 1 || (A.mode != MODE_LP && A.mode != MODE_SINGLE && A.mode != MODE_VANILLA)) return fail(B200_ERR_BAD_ARG, "b200_debug_backup needs a one-game engine of mode lp, single or vanilla");
+    if (M < 2 || M > A.M || D < 1 || D > A.trace_max) return fail(B200_ERR_BAD_ARG, "need 2 <= M <= max_nodes and 1 <= D <= trace_max");
+    if (leaf_kind != LEAF_TERMINAL && leaf_kind != LEAF_EXPANDED) return fail(B200_ERR_BAD_ARG, "leaf_kind: 0 terminal or 1 expanded");
+    if (!A.pc != !pc_len || (pc_len && (!pc_own || !pc_sib || !pc_ent || !pc_var)))
+        return fail(B200_ERR_BAD_ARG, "pc_len and the entry buffers are given exactly when the path cache is on");
+    if (pc_len && (*pc_len < 0 || *pc_len > (leaf_kind == LEAF_EXPANDED ? D - 1 : D))) return fail(B200_ERR_BAD_ARG, "pc_len beyond what a walk leaves valid");
+    for (int i = 0; i < M; ++i)
+        if (n_to_o[i] < 0 || n_to_o[i] >= M) return fail(B200_ERR_BAD_ARG, "n_to_o out of range");
+    for (int i = 0; i < M * 7; ++i)
+        if (child[i] < 0 || child[i] >= M) return fail(B200_ERR_BAD_ARG, "child out of range");
+    for (int d = 0; d < D; ++d)
+        if (trace[d] < 1 || trace[d] >= M) return fail(B200_ERR_BAD_ARG, "trace entry out of range");
+    CK(cudaSetDevice(e->cfg.device));
+    CK(cudaStreamSynchronize(e->stream));
+    std::vector<int32_t> row((size_t)M * ROW_WORDS, 0);
+    std::vector<int4> st(M);
+    for (int i = 0; i < M; ++i) {
+        int32_t *r = &row[(size_t)i * ROW_WORDS];
+        for (int a = 0; a < 7; ++a) { const int c = child[(size_t)i * 7 + a]; r[a] = c; r[8 + a] = n_to_o[c]; memcpy(&r[16 + a], &score[c], 4); }
+        r[15] = n_to_o[i]; memcpy(&r[23], &score[i], 4);
+        int4 s; s.x = visit[i]; memcpy(&s.y, &value[i], 4); memcpy(&s.z, &variance[i], 4); s.w = end[i] != 0;
+        st[i] = s;
+    }
+    std::vector<int2> meta(D);
+    for (int d = 0; d < D; ++d) {
+        const int32_t *r = &row[(size_t)trace[d] * ROW_WORDS];
+        int pick = 0;
+        if (d + 1 < D) {
+            const int want = n_to_o[trace[d + 1]];
+            pick = 7;
+            for (int a = 0; a < 7 && pick == 7; ++a) if (r[a] != 0 && r[8 + a] == want) pick = a;
+        }
+        meta[d] = make_int2(r[15] | (pick << 28), r[23]);
+    }
+    const int32_t st_ok = ST_OK;
+    CK(cudaMemcpyAsync(A.row, row.data(), row.size() * 4, cudaMemcpyHostToDevice, e->stream));
+    CK(cudaMemcpyAsync(A.stat, st.data(), (size_t)M * sizeof(int4), cudaMemcpyHostToDevice, e->stream));
+    CK(cudaMemcpyAsync(A.trace, trace, (size_t)D * 4, cudaMemcpyHostToDevice, e->stream));
+    CK(cudaMemcpyAsync(A.trace_meta, meta.data(), (size_t)D * sizeof(int2), cudaMemcpyHostToDevice, e->stream));
+    CK(cudaMemcpyAsync(A.trace_len, &D, 4, cudaMemcpyHostToDevice, e->stream));
+    CK(cudaMemcpyAsync(A.leaf_kind, &leaf_kind, 4, cudaMemcpyHostToDevice, e->stream));
+    CK(cudaMemcpyAsync(A.status, &st_ok, 4, cudaMemcpyHostToDevice, e->stream));
+    CK(cudaMemcpyAsync(A.eval_out, eval_out, 8 * sizeof(float2), cudaMemcpyHostToDevice, e->stream));
+    CK(cudaMemcpyAsync(A.rollout_val, &rollout_val, 4, cudaMemcpyHostToDevice, e->stream));
+    k_debug_link_rows<<<(M + 15) / 16, 128, 0, e->stream>>>(A, 0, M);
+    if (pc_len) {
+        k_debug_pc_fill<<<1, 8, 0, e->stream>>>(A, 0, *pc_len, D);
+        CK(cudaMemcpyAsync(A.pc_len, pc_len, 4, cudaMemcpyHostToDevice, e->stream));
+    }
+    step_backup(e);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(st.data(), A.stat, (size_t)M * sizeof(int4), cudaMemcpyDeviceToHost, e->stream));
+    std::vector<int4> own, ent((size_t)8 * A.trace_max);
+    std::vector<uint4> sib;
+    std::vector<int32_t> pvar((size_t)8 * A.trace_max);
+    if (pc_len) {
+        own.resize(D); sib.resize(D);
+        CK(cudaMemcpyAsync(pc_len, A.pc_len, 4, cudaMemcpyDeviceToHost, e->stream));
+        CK(cudaMemcpyAsync(own.data(), A.pc_own, (size_t)D * sizeof(int4), cudaMemcpyDeviceToHost, e->stream));
+        CK(cudaMemcpyAsync(sib.data(), A.pc_sib, (size_t)D * sizeof(uint4), cudaMemcpyDeviceToHost, e->stream));
+        CK(cudaMemcpyAsync(ent.data(), A.pc, ent.size() * sizeof(int4), cudaMemcpyDeviceToHost, e->stream));
+        CK(cudaMemcpyAsync(pvar.data(), A.pc_var, pvar.size() * 4, cudaMemcpyDeviceToHost, e->stream));
+    }
+    CK(cudaStreamSynchronize(e->stream));
+    for (int i = 0; i < M; ++i) { visit[i] = st[i].x; memcpy(&value[i], &st[i].y, 4); memcpy(&variance[i], &st[i].z, 4); }
+    if (pc_len) {
+        for (int d = 0; d < D; ++d) {
+            pc_own[4 * d] = own[d].x; pc_own[4 * d + 1] = own[d].y; pc_own[4 * d + 2] = own[d].z; pc_own[4 * d + 3] = own[d].w;
+            memcpy(pc_sib + 8 * d, &sib[d], 16);
+            for (int a = 0; a < 8; ++a) {   // slot-major [8][trace_max] on the device
+                const int4 v = ent[(size_t)a * A.trace_max + d];
+                int32_t *o = pc_ent + ((size_t)d * 8 + a) * 4;
+                o[0] = v.x; o[1] = v.y; o[2] = v.z; o[3] = v.w;
+                pc_var[(size_t)d * 8 + a] = pvar[(size_t)a * A.trace_max + d];
+            }
+        }
+    }
+    return B200_OK;
+}
+
 // ---------------------------------------------------------------------------------------------------- core twins
 struct TwinBufs {
     int32_t *child = nullptr, *visit = nullptr, *n2o = nullptr, *trace = nullptr, *out = nullptr;
@@ -1488,6 +1583,20 @@ extern "C" int b200_backup_trace_obs_LP(const int32_t *trace, int D, int32_t *vi
     k_twin_backup_lp<<<1, 1>>>(A, t, D, d_end, d_cn, d_co, k, d_v, d_var, gamma, mixture, averaged);
     CK(cudaGetLastError());
     TW(twin_backup_fetch(b, visit, value, variance, M));
+    return B200_OK;
+}
+
+// test aid: the walk's z(n) (search_dev.cuh ztab) for n[count]: out[i] as policy_clt's bound coefficient (core.h:93) on the device
+extern "C" int b200_debug_ztab(const int32_t *n, int count, float *out) {
+    if (!n || !out || count < 1) return fail(B200_ERR_BAD_ARG, "bad argument");
+    if (b200_device_count() == 0) return fail(B200_ERR_CUDA, "no CUDA device: this library has no CPU path");
+    TwinBufs b; Arena A;
+    TW(twin_arena(b, A));
+    int32_t *d_n = nullptr; float *d_out = nullptr;
+    TW(b.up(&d_n, n, (size_t)count)); TW(b.up(&d_out, (const float *)nullptr, (size_t)count));
+    k_debug_ztab<<<256, 256>>>(A, d_n, count, d_out);
+    CK(cudaGetLastError());
+    CK(cudaMemcpy(out, d_out, (size_t)count * 4, cudaMemcpyDeviceToHost));
     return B200_OK;
 }
 

@@ -895,6 +895,49 @@ __global__ void k_twin_backup_lp(Arena A, TwinArgs t, int D, const uint8_t *end,
     lp_backup(acc, D, k, co, cs, ev, evar, ce, gamma, mixture != 0, averaged != 0, true, leaf_score);
 }
 
+// ---------------------------------------------------------------- test aid of b200_debug_backup: a given tree as the engine would hold it
+// The de-duplicated child list of every node, written by the expansion's own finish_expansion (one 8-lane group per node).
+__global__ void k_debug_link_rows(Arena A, int g, int n_nodes) {
+    Grp gp;
+    const int node = blockIdx.x * (blockDim.x >> 3) + (threadIdx.x >> 3);
+    if (node >= n_nodes) return;
+    const int32_t *row = A.row + node_at(A, g, node) * ROW_WORDS;
+    const int c = gp.lane < 7 ? row[gp.lane] : 0, o = row[8 + gp.lane];
+    const float s = __int_as_float(row[16 + gp.lane]);
+    finish_expansion(A, gp, g, node, c, o, s);
+}
+
+// The path-cache entries of levels [0, n) as select_trace's uncached form stores them (one 8-lane group; the pick of each level is the one
+// recorded in trace_meta), and the own record of every trace level as the last backup left it.
+__global__ void k_debug_pc_fill(Arena A, int g, int n, int D) {
+    Grp gp;
+    ArenaAcc acc(A, g);
+    for (int L = 0; L < n; ++L) {
+        int o, oraw; float s_idx, s_own, sm; uint32_t lw; Uniq u;
+        acc.level(gp, true, acc.get_trace(L), L, o, s_idx, u, s_own, lw);
+        acc.get_trace_meta_raw(L, oraw, sm);
+        const bool has = u.first_mask != 0u;
+        const int4 st = (has && u.is_first) ? acc.stat(o) : make_int4(0, 0, 0, 0);
+        const bool cmp = has && u.is_first;                              // select_trace's choose(): val / root of every list entry
+        const float q_val = cmp ? clt_val(__int_as_float(st.y), u.rep_s, s_idx) : 0.f;
+        const float q_root = cmp ? clt_root(__int_as_float(st.z), st.x) : 0.f;
+        const int pk = has ? (int)(((uint32_t)oraw >> 28) & 7u) : 7;
+        acc.pc_store(L, gp.lane, gp.lane == 7 ? make_int4(0, __float_as_int(s_own), o, acc.get_trace(L)) : make_int4((int)lw, __float_as_int(q_val), st.x, __float_as_int(q_root)),
+                     gp.lane == 7 ? pk : __float_as_int(u.rep_s), gp.lane == 7 ? (uint16_t)pk : (uint16_t)(u.is_first ? o : 0));
+    }
+    for (int L = gp.lane; L < D; L += 8) {
+        int o; float sc;
+        acc.get_trace_meta(L, o, sc);
+        const int4 st = acc.stat(o);
+        acc.pown[L] = make_int4(st.x, st.y, st.z, 0);
+    }
+}
+
+// the walk's z(n) (ztab: the host table below 65536, the device's own evaluation of special.h:26-33 above), for a list of n
+__global__ void k_debug_ztab(Arena A, const int32_t *n, int count, float *out) {
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < count; i += gridDim.x * blockDim.x) out[i] = ztab(A, n[i]);
+}
+
 // get_all_childs (core.h:32-50) on the reference layout: mark[] = 1 for every traversed index (0 included)
 __global__ void k_twin_all_childs(const int32_t *child, int M, int index, uint8_t *mark, int32_t *queue) {
     if (threadIdx.x != 0) return;
