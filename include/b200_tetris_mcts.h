@@ -255,6 +255,14 @@ int b200_debug_net_acts(b200_engine *e, int dist, const int8_t *states, int k, i
 int b200_debug_backup(b200_engine *e, int M, const int32_t *child, const int32_t *n_to_o, const float *score, int32_t *visit, float *value,
                       float *variance, const uint8_t *end, const int32_t *trace, int D, int leaf_kind, const float *eval_out, float rollout_val,
                       int32_t *pc_len, int32_t *pc_own, uint16_t *pc_sib, int32_t *pc_ent, int32_t *pc_var);
+/* test aid: game `game` of an engine of mode lp, single or vanilla set to a tree in the reference's layout (child[M][7], n_to_o / score per
+ * node, visit / value / variance / end per observation), as expansions would have left it: link words by the production finish_expansion,
+ * root, the game's check_low stream (rng_state != 0), status ok, an empty path cache, and the game-over bit set exactly on the nodes without
+ * children, so that b200_run_sims runs the production walk and terminal backup on it.  b200_debug_game_state reads the stream back with the
+ * path cache's valid length (0 with the cache off). */
+int b200_debug_load_tree(b200_engine *e, int game, int M, const int32_t *child, const int32_t *n_to_o, const float *score, const int32_t *visit,
+                         const float *value, const float *variance, const uint8_t *end, int root, uint32_t rng_state);
+int b200_debug_game_state(b200_engine *e, int game, uint32_t *rng_state, int32_t *pc_len);
 int b200_export_dist(b200_engine *e, int game, float *node_stats /* [M][5] */, float *node_dist /* [M][bins] */);
 
 /* --- replay samples of the live search (ValueSim.store_nodes, agents/ValueSim.py:122-159): observations with

@@ -257,6 +257,9 @@ struct mo_agent {
     /* layout of the engine: the entry of level L keeps the children's statistics as of the walk that FILLED it; the statistics of the child
      * the walk picked there (pc_pick) are read from the own-statistics record of level L+1, which the backup rewrites every simulation */
     int pc_pick[512]; int32_t pc_own_visit[512]; float pc_own_value[512], pc_own_variance[512];
+    /* the last selection's phase 1: levels served, and {served levels whose pick changed, stopped at a cached level by check_low, ended on a
+     * cached terminal leaf} */
+    int pc_last_served, pc_last_ev[3];
 };
 
 static uint64_t hash_words(const uint32_t *w, int n) {
@@ -528,14 +531,14 @@ static void pc_fill(mo_agent *a, int L, const int32_t *trace, int D) {
  * follows the cached path up to the first lane that stops.  Returns the number of levels served; *idx_out = the node the walk stands on
  * afterwards (the leaf if *ended), picks[] = the pick (index into the level's child list) of every served level.  Checked against the true
  * walk in pc_on_select: a wrong stop rule shows up as pc_errors. */
-static int pc_emulate_phase1(const mo_agent *a, int root, int *idx_out, int *ended_out, int *picks) {
+static int pc_emulate_phase1(const mo_agent *a, int root, int *idx_out, int *ended_out, int *picks, int *ev) {
     int D = 0, idx = root, fast = a->pc_len > 0, ended = 0;
     const int pcl = a->pc_len;
     while (fast) {
-        int have[8], e_node[8], pick[8], next[8], leaf[8], bail[8], changed[8];
+        int have[8], e_node[8], pick[8], next[8], leaf[8], bail[8], changed[8], lowb[8];
         for (int lane = 0; lane < 8; ++lane) {
             int L = D + lane;
-            have[lane] = L < pcl; e_node[lane] = 0; pick[lane] = 7; next[lane] = 0; leaf[lane] = 0; bail[lane] = 0; changed[lane] = 0;
+            have[lane] = L < pcl; e_node[lane] = 0; pick[lane] = 7; next[lane] = 0; leaf[lane] = 0; bail[lane] = 0; changed[lane] = 0; lowb[lane] = 0;
             if (!have[lane]) continue;
             e_node[lane] = a->pc_node[L];
             int k = a->pc_k[L];
@@ -550,7 +553,7 @@ static int pc_emulate_phase1(const mo_agent *a, int root, int *idx_out, int *end
                 float t = vl + a->score[c];
                 vis[j] = v; val[j] = t - a->score[a->pc_node[L]]; var[j] = vr;
             }
-            if (lowhit) { bail[lane] = 1; continue; }
+            if (lowhit) { bail[lane] = 1; lowb[lane] = 1; continue; }
             int nx = mo_policy_clt(a->pc_cn[L], vis, val, var, k);
             for (int j = 0; j < k; ++j) if (a->pc_cn[L][j] == nx) pick[lane] = j;
             next[lane] = nx;
@@ -564,9 +567,11 @@ static int pc_emulate_phase1(const mo_agent *a, int root, int *idx_out, int *end
         for (int lane = 7; lane >= 0; --lane) if (!have[lane] || bail[lane] || leaf[lane] || changed[lane]) first = lane;
         int first_served = first < 8 && have[first] && !bail[first];
         int served = first + (first_served ? 1 : 0);
-        for (int lane = 0; lane < served; ++lane) picks[D + lane] = leaf[lane] ? -1 : pick[lane];
+        for (int lane = 0; lane < served; ++lane) { picks[D + lane] = leaf[lane] ? -1 : pick[lane]; ev[0] += changed[lane]; }
+        if (first < 8 && lowb[first] && e_node[first] == (first == 0 ? idx : next[first - 1])) ev[1] += 1;
         int last_next = next[served > 0 ? served - 1 : 0];
         ended = first_served && leaf[first];
+        ev[2] |= ended;
         D += served;
         if (ended) idx = e_node[first];
         else if (served > 0) idx = last_next;
@@ -581,7 +586,9 @@ static void pc_on_select(mo_agent *a, const int32_t *trace, int D) {
     if (!a->pc_on) return;
     {   /* the engine's phase 1 must serve a prefix of the TRUE trace, stand on the true next node (or the true leaf), with the true picks */
         int idx = 0, ended = 0, picks[512];
-        int P = pc_emulate_phase1(a, trace[0], &idx, &ended, picks);
+        a->pc_last_ev[0] = a->pc_last_ev[1] = a->pc_last_ev[2] = 0;
+        int P = pc_emulate_phase1(a, trace[0], &idx, &ended, picks, a->pc_last_ev);
+        a->pc_last_served = P;
         int bad = P > D || (ended ? (P != D || idx != trace[D - 1]) : (P < D ? idx != trace[P] : 1));
         if (P == D && !ended) bad = 1;                       /* a walk that serves every level must have ended on a cached leaf */
         for (int L = 0; L < P && L + 1 < D && !bad; ++L) bad = picks[L] < 0 || a->pc_cn[L][picks[L]] != trace[L + 1];
@@ -625,12 +632,21 @@ static void pc_on_select(mo_agent *a, const int32_t *trace, int D) {
 static void pc_on_backup(mo_agent *a, const int32_t *trace, int D, int expanded) {
     if (!a->pc_on || a->pc_len == 0) return;             /* invalidated since the selection (collection / tree drop inside the expansion) */
     int newlen = expanded ? D - 1 : D;                   /* the expanded leaf's entry says "no children": stale */
-    /* Stale copies after this backup, by level: (a) an observation twice on the trace (i < j): the backup runs leaf -> root, so the own record
-     * of the deeper occurrence (read by level j-1) holds an intermediate value; (b) a cached child observation that is some trace node's own
-     * without being that level's picked child.  Everything above the shallowest stale level stays valid: the cache is truncated there. */
+    /* Stale copies after this backup, by level, as k_backup (backup_game) finds them: (a) an observation twice on the trace (i < j): the
+     * backup runs leaf -> root in windows of 32 levels, so the own record of the deeper occurrence (read by level j-1) holds an
+     * intermediate value.  k_backup truncates at the shallower occurrence i when the two lie in different windows, and below the window
+     * (its lowest level - 1) when they share one, whose levels it then folds one by one without writing own records; (b) a cached child
+     * observation that is some trace node's own without being that level's picked child.  Everything above the shallowest stale level stays
+     * valid: the cache is truncated there. */
     int stale = newlen;
     for (int i = 0; i < D; ++i)
-        for (int j = i + 1; j < D; ++j) if (a->n2o[trace[i]] == a->n2o[trace[j]] && j - 1 < stale) stale = j - 1;
+        for (int j = i + 1; j < D; ++j) {
+            if (a->n2o[trace[i]] != a->n2o[trace[j]]) continue;
+            int wi = (D - 1 - i) / 32, wj = (D - 1 - j) / 32;  /* window index counted from the leaf */
+            int bottom = D - 1 - 32 * wi - 31;                 /* the window's lowest level */
+            int s_ij = wi == wj ? (bottom - 1 > 0 ? bottom - 1 : 0) : i;
+            if (s_ij < stale) stale = s_ij;
+        }
     for (int L = 0; L < stale; ++L)
         for (int j = 0; j < a->pc_k[L]; ++j) {
             if (j == a->pc_pick[L]) continue;
@@ -644,6 +660,37 @@ static void pc_on_backup(mo_agent *a, const int32_t *trace, int D, int expanded)
     a->pc_len = newlen;
 }
 void mo_agent_pc_enable(mo_agent *a, int on) { a->pc_on = on; a->pc_len = 0; }
+
+/* The path-cache model over a given sequence of simulations on a fixed tree in the reference's layout (child[M][7], score, n2o): every walk
+ * ends at a terminal leaf, nothing is expanded, the cache starts empty.  Simulation s walks traces[trace_off[s] .. trace_off[s+1]) on the
+ * statistics visit / value / variance[s][M] and its backup leaves [s+1][M].  Per simulation: served[s] = the levels the engine's phase 1
+ * serves, pc_len[s] = the valid length after the backup, ev[s][3] = {served levels whose pick changed, stops at a cached level because of
+ * check_low, the walk ended on a cached terminal leaf}.  Returns the number of stale reads the model found (0 when the rules hold). */
+long mo_pc_replay(int M, const int32_t *child, const float *score, const int32_t *n2o, int low, int S, const int32_t *traces,
+                  const int32_t *trace_off, const int32_t *visit, const float *value, const float *variance, int32_t *served,
+                  int32_t *pc_len, int32_t *ev) {
+    mo_config cfg;
+    memset(&cfg, 0, sizeof(cfg));
+    cfg.max_nodes = M; cfg.low = low;
+    mo_agent *a = mo_agent_create(&cfg, 1, 0, 0);
+    memcpy(a->child, child, (size_t)M * MO_NA * 4); memcpy(a->score, score, (size_t)M * 4); memcpy(a->n2o, n2o, (size_t)M * 4);
+    a->pc_on = 1; a->pc_len = 0;
+    for (int s = 0; s < S; ++s) {
+        const int32_t *tr = traces + trace_off[s];
+        const int D = trace_off[s + 1] - trace_off[s];
+        const size_t b = (size_t)s * M;
+        memcpy(a->ovisit, visit + b, (size_t)M * 4); memcpy(a->ovalue, value + b, (size_t)M * 4); memcpy(a->ovariance, variance + b, (size_t)M * 4);
+        pc_on_select(a, tr, D);
+        served[s] = a->pc_last_served;
+        for (int k = 0; k < 3; ++k) ev[3 * s + k] = a->pc_last_ev[k];
+        memcpy(a->ovisit, visit + b + M, (size_t)M * 4); memcpy(a->ovalue, value + b + M, (size_t)M * 4); memcpy(a->ovariance, variance + b + M, (size_t)M * 4);
+        pc_on_backup(a, tr, D, 0);
+        pc_len[s] = a->pc_len;
+    }
+    long err = a->pc_errors;
+    mo_agent_destroy(a);
+    return err;
+}
 void mo_agent_pc_stats(const mo_agent *a, long *out7) {
     out7[0] = a->pc_errors; out7[1] = a->pc_irregular; out7[2] = a->pc_shared; out7[3] = a->pc_levels; out7[4] = a->pc_sims; out7[5] = a->pc_full_walks; out7[6] = a->pc_len;
 }

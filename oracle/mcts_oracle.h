@@ -84,6 +84,10 @@ int mo_agent_last_trace(const mo_agent *a, int32_t *trace, int max);
 /* CPU model of the engine's path cache (diagnostic): enable, then out7 = {stale entries found (must be 0), invalidations by a transposition
  * inside the path, levels served from the cache, levels walked, simulations, simulations that found no cache, current valid length} */
 void mo_agent_pc_enable(mo_agent *a, int on);
+/* the path-cache model over given walks on a fixed tree of terminal leaves: levels served, valid length and events per simulation */
+long mo_pc_replay(int M, const int32_t *child, const float *score, const int32_t *n2o, int low, int S, const int32_t *traces,
+                  const int32_t *trace_off, const int32_t *visit, const float *value, const float *variance, int32_t *served,
+                  int32_t *pc_len, int32_t *ev);
 void mo_agent_pc_stats(const mo_agent *a, long *out7);
 void mo_agent_export_dist(const mo_agent *a, float *node_stats, float *node_dist);   /* MO_MODE_DIST: f32[M][5], f32[M][bins] */
 void mo_synthetic_dist(const uint32_t *obskey12, int bins, float *dist);             /* test evaluator shared with the device */

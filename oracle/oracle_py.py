@@ -59,6 +59,8 @@ def _sig(L):
     L.mo_norm_quantile.restype = C.c_double
     L.mo_norm_quantile.argtypes = [C.c_double]
     L.mo_norm_quantile_f32.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+    L.mo_pc_replay.restype = C.c_long
+    L.mo_pc_replay.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int] + [C.c_void_p] * 8
     L.mo_agent_create.restype = C.c_void_p
     L.mo_agent_create.argtypes = [C.POINTER(MoConfig), C.c_int, C.c_int, C.c_int]
     L.mo_agent_destroy.argtypes = [C.c_void_p]
@@ -171,6 +173,23 @@ def norm_quantile_f32(n):
     out = np.empty(len(n), np.float32)
     lib().mo_norm_quantile_f32(_p(n), len(n), _p(out))
     return out
+
+
+def pc_replay(child, score, n2o, low, traces, states):
+    """The path-cache model (mcts_oracle.c pc_*) over given walks on a fixed tree whose childless nodes are terminal, from an empty cache:
+    traces[s] is simulation s's walk, states[s] = (visit, value, variance) before it and states[s + 1] after its backup.  Returns
+    (served[S], pc_len[S], events[S, 3], stale reads): the levels the engine's phase 1 serves, the valid length after each backup, and
+    per simulation {served levels whose pick changed, stops at a cached level because of check_low, the walk ended on a cached leaf}."""
+    S, M = len(traces), len(n2o)
+    tr = np.ascontiguousarray(np.concatenate(traces), np.int32)
+    off = np.zeros(S + 1, np.int32)
+    off[1:] = np.cumsum([len(t) for t in traces])
+    vis, val, var = (np.ascontiguousarray(np.stack([st[k] for st in states[:S + 1]]), dt) for k, dt in ((0, np.int32), (1, np.float32), (2, np.float32)))
+    served, pcl, ev = np.zeros(S, np.int32), np.zeros(S, np.int32), np.zeros((S, 3), np.int32)
+    err = lib().mo_pc_replay(M, _p(np.ascontiguousarray(child, np.int32)), _p(np.ascontiguousarray(score, np.float32)),
+                             _p(np.ascontiguousarray(n2o, np.int32)), int(low), S, _p(tr), _p(off), _p(vis), _p(val), _p(var),
+                             _p(served), _p(pcl), _p(ev))
+    return served, pcl, ev, int(err)
 
 
 def select_trace_obs(index, child, visit, value, variance, score, n2o, low, max_trace=512, rng_state=None):

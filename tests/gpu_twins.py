@@ -73,3 +73,18 @@ def ztab(n):
     out = np.empty(len(n), np.float32)
     L.check(L.lib().b200_debug_ztab(L.ptr(n), len(n), L.ptr(out)))
     return out
+
+
+def debug_load_tree(eng, game, c):
+    """Game `game` of engine `eng` set to the tree of case c (tests/select_edges.py layout) through b200_debug_load_tree: root c["root"],
+    check_low stream c["seed"], every childless node terminal."""
+    L.check(L.lib().b200_debug_load_tree(eng.h, int(game), len(c["n2o"]), L.ptr(c["child"]), L.ptr(c["n2o"]), L.ptr(c["score"]),
+                                         L.ptr(c["visit"]), L.ptr(c["value"]), L.ptr(c["variance"]), L.ptr(c["end"]), int(c["root"]),
+                                         int(c["seed"])))
+
+
+def debug_game_state(eng, game):
+    """(check_low stream state, path cache valid length) of one game."""
+    rng, pcl = np.zeros(1, np.uint32), np.zeros(1, np.int32)
+    L.check(L.lib().b200_debug_game_state(eng.h, int(game), L.ptr(rng), L.ptr(pcl)))
+    return int(rng[0]), int(pcl[0])

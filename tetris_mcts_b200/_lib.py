@@ -98,6 +98,8 @@ def lib():
         L.b200_debug_net_acts.argtypes = [P, C.c_int, P, C.c_int, C.c_int, P]
         L.b200_debug_backup.argtypes = [P, C.c_int] + [P] * 8 + [C.c_int, C.c_int, P, C.c_float] + [P] * 5
         L.b200_debug_ztab.argtypes = [P, C.c_int, P]
+        L.b200_debug_load_tree.argtypes = [P, C.c_int, C.c_int] + [P] * 7 + [C.c_int, C.c_uint32]
+        L.b200_debug_game_state.argtypes = [P, C.c_int, P, P]
         L.b200_export_dist.argtypes = [P, C.c_int, P, P]
         L.b200_dist_shift_distribution.argtypes = [P, C.c_int, C.c_double, C.c_double, C.c_double, P]
         L.b200_dist_mean_variance.argtypes = [P, C.c_int, C.c_double, C.c_double, P, P]

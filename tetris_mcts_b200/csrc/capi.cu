@@ -1373,6 +1373,84 @@ extern "C" int b200_tetris_state(const uint32_t *recs, int8_t *out, int n) {
     return env_stream_op(const_cast<uint32_t *>(recs), nullptr, out, n);
 }
 
+// test aids on trees given in the reference's layout (agents/agent.py:58-88): every child id and observation id within [0, M)
+static bool ref_tree_in_range(int M, const int32_t *child, const int32_t *n_to_o) {
+    for (int i = 0; i < M; ++i)
+        if (n_to_o[i] < 0 || n_to_o[i] >= M) return false;
+    for (int i = 0; i < M * 7; ++i)
+        if (child[i] < 0 || child[i] >= M) return false;
+    return true;
+}
+
+// the rows (c / o / s from child, n_to_o, score; the link words are left to finish_expansion, k_debug_link_rows) and the statistics
+// (visit / value / variance / end per observation) of such a tree, as the engine holds them
+static void ref_tree_rows(int M, const int32_t *child, const int32_t *n_to_o, const float *score, const int32_t *visit, const float *value,
+                          const float *variance, const uint8_t *end, std::vector<int32_t> &row, std::vector<int4> &st) {
+    row.assign((size_t)M * ROW_WORDS, 0);
+    st.resize(M);
+    for (int i = 0; i < M; ++i) {
+        int32_t *r = &row[(size_t)i * ROW_WORDS];
+        for (int a = 0; a < 7; ++a) { const int c = child[(size_t)i * 7 + a]; r[a] = c; r[8 + a] = n_to_o[c]; memcpy(&r[16 + a], &score[c], 4); }
+        r[15] = n_to_o[i]; memcpy(&r[23], &score[i], 4);
+        int4 s; s.x = visit[i]; memcpy(&s.y, &value[i], 4); memcpy(&s.z, &variance[i], 4); s.w = end[i] != 0;
+        st[i] = s;
+    }
+}
+
+// test aid: game `game` of an engine (mode lp, single or vanilla) as expansions would have left the tree given in the reference's layout:
+// the rows with the link words of the production finish_expansion, the statistics, the root, the game's check_low stream srng = rng_state
+// (non-zero), status ST_OK, an empty path cache, and node records whose game-over bit is set exactly on the nodes without children.  Every
+// walk of b200_run_sims then ends at a terminal leaf: the production walk (k_select_expand) and the terminal backup (k_backup) run on the
+// given statistics with no expansion, evaluation or collection.  Nodes >= M of the game keep what they held (no walk reaches them).
+extern "C" int b200_debug_load_tree(b200_engine *e, int game, int M, const int32_t *child, const int32_t *n_to_o, const float *score,
+                                    const int32_t *visit, const float *value, const float *variance, const uint8_t *end, int root,
+                                    uint32_t rng_state) {
+    if (!e || !child || !n_to_o || !score || !visit || !value || !variance || !end) return fail(B200_ERR_BAD_ARG, "bad argument");
+    REFUSE_IF_OPEN(e, "b200_debug_load_tree");
+    Arena &A = e->A;
+    if (A.mode != MODE_LP && A.mode != MODE_SINGLE && A.mode != MODE_VANILLA) return fail(B200_ERR_BAD_ARG, "b200_debug_load_tree needs an engine of mode lp, single or vanilla");
+    if (game < 0 || game >= A.G || M < 2 || M > A.M || root < 1 || root >= M || rng_state == 0u)
+        return fail(B200_ERR_BAD_ARG, "need 0 <= game < n_games, 2 <= M <= max_nodes, 1 <= root < M and rng_state != 0");
+    if (!ref_tree_in_range(M, child, n_to_o)) return fail(B200_ERR_BAD_ARG, "child or n_to_o out of range");
+    CK(cudaSetDevice(e->cfg.device));
+    CK(cudaStreamSynchronize(e->stream));
+    std::vector<int32_t> row;
+    std::vector<int4> st;
+    ref_tree_rows(M, child, n_to_o, score, visit, value, variance, end, row, st);
+    std::vector<uint32_t> rec((size_t)M * REC_WORDS, 0u);
+    for (int i = 0; i < M; ++i) {
+        bool leaf = true;
+        for (int a = 0; a < 7; ++a) leaf = leaf && child[(size_t)i * 7 + a] == 0;
+        rec[(size_t)i * REC_WORDS + 10] = leaf ? 1u << 21 : 0u;        // the game-over bit k_select_expand reads from the leaf's record
+    }
+    const int32_t zero = 0, st_ok = ST_OK;
+    CK(cudaMemcpyAsync(A.row + (size_t)game * A.M * ROW_WORDS, row.data(), row.size() * 4, cudaMemcpyHostToDevice, e->stream));
+    CK(cudaMemcpyAsync(A.stat + (size_t)game * A.M, st.data(), (size_t)M * sizeof(int4), cudaMemcpyHostToDevice, e->stream));
+    CK(cudaMemcpyAsync(A.rec + (size_t)game * A.M * REC_WORDS, rec.data(), rec.size() * 4, cudaMemcpyHostToDevice, e->stream));
+    CK(cudaMemcpyAsync(A.root + game, &root, 4, cudaMemcpyHostToDevice, e->stream));
+    CK(cudaMemcpyAsync(A.srng + game, &rng_state, 4, cudaMemcpyHostToDevice, e->stream));
+    CK(cudaMemcpyAsync(A.status + game, &st_ok, 4, cudaMemcpyHostToDevice, e->stream));
+    CK(cudaMemcpyAsync(A.pending + game, &zero, 4, cudaMemcpyHostToDevice, e->stream));
+    CK(cudaMemcpyAsync(A.trace_len + game, &zero, 4, cudaMemcpyHostToDevice, e->stream));
+    if (A.pc) CK(cudaMemcpyAsync(A.pc_len + game, &zero, 4, cudaMemcpyHostToDevice, e->stream));
+    k_debug_link_rows<<<(M + 15) / 16, 128, 0, e->stream>>>(A, game, M);
+    CK(cudaGetLastError());
+    CK(cudaStreamSynchronize(e->stream));
+    return B200_OK;
+}
+
+// test aid: a game's check_low stream state and its path cache's valid length (0 with the cache off)
+extern "C" int b200_debug_game_state(b200_engine *e, int game, uint32_t *rng_state, int32_t *pc_len) {
+    if (!e || !rng_state || !pc_len || game < 0 || game >= e->A.G) return fail(B200_ERR_BAD_ARG, "bad argument");
+    REFUSE_IF_OPEN(e, "b200_debug_game_state");
+    CK(cudaSetDevice(e->cfg.device));
+    *pc_len = 0;
+    CK(cudaMemcpyAsync(rng_state, e->A.srng + game, 4, cudaMemcpyDeviceToHost, e->stream));
+    if (e->A.pc) CK(cudaMemcpyAsync(pc_len, e->A.pc_len + game, 4, cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaStreamSynchronize(e->stream));
+    return B200_OK;
+}
+
 // development / test aid: the production k_backup (through step_backup, the launch run_sims uses) on a tree given in the reference's layout
 // (agents/agent.py:58-88), on game 0 of a one-game engine.  The game's row (c / o / s from child, n_to_o, score; the link words by
 // finish_expansion), stat (visit / value / variance / end per observation), trace, trace_meta (own observation | pick << 28, own score; the
@@ -1394,23 +1472,14 @@ extern "C" int b200_debug_backup(b200_engine *e, int M, const int32_t *child, co
     if (!A.pc != !pc_len || (pc_len && (!pc_own || !pc_sib || !pc_ent || !pc_var)))
         return fail(B200_ERR_BAD_ARG, "pc_len and the entry buffers are given exactly when the path cache is on");
     if (pc_len && (*pc_len < 0 || *pc_len > (leaf_kind == LEAF_EXPANDED ? D - 1 : D))) return fail(B200_ERR_BAD_ARG, "pc_len beyond what a walk leaves valid");
-    for (int i = 0; i < M; ++i)
-        if (n_to_o[i] < 0 || n_to_o[i] >= M) return fail(B200_ERR_BAD_ARG, "n_to_o out of range");
-    for (int i = 0; i < M * 7; ++i)
-        if (child[i] < 0 || child[i] >= M) return fail(B200_ERR_BAD_ARG, "child out of range");
+    if (!ref_tree_in_range(M, child, n_to_o)) return fail(B200_ERR_BAD_ARG, "child or n_to_o out of range");
     for (int d = 0; d < D; ++d)
         if (trace[d] < 1 || trace[d] >= M) return fail(B200_ERR_BAD_ARG, "trace entry out of range");
     CK(cudaSetDevice(e->cfg.device));
     CK(cudaStreamSynchronize(e->stream));
-    std::vector<int32_t> row((size_t)M * ROW_WORDS, 0);
-    std::vector<int4> st(M);
-    for (int i = 0; i < M; ++i) {
-        int32_t *r = &row[(size_t)i * ROW_WORDS];
-        for (int a = 0; a < 7; ++a) { const int c = child[(size_t)i * 7 + a]; r[a] = c; r[8 + a] = n_to_o[c]; memcpy(&r[16 + a], &score[c], 4); }
-        r[15] = n_to_o[i]; memcpy(&r[23], &score[i], 4);
-        int4 s; s.x = visit[i]; memcpy(&s.y, &value[i], 4); memcpy(&s.z, &variance[i], 4); s.w = end[i] != 0;
-        st[i] = s;
-    }
+    std::vector<int32_t> row;
+    std::vector<int4> st;
+    ref_tree_rows(M, child, n_to_o, score, visit, value, variance, end, row, st);
     std::vector<int2> meta(D);
     for (int d = 0; d < D; ++d) {
         const int32_t *r = &row[(size_t)trace[d] * ROW_WORDS];

@@ -820,6 +820,11 @@ __global__ void __launch_bounds__(128) k_dist_backup(Arena A) {
 }
 
 // ---------------------------------------------------------------- compute_stats / get_action (agent.py:153-185)
+// np.argmax (agent.py:185) over values seen in order: the first NaN if there is one (a NaN compares as the largest value), otherwise the
+// first maximum.  `best` is the value held so far; once it is a NaN nothing replaces it.
+__device__ __forceinline__ bool argmax_takes(int a, float val, float best) {
+    return a == 0 || (best == best && (val != val || val > best));
+}
 __global__ void k_root_stats(Arena A, float *stats, int32_t *action) {
     int g = blockIdx.x * blockDim.x + threadIdx.x;
     if (g >= A.G) return;
@@ -836,7 +841,7 @@ __global__ void k_root_stats(Arena A, float *stats, int32_t *action) {
             const float *ns = nsb + (size_t)c * NSTAT_WORDS;
             float val = __fsub_rn(__fadd_rn(ns[1], ns[2]), rr);
             stats[(size_t)g * 21 + a] = ns[0]; stats[(size_t)g * 21 + 7 + a] = val; stats[(size_t)g * 21 + 14 + a] = ns[3];
-            if (a == 0 || val > best) { best = val; arg = a; }
+            if (argmax_takes(a, val, best)) { best = val; arg = a; }
         }
         action[g] = arg;
         return;
@@ -850,7 +855,7 @@ __global__ void k_root_stats(Arena A, float *stats, int32_t *action) {
         stats[(size_t)g * 21 + a] = (float)st.x;
         stats[(size_t)g * 21 + 7 + a] = val;
         stats[(size_t)g * 21 + 14 + a] = __int_as_float(st.z);
-        if (a == 0 || val > best) { best = val; arg = a; }      // np.argmax: first maximum
+        if (argmax_takes(a, val, best)) { best = val; arg = a; }
     }
     action[g] = arg;
 }

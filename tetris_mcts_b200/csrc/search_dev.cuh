@@ -256,7 +256,8 @@ __device__ __forceinline__ uint2 touch64(const void *p) {
 //   * k_backup rewrites pc_own of every trace level (one coalesced 16-byte store per level);
 //   * when a cached level picks another child than last time, the old pick's latest statistics go back into the entry first;
 //   * any other copy — the same observation under another node of the path (transposition), or twice on the trace — goes stale:
-//     k_backup finds those with a bitmap of the trace's own observations and truncates pc_len at the shallowest stale level;
+//     k_backup finds those with a bitmap of the trace's own observations and truncates pc_len at the shallowest stale level (for an
+//     observation twice on the trace: the shallower occurrence, or below the 32-level window when both lie in one);
 //   * the entry of a leaf that gets expanded says "no children": the walk leaves pc_len = D - 1;
 //   * k_update_root, k_gc (collections and dropped trees) and reset_tree set pc_len = 0.
 // The CPU model applies exactly these rules and checks every value a cached level would read against the arena at every selection
@@ -438,7 +439,7 @@ __device__ __forceinline__ int select_trace(const Acc &acc, bool active, int roo
     bool walking = active;
     // core.h:65-105 for one level, from the values every lane holds for its child slot (`on`: this lane's group is at a node WITH children):
     // check_low, then policy_clt.  Shared by the cached and the uncached form of a level, so both pick bit for bit the same child.
-    auto choose = [&](bool on, const Uniq &u, const int4 &st, float s_idx, float &val_out, float &root_out) -> int {
+    auto choose = [&](bool on, const Uniq &u, const int4 &st, int o, float s_idx, float &val_out, float &root_out) -> int {
         const unsigned lowmask = gp.ballot(on && u.is_first && st.x < low);   // core.h:65-77
         int pick = 0;
         if (__any_sync(0xffffffffu, lowmask != 0u)) {                   // warp-uniform branch: the draw of every group that needs one
@@ -470,7 +471,11 @@ __device__ __forceinline__ int select_trace(const Acc &acc, bool active, int roo
         }
         const int first = __ffs(u.first_mask) - 1;
         const unsigned nanmask = gp.ballot(cmp && q != q);
-        if (lowmask == 0u) pick = (first >= 0 && ((nanmask >> first) & 1u)) ? first : ql;
+        bool drawn = lowmask != 0u;
+        // core.h:202-205: a drawn observation 0 falls through to policy_clt.  Only the reference's layout can list observation 0 as a child
+        // (the engine's arena never allocates it), so the engine's walk is compiled without the test.
+        if constexpr (!Acc::has_pc) drawn = gp.bcast(o, pick) != 0 && drawn;
+        if (!drawn) pick = (first >= 0 && ((nanmask >> first) & 1u)) ? first : ql;
         return pick;
     };
     if constexpr (Acc::has_pc) {
@@ -537,7 +542,7 @@ __device__ __forceinline__ int select_trace(const Acc &acc, bool active, int roo
         int4 st = make_int4(0, 0, 0, 0);
         if (walking && u.is_first) st = acc.stat(o, D);                 // the children live one level below
         float q_val, q_root;
-        const int pick = choose(walking, u, st, s_idx, q_val, q_root);
+        const int pick = choose(walking, u, st, o, s_idx, q_val, q_root);
         const int next = gp.bcast(u.rep_c, pick);
         if (at_level && gp.lane == 7) acc.put_trace_meta(D - 1, o | (walking ? pick << 28 : 0), s_idx);   // lane 7 holds the node's own observation and score
         if constexpr (Acc::has_pc) {
