@@ -104,6 +104,25 @@ int b200_engine_get_stream(b200_engine *e, void **cuda_stream_out);
  *     b200_load_dist_weights (B200_EVAL_NET_TC, B200_EVAL_DIST_FP16). */
 int b200_load_weights(b200_engine *e, const float *weights);
 
+/* --- snapshot (no reference counterpart: the reference checkpoints the model only).  b200_engine_save writes everything a later call can
+ *     read to `path`: every b200_config field, the path-cache / deep-lane / gc_headroom settings, the weights as b200_load_weights /
+ *     b200_load_dist_weights took them, the counters and the finished-games log, the replay memory with its policy (the std::mt19937 and
+ *     the trimming sampler included), and each game's arena packed on the device to its live slots, free lists, records, table entries and
+ *     last trace, with a 64-bit checksum per game (DESIGN §4c).  The image streams through a bounded staging buffer: two halves of
+ *     max(b200_snapshot_set_staging / 2, the largest packed game) bytes in device memory and the same again in pinned host memory, so
+ *     64 MB of each (128 MB in all) by default.  It is
+ *     written to path + ".tmp", flushed, synced and renamed: an interrupted save leaves a previous image at `path` intact.  *bytes_out
+ *     (may be NULL) = the file's size.  A step open between b200_ext_step_begin and _end returns B200_ERR_BAD_ARG.
+ *   b200_engine_load creates an engine from such an image (device -1: the saved ordinal) that continues bit for bit as the saved one
+ *     would have: the same actions, statistics, arenas, counters, memory and policy draws.  The path cache restarts empty (it changes no
+ *     result).  A truncated or corrupted file, a wrong magic or format version, or an unknown field returns B200_ERR_BAD_ARG with the
+ *     reason in b200_last_error and leaves nothing allocated.  The checksums detect corruption; an image is not authenticated.
+ *   b200_snapshot_timing: seconds of this thread's last save {device pack, D2H, write} and load {read, H2D, device unpack}. */
+int b200_engine_save(b200_engine *e, const char *path, int64_t *bytes_out);
+int b200_engine_load(const char *path, int device, b200_engine **out);
+int b200_snapshot_set_staging(int64_t bytes);   /* process-wide; <= 0: the default */
+int b200_snapshot_timing(double *sec6);
+
 /* --- TreeAgent.update_root (agents/agent.py:296-301) for all games: recs[n_games][20] */
 int b200_set_games(b200_engine *e, const uint32_t *recs);
 int b200_get_games(b200_engine *e, uint32_t *recs);

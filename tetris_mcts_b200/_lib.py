@@ -108,6 +108,10 @@ def lib():
         L.b200_ext_capacity.argtypes = [P, P, P]
         L.b200_ext_step_begin.argtypes = [P, P, C.c_int, P, P]
         L.b200_ext_step_end.argtypes = [P, P]
+        L.b200_engine_save.argtypes = [P, C.c_char_p, P]
+        L.b200_engine_load.argtypes = [C.c_char_p, C.c_int, C.POINTER(P)]
+        L.b200_snapshot_set_staging.argtypes = [C.c_int64]
+        L.b200_snapshot_timing.argtypes = [P]
         _lib = L
     return _lib
 

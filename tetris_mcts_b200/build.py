@@ -7,7 +7,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libb200_tetris_mcts.so")
 SOURCES = ["capi.cu", "trainer.cu"]
-HEADERS = ["gmma.cuh", "tetris_dev.cuh", "search_dev.cuh", "kernels.cuh", "valuenet_simt.cuh", "valuenet_tc.cuh", "dist_dev.cuh", "distnet_simt.cuh", "distnet_tc.cuh", "ext_eval.cuh"]
+HEADERS = ["gmma.cuh", "tetris_dev.cuh", "search_dev.cuh", "kernels.cuh", "valuenet_simt.cuh", "valuenet_tc.cuh", "dist_dev.cuh", "distnet_simt.cuh", "distnet_tc.cuh", "ext_eval.cuh", "snapshot.cuh"]
 FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-Xcompiler", "-fPIC", "-shared"]
 
 

@@ -2,11 +2,17 @@
 // One engine = one CUDA stream + the per-game arenas in HBM.  No CPU compute path exists in this file: every
 // entry point either launches kernels or moves bytes.
 #include <cuda_runtime.h>
+#include <unistd.h>
+#include <array>
+#include <cerrno>
+#include <chrono>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <functional>
+#include <map>
+#include <sstream>
 #include <string>
 #include <vector>
 
@@ -19,6 +25,7 @@
 #include "valuenet_tc.cuh"
 #include "distnet_tc.cuh"
 #include "ext_eval.cuh"
+#include "snapshot.cuh"
 
 using namespace b200;
 
@@ -55,6 +62,8 @@ struct b200_engine {
     float *d_act3 = nullptr; size_t act3_rows = 0;
     void *tc_state = nullptr; void *dn_tc_state = nullptr;
     bool have_dist_weights = false; float *d_dnw = nullptr; DistNetWeights DW{}; float *d_dn_act = nullptr; size_t dn_rows = 0;
+    std::vector<float> h_w, h_dnw;   // the weights as the caller passed them (state_dict order): what b200_engine_save writes
+    int dn_atoms = 0;
     int n_sm = 132;
     // timing
     bool timing = false;
@@ -381,6 +390,7 @@ extern "C" int b200_load_weights(b200_engine *e, const float *w) {
         if (rc) return fail(B200_ERR_CUDA, "tensor-core weight preparation failed");
     }
     e->have_weights = true;
+    e->h_w.assign(w, w + B200_N_WEIGHTS);
     drop_step_graph(e);
     return B200_OK;
 }
@@ -449,6 +459,8 @@ __global__ void k_states_to_keys(const int8_t *states, int k, uint32_t *keys, ui
 
 // net_tc and dist_fp16 run the same tensor-core distributional kernels and weight layout, with two fp16 terms per operand or one (distnet_tc.cuh)
 static bool dn_tc_net(const b200_engine *e) { return e->cfg.eval_kind == B200_EVAL_NET_TC || e->cfg.eval_kind == B200_EVAL_DIST_FP16; }
+// floats of model_distributional.py's state_dict vector: conv1, conv2, fc1, fc_v (weights and biases)
+static size_t dn_weight_count(int atoms) { return (size_t)512 + 32 + 16384 + 32 + 128 * 2048 + 128 + (size_t)atoms * 128 + atoms; }
 
 extern "C" int b200_load_dist_weights(b200_engine *e, const float *w, int atoms) {
     if (!e || !w || atoms < 2 || atoms > 64) return fail(B200_ERR_BAD_ARG, "bad argument");
@@ -474,6 +486,7 @@ extern "C" int b200_load_dist_weights(b200_engine *e, const float *w, int atoms)
     CK(cudaFuncSetAttribute(k_dn_fc_dbg, cudaFuncAttributeMaxDynamicSharedMemorySize, DN_FC_SMEM));
     if (dn_tc_prepare(&e->dn_tc_state, w, atoms, e->stream)) return fail(B200_ERR_CUDA, "tensor-core weight preparation (distributional network) failed");
     e->have_dist_weights = true;
+    e->h_dnw.assign(w, w + dn_weight_count(atoms)); e->dn_atoms = atoms;   // the state_dict vector dn_relayout reads
     drop_step_graph(e);
     return B200_OK;
 }
@@ -2005,5 +2018,457 @@ extern "C" int b200_replay_peek_dev(b200_engine *e, void *out_dev, int n) {
     CK(cudaSetDevice(e->cfg.device));
     if (n > 0) CK(cudaMemcpyAsync(out_dev, e->A.replay, (size_t)n * 212, cudaMemcpyDeviceToDevice, e->stream));
     CK(cudaStreamSynchronize(e->stream));
+    return B200_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------- snapshot (b200_engine_save / _load)
+// File: "B200SNAP", u32 version, u32 byte-order mark, then fields {u32 id, u32 0, u64 nbytes, payload, u64 checksum(payload)}; the arena field
+// comes last but one and carries its own layout (u64 n_games, u64 words[n_games], u64 checksum(words), the packed games of snapshot.cuh,
+// each with its device checksum); a field of id 0 ends the file.  Scalars are 8-byte payloads (int64, or the bits of a double).
+namespace {
+
+constexpr char SNAP_MAGIC[8] = {'B', '2', '0', '0', 'S', 'N', 'A', 'P'};
+constexpr uint32_t SNAP_VERSION = 1, SNAP_BOM = 0x01020304u;
+enum : uint32_t {
+    F_END = 0,
+    // b200_config, one field each
+    F_N_GAMES = 1, F_MAX_NODES, F_MODE, F_LOW, F_LP_END_FROM_OBS, F_LP_VAR_GAMMA2, F_STALE_POP, F_OVERFLOW_RESET, F_EVAL_KIND, F_TRACE_MAX,
+    F_ACTIONS_PER_DROP, F_SCORING, F_RANDOMIZER, F_DEVICE, F_SEED, F_GAMMA, F_ROLLOUT_VARIANCE, F_DIST_BINS, F_DIST_VMIN, F_DIST_VMAX,
+    // engine settings that change results or run shape
+    F_PATH_CACHE = 32, F_DEEP_CAP, F_GC_HEADROOM,
+    // networks, as b200_load_weights / b200_load_dist_weights took them
+    F_WEIGHTS = 40, F_DIST_ATOMS, F_DIST_WEIGHTS,
+    F_COUNTERS = 48, F_FIN_COUNT, F_FIN_LOG,
+    // replay memory and its policy (ReplayPolicy)
+    F_REPLAY_MIN_VISITS = 56, F_REPLAY_CAPACITY, F_REPLAY_CAP, F_REPLAY_COUNT, F_REPLAY_ROWS,
+    F_RP_POLICY = 64, F_RP_MEMORY_SIZE, F_RP_EPISODES_PER_TRAIN, F_RP_GROWTH, F_RP_MEMORY_INDEX, F_RP_ACCUMULATED, F_RP_LAST_ACCUMULATION,
+    F_RP_LAST_TRAINING, F_RP_N_TRAINS, F_RP_DROP_PROB, F_RP_NODES_PER_EPISODE, F_RP_MT, F_RP_SAMPLER,
+    F_ARENA = 128,
+};
+static bool snap_known(uint32_t id) {
+    return (id >= F_N_GAMES && id <= F_DIST_VMAX) || (id >= F_PATH_CACHE && id <= F_GC_HEADROOM) || (id >= F_WEIGHTS && id <= F_DIST_WEIGHTS) ||
+           (id >= F_COUNTERS && id <= F_FIN_LOG) || (id >= F_REPLAY_MIN_VISITS && id <= F_REPLAY_ROWS) || (id >= F_RP_POLICY && id <= F_RP_SAMPLER);
+}
+
+int64_t g_snap_staging = 64ll << 20;   // b200_snapshot_set_staging
+thread_local double g_snap_sec[6];      // pack, D2H, write | read, H2D, unpack of this thread's last save | load
+
+uint64_t host_checksum(const void *p, size_t n, uint64_t h = 0xcbf29ce484222325ull) {   // FNV-1a over 8-byte words, then the tail bytes
+    const uint8_t *b = (const uint8_t *)p;
+    size_t i = 0;
+    for (; i + 8 <= n; i += 8) { uint64_t w; memcpy(&w, b + i, 8); h = (h ^ w) * 0x100000001b3ull; }
+    for (; i < n; ++i) h = (h ^ b[i]) * 0x100000001b3ull;
+    return h;
+}
+double now_s() { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
+
+struct Pinned {   // the two host halves of the staging buffer
+    void *p = nullptr;
+    ~Pinned() { if (p) cudaFreeHost(p); }
+};
+struct Events {
+    std::vector<cudaEvent_t> ev;
+    ~Events() { for (auto x : ev) cudaEventDestroy(x); }
+    cudaEvent_t make() { cudaEvent_t x = nullptr; cudaEventCreate(&x); ev.push_back(x); return x; }
+};
+
+struct Writer {
+    FILE *f = nullptr;
+    bool ok = true;
+    void raw(const void *p, size_t n) { if (ok && n && fwrite(p, 1, n, f) != n) ok = false; }
+    void field(uint32_t id, const void *p, uint64_t n) {
+        const uint32_t hdr[2] = {id, 0u};
+        raw(hdr, 8); raw(&n, 8); raw(p, n);
+        const uint64_t cs = host_checksum(p, n);
+        raw(&cs, 8);
+    }
+    void i64(uint32_t id, int64_t v) { field(id, &v, 8); }
+    void f64(uint32_t id, double v) { field(id, &v, 8); }
+};
+
+struct Reader {
+    FILE *f = nullptr;
+    uint64_t left = 0;                   // bytes of the file not read yet
+    bool raw(void *p, uint64_t n) { if (n > left || fread(p, 1, n, f) != n) return false; left -= n; return true; }
+};
+
+// the staging halves: each holds the largest game; chunks of whole games of at most `half` bytes
+static size_t snap_half(const std::vector<long long> &words) {
+    long long most = 0;
+    for (long long w : words) most = std::max(most, w);
+    return std::max<size_t>((size_t)(g_snap_staging / 2), (size_t)most * 4);
+}
+
+}  // namespace
+
+extern "C" int b200_snapshot_set_staging(int64_t bytes) {
+    g_snap_staging = bytes > 0 ? bytes : (64ll << 20);
+    return B200_OK;
+}
+
+extern "C" int b200_snapshot_timing(double *sec6) {
+    if (!sec6) return fail(B200_ERR_BAD_ARG, "null argument");
+    memcpy(sec6, g_snap_sec, sizeof(g_snap_sec));
+    return B200_OK;
+}
+
+extern "C" int b200_engine_save(b200_engine *e, const char *path, int64_t *bytes_out) {
+    if (!e || !path) return fail(B200_ERR_BAD_ARG, "null argument");
+    REFUSE_IF_OPEN(e, "b200_engine_save");
+    CK(cudaSetDevice(e->cfg.device));
+    CK(cudaStreamSynchronize(e->stream));
+    if (e->stream1) CK(cudaStreamSynchronize(e->stream1));
+    for (double &s : g_snap_sec) s = 0.0;
+    const Arena &A = e->A;
+    const int G = A.G;
+    // sizes of the packed games
+    Scratch tmp;
+    long long *d_words = nullptr, *d_off = nullptr; int32_t *d_ent = nullptr;
+    CK(tmp.get(&d_words, (size_t)G * 8)); CK(tmp.get(&d_ent, (size_t)G * 8)); CK(tmp.get(&d_off, (size_t)(G + 1) * 8));
+    k_snap_count<<<G, 256, 0, e->stream>>>(A, d_words, d_ent);
+    CK(cudaGetLastError());
+    std::vector<long long> words(G), off(G + 1, 0);
+    CK(cudaMemcpyAsync(words.data(), d_words, (size_t)G * 8, cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaStreamSynchronize(e->stream));
+    for (int g = 0; g < G; ++g) off[g + 1] = off[g] + words[g];
+    CK(cudaMemcpyAsync(d_off, off.data(), (size_t)(G + 1) * 8, cudaMemcpyHostToDevice, e->stream));
+    // the host-side state
+    std::vector<uint64_t> counters(48);
+    int32_t fin_count = 0, replay_count = 0;
+    CK(cudaMemcpyAsync(counters.data(), A.counters, 48 * 8, cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaMemcpyAsync(&fin_count, A.fin_count, 4, cudaMemcpyDeviceToHost, e->stream));
+    if (A.replay) CK(cudaMemcpyAsync(&replay_count, A.replay_count, 4, cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaStreamSynchronize(e->stream));
+    std::vector<int32_t> fin((size_t)std::min(fin_count, A.fin_cap) * 4);
+    if (!fin.empty()) CK(cudaMemcpy(fin.data(), A.fin_log, fin.size() * 4, cudaMemcpyDeviceToHost));
+    std::vector<uint8_t> rows;
+    if (A.replay) {
+        rows.resize((size_t)std::max(0, std::min(replay_count, e->replay_alloc)) * 212);
+        if (!rows.empty()) CK(cudaMemcpy(rows.data(), A.replay, rows.size(), cudaMemcpyDeviceToHost));
+    }
+    // staging: two device halves and two pinned halves, packed / copied / written in turn
+    const size_t half = snap_half(words);
+    uint8_t *d_stage = nullptr;
+    CK(tmp.get(&d_stage, 2 * half));
+    Pinned pin;
+    CK(cudaHostAlloc(&pin.p, 2 * half, cudaHostAllocDefault));
+    const std::string tmp_path = std::string(path) + ".tmp";
+    Writer W;
+    W.f = fopen(tmp_path.c_str(), "wb");
+    if (!W.f) return fail(B200_ERR_BAD_ARG, "b200_engine_save: cannot open " + tmp_path + " for writing: " + strerror(errno));
+    struct Closer { Writer &w; std::string p; bool keep = false; ~Closer() { if (w.f) fclose(w.f); if (!keep) remove(p.c_str()); } } closer{W, tmp_path};
+    W.raw(SNAP_MAGIC, 8); W.raw(&SNAP_VERSION, 4); W.raw(&SNAP_BOM, 4);
+    const b200_config &c = e->cfg;
+    W.i64(F_N_GAMES, c.n_games); W.i64(F_MAX_NODES, c.max_nodes); W.i64(F_MODE, c.mode); W.i64(F_LOW, c.low);
+    W.i64(F_LP_END_FROM_OBS, c.lp_end_from_obs); W.i64(F_LP_VAR_GAMMA2, c.lp_var_gamma2); W.i64(F_STALE_POP, c.stale_pop);
+    W.i64(F_OVERFLOW_RESET, c.overflow_reset); W.i64(F_EVAL_KIND, c.eval_kind); W.i64(F_TRACE_MAX, c.trace_max);
+    W.i64(F_ACTIONS_PER_DROP, c.actions_per_drop); W.i64(F_SCORING, c.scoring); W.i64(F_RANDOMIZER, c.randomizer); W.i64(F_DEVICE, c.device);
+    W.i64(F_SEED, c.seed); W.f64(F_GAMMA, c.gamma); W.f64(F_ROLLOUT_VARIANCE, c.rollout_variance); W.i64(F_DIST_BINS, c.dist_bins);
+    W.f64(F_DIST_VMIN, c.dist_vmin); W.f64(F_DIST_VMAX, c.dist_vmax);
+    W.i64(F_PATH_CACHE, A.pc != nullptr); W.i64(F_DEEP_CAP, e->deep_cap); W.i64(F_GC_HEADROOM, e->gc_headroom);
+    if (e->have_weights) W.field(F_WEIGHTS, e->h_w.data(), e->h_w.size() * 4);
+    if (e->have_dist_weights) { W.i64(F_DIST_ATOMS, e->dn_atoms); W.field(F_DIST_WEIGHTS, e->h_dnw.data(), e->h_dnw.size() * 4); }
+    W.field(F_COUNTERS, counters.data(), counters.size() * 8);
+    W.i64(F_FIN_COUNT, fin_count);
+    W.field(F_FIN_LOG, fin.data(), fin.size() * 4);
+    if (A.replay) {
+        W.i64(F_REPLAY_MIN_VISITS, A.replay_min_visits); W.i64(F_REPLAY_CAPACITY, e->replay_alloc / 2); W.i64(F_REPLAY_CAP, A.replay_cap);
+        W.i64(F_REPLAY_COUNT, replay_count); W.field(F_REPLAY_ROWS, rows.data(), rows.size());
+    }
+    if (e->rp.policy >= 0) {
+        const ReplayPolicy &P = e->rp;
+        W.i64(F_RP_POLICY, P.policy); W.i64(F_RP_MEMORY_SIZE, P.memory_size); W.i64(F_RP_EPISODES_PER_TRAIN, P.episodes_per_train);
+        W.i64(F_RP_GROWTH, P.memory_growth_rate); W.i64(F_RP_MEMORY_INDEX, P.memory_index); W.i64(F_RP_ACCUMULATED, P.accumulated_nodes);
+        W.i64(F_RP_LAST_ACCUMULATION, P.last_accumulation_episode); W.i64(F_RP_LAST_TRAINING, P.last_training_episode);
+        W.i64(F_RP_N_TRAINS, P.n_trains); W.f64(F_RP_DROP_PROB, P.memory_drop_prob);
+        const std::vector<int32_t> npe(P.nodes_per_episode.begin(), P.nodes_per_episode.end());
+        W.field(F_RP_NODES_PER_EPISODE, npe.data(), npe.size() * 4);
+        std::ostringstream mt;
+        mt << P.mt;
+        const std::string s = mt.str();
+        W.field(F_RP_MT, s.data(), s.size());
+        W.field(F_RP_SAMPLER, P.sampler.data(), P.sampler.size() * 4);
+    }
+    // the arena
+    {
+        const uint32_t hdr[2] = {F_ARENA, 0u};
+        const uint64_t G64 = (uint64_t)G, nbytes = 8 + 8 * G64 + 8 + (uint64_t)off[G] * 4;
+        std::vector<uint64_t> w64(words.begin(), words.end());
+        const uint64_t cs = host_checksum(w64.data(), w64.size() * 8);
+        W.raw(hdr, 8); W.raw(&nbytes, 8); W.raw(&G64, 8); W.raw(w64.data(), w64.size() * 8); W.raw(&cs, 8);
+    }
+    Events ev;
+    const int grid_max = e->gc_pool_main;
+    std::vector<std::array<cudaEvent_t, 3>> chunk_ev;
+    std::vector<std::pair<size_t, int>> pending;   // (bytes, buffer) of the chunk copied but not written yet
+    auto write_chunk = [&](size_t bytes, int buf, cudaEvent_t done) -> int {
+        CK(cudaEventSynchronize(done));
+        const double t0 = now_s();
+        W.raw((uint8_t *)pin.p + buf * half, bytes);
+        g_snap_sec[2] += now_s() - t0;
+        return B200_OK;
+    };
+    int g0 = 0, k = 0;
+    size_t prev_bytes = 0; int prev_buf = -1; cudaEvent_t prev_done = nullptr;
+    while (g0 < G) {
+        int g1 = g0;
+        while (g1 < G && (size_t)(off[g1 + 1] - off[g0]) * 4 <= half) ++g1;
+        const int buf = k & 1;
+        const size_t bytes = (size_t)(off[g1] - off[g0]) * 4;
+        std::array<cudaEvent_t, 3> ce{ev.make(), ev.make(), ev.make()};
+        CK(cudaEventRecord(ce[0], e->stream));
+        k_snap_pack<<<std::min(grid_max, g1 - g0), GC_THREADS, 0, e->stream>>>(A, g0, g1, d_off, off[g0], d_ent, (uint32_t *)(d_stage + buf * half));
+        CK(cudaGetLastError());
+        CK(cudaEventRecord(ce[1], e->stream));
+        // the pinned half this chunk lands in was written out two chunks ago (write_chunk below runs in order)
+        CK(cudaMemcpyAsync((uint8_t *)pin.p + buf * half, d_stage + buf * half, bytes, cudaMemcpyDeviceToHost, e->stream));
+        CK(cudaEventRecord(ce[2], e->stream));
+        chunk_ev.push_back(ce);
+        if (prev_buf >= 0) { int rc = write_chunk(prev_bytes, prev_buf, prev_done); if (rc) return rc; }
+        prev_bytes = bytes; prev_buf = buf; prev_done = ce[2];
+        g0 = g1; ++k;
+    }
+    if (prev_buf >= 0) { int rc = write_chunk(prev_bytes, prev_buf, prev_done); if (rc) return rc; }
+    CK(cudaStreamSynchronize(e->stream));
+    for (auto &ce : chunk_ev) {
+        float a = 0.f, b = 0.f;
+        cudaEventElapsedTime(&a, ce[0], ce[1]); cudaEventElapsedTime(&b, ce[1], ce[2]);
+        g_snap_sec[0] += a * 1e-3; g_snap_sec[1] += b * 1e-3;
+    }
+    {
+        const uint32_t end[2] = {F_END, 0u};
+        const uint64_t zero = 0;
+        W.raw(end, 8); W.raw(&zero, 8); W.raw(&zero, 8);
+    }
+    const double t0 = now_s();
+    if (W.ok && fflush(W.f) != 0) W.ok = false;
+    if (W.ok && fsync(fileno(W.f)) != 0) W.ok = false;
+    const long long total = W.ok ? (long long)ftello(W.f) : -1;
+    g_snap_sec[2] += now_s() - t0;
+    if (!W.ok) return fail(B200_ERR_BAD_ARG, "b200_engine_save: writing " + tmp_path + " failed: " + strerror(errno));
+    fclose(W.f); W.f = nullptr;
+    if (rename(tmp_path.c_str(), path) != 0) return fail(B200_ERR_BAD_ARG, std::string("b200_engine_save: rename to ") + path + " failed: " + strerror(errno));
+    closer.keep = true;
+    if (bytes_out) *bytes_out = total;
+    return B200_OK;
+}
+
+namespace {
+struct Fields {
+    std::map<uint32_t, std::vector<uint8_t>> v;
+    bool has(uint32_t id) const { return v.count(id) != 0; }
+    bool scalar(uint32_t id, int64_t &out) const {
+        auto it = v.find(id);
+        if (it == v.end() || it->second.size() != 8) return false;
+        memcpy(&out, it->second.data(), 8);
+        return true;
+    }
+    bool real(uint32_t id, double &out) const {
+        auto it = v.find(id);
+        if (it == v.end() || it->second.size() != 8) return false;
+        memcpy(&out, it->second.data(), 8);
+        return true;
+    }
+};
+}  // namespace
+
+static int snap_bad(const std::string &path, const std::string &why) { return fail(B200_ERR_BAD_ARG, "b200_engine_load: " + path + ": " + why); }
+
+// everything of the engine but its arena, from the fields before it
+static int snap_restore_host(b200_engine *e, const Fields &F, const std::string &path) {
+    int64_t v = 0;
+    int rc = 0;
+    if (F.scalar(F_GC_HEADROOM, v)) e->gc_headroom = (int)v;
+    if (F.scalar(F_PATH_CACHE, v) && v) { rc = b200_set_path_cache(e, 1); if (rc) return rc; }   // saved on, restored with an empty cache
+    if (F.scalar(F_DEEP_CAP, v) && v) { rc = b200_set_deep_lane(e, (int)v); if (rc) return rc; }
+    if (F.has(F_WEIGHTS)) {
+        const auto &w = F.v.at(F_WEIGHTS);
+        if (w.size() != (size_t)B200_N_WEIGHTS * 4) return snap_bad(path, "value weights of the wrong size");
+        rc = b200_load_weights(e, reinterpret_cast<const float *>(w.data()));
+        if (rc) return rc;
+    }
+    if (F.has(F_DIST_WEIGHTS)) {
+        int64_t atoms = 0;
+        if (!F.scalar(F_DIST_ATOMS, atoms) || atoms < 2 || atoms > 64 || F.v.at(F_DIST_WEIGHTS).size() != dn_weight_count((int)atoms) * 4)
+            return snap_bad(path, "distributional weights of the wrong size");
+        rc = b200_load_dist_weights(e, reinterpret_cast<const float *>(F.v.at(F_DIST_WEIGHTS).data()), (int)atoms);
+        if (rc) return rc;
+    }
+    Arena &A = e->A;
+    const auto &cnt = F.v.count(F_COUNTERS) ? F.v.at(F_COUNTERS) : std::vector<uint8_t>();
+    if (cnt.size() != 48 * 8) return snap_bad(path, "counters missing");
+    int64_t fin_count = 0;
+    if (!F.scalar(F_FIN_COUNT, fin_count) || fin_count < 0 || !F.has(F_FIN_LOG) ||
+        F.v.at(F_FIN_LOG).size() != (size_t)std::min<int64_t>(fin_count, A.fin_cap) * 16)
+        return snap_bad(path, "finished-games log inconsistent");
+    CK(cudaMemcpyAsync(A.counters, cnt.data(), cnt.size(), cudaMemcpyHostToDevice, e->stream));
+    const int32_t fc = (int32_t)fin_count;
+    CK(cudaMemcpyAsync(A.fin_count, &fc, 4, cudaMemcpyHostToDevice, e->stream));
+    if (!F.v.at(F_FIN_LOG).empty()) CK(cudaMemcpyAsync(A.fin_log, F.v.at(F_FIN_LOG).data(), F.v.at(F_FIN_LOG).size(), cudaMemcpyHostToDevice, e->stream));
+    CK(cudaStreamSynchronize(e->stream));
+    if (F.has(F_REPLAY_CAPACITY)) {
+        int64_t mv = 0, cap = 0, rcap = 0, count = 0;
+        if (!F.scalar(F_REPLAY_MIN_VISITS, mv) || !F.scalar(F_REPLAY_CAPACITY, cap) || !F.scalar(F_REPLAY_CAP, rcap) || !F.scalar(F_REPLAY_COUNT, count) ||
+            !F.has(F_REPLAY_ROWS) || cap < 1 || cap > (1 << 29) || rcap < 0 || rcap > 2 * cap || count < 0 ||
+            F.v.at(F_REPLAY_ROWS).size() != (size_t)std::min<int64_t>(count, 2 * cap) * 212)
+            return snap_bad(path, "replay memory fields inconsistent");
+        rc = b200_replay_enable(e, (int)mv, (int)cap);
+        if (rc) return rc;
+        const auto &rows = F.v.at(F_REPLAY_ROWS);
+        if (!rows.empty()) CK(cudaMemcpyAsync(A.replay, rows.data(), rows.size(), cudaMemcpyHostToDevice, e->stream));
+        A.replay_cap = (int)rcap;
+        rc = rp_set_count(e, (int32_t)count);
+        if (rc) return rc;
+    }
+    if (F.has(F_RP_POLICY)) {
+        if (!A.replay) return snap_bad(path, "a replay policy without a replay memory");
+        ReplayPolicy P;
+        int64_t x[9];
+        const uint32_t ids[9] = {F_RP_POLICY, F_RP_MEMORY_SIZE, F_RP_EPISODES_PER_TRAIN, F_RP_GROWTH, F_RP_MEMORY_INDEX, F_RP_ACCUMULATED,
+                                 F_RP_LAST_ACCUMULATION, F_RP_LAST_TRAINING, F_RP_N_TRAINS};
+        for (int i = 0; i < 9; ++i) if (!F.scalar(ids[i], x[i])) return snap_bad(path, "replay policy field " + std::to_string(ids[i]) + " missing");
+        if (x[0] < 0 || x[0] > 3 || x[1] != e->replay_alloc / 2) return snap_bad(path, "replay policy inconsistent with the memory");
+        P.policy = (int)x[0]; P.memory_size = (int)x[1]; P.episodes_per_train = (int)x[2]; P.memory_growth_rate = (int)x[3]; P.memory_index = (int)x[4];
+        P.accumulated_nodes = (int)x[5]; P.last_accumulation_episode = (int)x[6]; P.last_training_episode = (int)x[7]; P.n_trains = (int)x[8];
+        if (!F.real(F_RP_DROP_PROB, P.memory_drop_prob) || !F.has(F_RP_NODES_PER_EPISODE) || !F.has(F_RP_MT) || !F.has(F_RP_SAMPLER))
+            return snap_bad(path, "replay policy fields missing");
+        const auto &npe = F.v.at(F_RP_NODES_PER_EPISODE), &smp = F.v.at(F_RP_SAMPLER), &mt = F.v.at(F_RP_MT);
+        if (npe.size() % 4 || smp.size() % 4 || (!smp.empty() && smp.size() != (size_t)P.memory_size * 4)) return snap_bad(path, "replay policy lists malformed");
+        for (size_t i = 0; i < npe.size(); i += 4) { int32_t q; memcpy(&q, &npe[i], 4); P.nodes_per_episode.push_back(q); }
+        P.sampler.resize(smp.size() / 4);
+        if (!smp.empty()) memcpy(P.sampler.data(), smp.data(), smp.size());
+        for (int s : P.sampler) if (s < 0 || s >= P.memory_size) return snap_bad(path, "replay policy sampler index out of range");
+        std::istringstream in(std::string(mt.begin(), mt.end()));
+        in >> P.mt;
+        if (in.fail()) return snap_bad(path, "replay policy random state malformed");
+        e->rp = P;
+    }
+    return B200_OK;
+}
+
+extern "C" int b200_engine_load(const char *path, int device, b200_engine **out) {
+    if (!path || !out) return fail(B200_ERR_BAD_ARG, "null argument");
+    *out = nullptr;
+    for (double &s : g_snap_sec) s = 0.0;
+    const std::string P = path;
+    Reader R;
+    R.f = fopen(path, "rb");
+    if (!R.f) return snap_bad(P, std::string("cannot open: ") + strerror(errno));
+    struct FileGuard { FILE *f; ~FileGuard() { fclose(f); } } fguard{R.f};
+    if (fseeko(R.f, 0, SEEK_END) != 0) return snap_bad(P, "not seekable");
+    R.left = (uint64_t)ftello(R.f);
+    fseeko(R.f, 0, SEEK_SET);
+    char magic[8]; uint32_t version = 0, bom = 0;
+    if (!R.raw(magic, 8) || !R.raw(&version, 4) || !R.raw(&bom, 4)) return snap_bad(P, "truncated header");
+    if (memcmp(magic, SNAP_MAGIC, 8) != 0) return snap_bad(P, "not an engine image (wrong magic)");
+    if (bom != SNAP_BOM) return snap_bad(P, "written with another byte order");
+    if (version != SNAP_VERSION) return snap_bad(P, "format version " + std::to_string(version) + ", this library reads version " + std::to_string(SNAP_VERSION));
+    Fields F;
+    uint32_t hdr[2]; uint64_t nbytes = 0;
+    for (;;) {
+        if (!R.raw(hdr, 8) || !R.raw(&nbytes, 8)) return snap_bad(P, "truncated");
+        if (hdr[0] == F_ARENA) break;
+        if (hdr[0] == F_END) return snap_bad(P, "no arena");
+        if (!snap_known(hdr[0]) || hdr[1] != 0u) return snap_bad(P, "unknown field " + std::to_string(hdr[0]));
+        if (F.has(hdr[0])) return snap_bad(P, "field " + std::to_string(hdr[0]) + " twice");
+        if (nbytes > R.left || R.left - nbytes < 8) return snap_bad(P, "truncated");
+        std::vector<uint8_t> b(nbytes);
+        uint64_t cs = 0;
+        if (!R.raw(b.data(), nbytes) || !R.raw(&cs, 8)) return snap_bad(P, "truncated");
+        if (cs != host_checksum(b.data(), b.size())) return snap_bad(P, "field " + std::to_string(hdr[0]) + ": checksum mismatch");
+        F.v[hdr[0]] = std::move(b);
+    }
+    // the configuration: every field present
+    b200_config c;
+    memset(&c, 0, sizeof(c));
+    {
+        int64_t x[15];
+        const uint32_t ids[15] = {F_N_GAMES, F_MAX_NODES, F_MODE, F_LOW, F_LP_END_FROM_OBS, F_LP_VAR_GAMMA2, F_STALE_POP, F_OVERFLOW_RESET,
+                                  F_EVAL_KIND, F_TRACE_MAX, F_ACTIONS_PER_DROP, F_SCORING, F_RANDOMIZER, F_DEVICE, F_SEED};
+        for (int i = 0; i < 15; ++i) if (!F.scalar(ids[i], x[i])) return snap_bad(P, "configuration field " + std::to_string(ids[i]) + " missing");
+        int64_t bins = 0;
+        if (!F.real(F_GAMMA, c.gamma) || !F.real(F_ROLLOUT_VARIANCE, c.rollout_variance) || !F.scalar(F_DIST_BINS, bins) ||
+            !F.real(F_DIST_VMIN, c.dist_vmin) || !F.real(F_DIST_VMAX, c.dist_vmax))
+            return snap_bad(P, "configuration incomplete");
+        c.n_games = (int32_t)x[0]; c.max_nodes = (int32_t)x[1]; c.mode = (int32_t)x[2]; c.low = (int32_t)x[3]; c.lp_end_from_obs = (int32_t)x[4];
+        c.lp_var_gamma2 = (int32_t)x[5]; c.stale_pop = (int32_t)x[6]; c.overflow_reset = (int32_t)x[7]; c.eval_kind = (int32_t)x[8];
+        c.trace_max = (int32_t)x[9]; c.actions_per_drop = (int32_t)x[10]; c.scoring = (int32_t)x[11]; c.randomizer = (int32_t)x[12];
+        c.device = device >= 0 ? device : (int32_t)x[13]; c.seed = (uint32_t)x[14]; c.dist_bins = (int32_t)bins;
+        if (x[0] < 1 || x[0] > (1 << 24)) return snap_bad(P, "n_games out of range");
+    }
+    // the arena's framing, checked before anything is allocated
+    const int G = c.n_games;
+    uint64_t G64 = 0;
+    if (!R.raw(&G64, 8) || G64 != (uint64_t)G) return snap_bad(P, "arena of another number of games");
+    std::vector<uint64_t> w64(G);
+    uint64_t wcs = 0;
+    if (!R.raw(w64.data(), (uint64_t)G * 8) || !R.raw(&wcs, 8)) return snap_bad(P, "truncated");
+    if (wcs != host_checksum(w64.data(), w64.size() * 8)) return snap_bad(P, "arena size table: checksum mismatch");
+    std::vector<long long> words(G), off(G + 1, 0);
+    for (int g = 0; g < G; ++g) {
+        if (w64[g] < (uint64_t)SNAP_HDR + 2 || w64[g] > (1ull << 40)) return snap_bad(P, "game " + std::to_string(g) + ": size out of range");
+        words[g] = (long long)w64[g];
+        off[g + 1] = off[g] + words[g];
+    }
+    if (nbytes != 8 + 8 * (uint64_t)G + 8 + (uint64_t)off[G] * 4) return snap_bad(P, "arena length does not match its games");
+    if ((uint64_t)off[G] * 4 + 24 > R.left) return snap_bad(P, "truncated");
+    // the engine
+    b200_engine *e = nullptr;
+    int rc = b200_engine_create(&c, &e);
+    if (rc) return rc;
+    struct Guard { b200_engine *e; ~Guard() { if (e) b200_engine_destroy(e); } } guard{e};
+    rc = snap_restore_host(e, F, P);
+    if (rc) return rc;
+    F.v.clear();
+    const Arena &A = e->A;
+    const size_t half = snap_half(words);
+    Scratch tmp;
+    uint8_t *d_stage = nullptr; long long *d_off = nullptr; unsigned long long *d_err = nullptr;
+    CK(tmp.get(&d_stage, 2 * half)); CK(tmp.get(&d_off, (size_t)(G + 1) * 8)); CK(tmp.get(&d_err, 8));
+    const unsigned long long err0 = ~0ull;
+    CK(cudaMemcpyAsync(d_off, off.data(), (size_t)(G + 1) * 8, cudaMemcpyHostToDevice, e->stream));
+    CK(cudaMemcpyAsync(d_err, &err0, 8, cudaMemcpyHostToDevice, e->stream));
+    Pinned pin;
+    CK(cudaHostAlloc(&pin.p, 2 * half, cudaHostAllocDefault));
+    Events ev;
+    std::vector<std::array<cudaEvent_t, 3>> chunk_ev;
+    cudaEvent_t copied[2] = {nullptr, nullptr};   // the H2D of the chunk last read into each pinned half
+    int g0 = 0, k = 0;
+    while (g0 < G) {
+        int g1 = g0;
+        while (g1 < G && (size_t)(off[g1 + 1] - off[g0]) * 4 <= half) ++g1;
+        const int buf = k & 1;
+        const size_t bytes = (size_t)(off[g1] - off[g0]) * 4;
+        if (copied[buf]) CK(cudaEventSynchronize(copied[buf]));
+        const double t0 = now_s();
+        if (!R.raw((uint8_t *)pin.p + buf * half, bytes)) return snap_bad(P, "truncated");
+        g_snap_sec[3] += now_s() - t0;
+        std::array<cudaEvent_t, 3> ce{ev.make(), ev.make(), ev.make()};
+        CK(cudaEventRecord(ce[0], e->stream));
+        CK(cudaMemcpyAsync(d_stage + buf * half, (uint8_t *)pin.p + buf * half, bytes, cudaMemcpyHostToDevice, e->stream));
+        CK(cudaEventRecord(ce[1], e->stream));
+        k_snap_unpack<<<std::min(e->gc_pool_main, g1 - g0), GC_THREADS, 0, e->stream>>>(A, g0, g1, d_off, off[g0], (const uint32_t *)(d_stage + buf * half), d_err);
+        CK(cudaGetLastError());
+        CK(cudaEventRecord(ce[2], e->stream));
+        chunk_ev.push_back(ce);
+        copied[buf] = ce[1];
+        g0 = g1; ++k;
+    }
+    unsigned long long err = 0;
+    CK(cudaMemcpyAsync(&err, d_err, 8, cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaStreamSynchronize(e->stream));
+    for (auto &ce : chunk_ev) {
+        float a = 0.f, b = 0.f;
+        cudaEventElapsedTime(&a, ce[0], ce[1]); cudaEventElapsedTime(&b, ce[1], ce[2]);
+        g_snap_sec[4] += a * 1e-3; g_snap_sec[5] += b * 1e-3;
+    }
+    if (err != ~0ull) {
+        static const char *why[] = {"", "checksum mismatch", "header or size inconsistent", "free lists malformed", "index out of range"};
+        const unsigned reason = (unsigned)(err & 0xffu);
+        return snap_bad(P, "game " + std::to_string(err >> 8) + ": " + why[reason >= 1 && reason <= 4 ? reason : 0]);
+    }
+    if (!R.raw(hdr, 8) || !R.raw(&nbytes, 8) || hdr[0] != F_END || hdr[1] != 0u || nbytes != 0) return snap_bad(P, "truncated (no end mark)");
+    guard.e = nullptr;
+    *out = e;
     return B200_OK;
 }

@@ -65,6 +65,34 @@ class BatchedEngine:
         except Exception:
             pass
 
+    # ------------------------------------------------------------------ snapshot (b200_engine_save / b200_engine_load)
+    def save(self, path):
+        """Write everything the engine would read next to `path` (include/b200_tetris_mcts.h, DESIGN §4c): trees, games, search streams,
+        counters, weights, replay memory and policy.  Written to path + ".tmp" and renamed.  Returns the image's size in bytes."""
+        n = np.zeros(1, np.int64)
+        L.check(L.lib().b200_engine_save(self.h, os.fsencode(path), L.ptr(n)))
+        return int(n[0])
+
+    @classmethod
+    def load(cls, path, device=None):
+        """The engine a save() wrote, continuing bit for bit as the saved one would (its path cache restarts empty).  device None: the saved
+        ordinal.  A truncated, corrupted or foreign file raises B200Error (BAD_ARG)."""
+        fields = read_image_fields(path)
+        h = L.P()
+        L.check(L.lib().b200_engine_load(os.fsencode(path), -1 if device is None else int(device), C.byref(h)))
+        self = cls.__new__(cls)
+        cfg = L.Config()
+        for name, _t in L.Config._fields_:
+            setattr(cfg, name, fields[name])
+        if device is not None:
+            cfg.device = int(device)
+        self.cfg, self.h, self._ext = cfg, h, None
+        self.n_games, self.max_nodes, self.mode, self.eval_kind = int(cfg.n_games), int(cfg.max_nodes), int(cfg.mode), int(cfg.eval_kind)
+        self.path_cache = bool(fields.get("path_cache", 0))
+        if "dist_atoms" in fields:
+            self._atoms = int(fields["dist_atoms"])
+        return self
+
     # ------------------------------------------------------------------ weights (model/model.py:163-174 Model.load)
     def load_weights(self, weights):
         w = np.ascontiguousarray(weights, np.float32).ravel()
@@ -340,6 +368,57 @@ class BatchedEngine:
         cnt = np.zeros(1, np.int32)
         L.check(L.lib().b200_collect_samples_dev(self.h, int(min_visits), C.c_void_p(int(dev_ptr)), int(capacity), L.ptr(cnt)))
         return int(cnt[0])
+
+
+IMAGE_MAGIC, IMAGE_VERSION, IMAGE_BOM = b"B200SNAP", 1, 0x01020304
+# the scalar fields of an engine image (capi.cu "snapshot"): id -> (name, is a double)
+IMAGE_SCALARS = {1: ("n_games", False), 2: ("max_nodes", False), 3: ("mode", False), 4: ("low", False), 5: ("lp_end_from_obs", False),
+                 6: ("lp_var_gamma2", False), 7: ("stale_pop", False), 8: ("overflow_reset", False), 9: ("eval_kind", False),
+                 10: ("trace_max", False), 11: ("actions_per_drop", False), 12: ("scoring", False), 13: ("randomizer", False),
+                 14: ("device", False), 15: ("seed", False), 16: ("gamma", True), 17: ("rollout_variance", True), 18: ("dist_bins", False),
+                 19: ("dist_vmin", True), 20: ("dist_vmax", True), 32: ("path_cache", False), 33: ("deep_cap", False),
+                 34: ("gc_headroom", False), 41: ("dist_atoms", False)}
+IMAGE_ARENA = 128
+
+
+def read_image_fields(path):
+    """The named scalar fields of an engine image, read up to its arena without loading anything: {"n_games": .., "gamma": .., ...}.
+    Raises ValueError on a file that is not an image of this format version or ends early."""
+    import struct
+    with open(path, "rb") as f:
+        head = f.read(16)
+        if len(head) < 16:
+            raise ValueError("%s: truncated header" % path)
+        if head[:8] != IMAGE_MAGIC:
+            raise ValueError("%s: not an engine image (wrong magic)" % path)
+        version, bom = struct.unpack("<II", head[8:])
+        if bom != IMAGE_BOM:
+            raise ValueError("%s: written with another byte order" % path)
+        if version != IMAGE_VERSION:
+            raise ValueError("%s: format version %d, this library reads version %d" % (path, version, IMAGE_VERSION))
+        out = {}
+        while True:
+            hdr = f.read(16)
+            if len(hdr) < 16:
+                raise ValueError("%s: truncated" % path)
+            fid, _zero, nbytes = struct.unpack("<IIQ", hdr)
+            if fid == IMAGE_ARENA:
+                break
+            if fid == 0:
+                raise ValueError("%s: no arena" % path)
+            if fid in IMAGE_SCALARS and nbytes == 8:
+                name, real = IMAGE_SCALARS[fid]
+                raw = f.read(8)
+                if len(raw) < 8:
+                    raise ValueError("%s: truncated" % path)
+                out[name] = struct.unpack("<d" if real else "<q", raw)[0]
+                f.seek(8, 1)
+            else:
+                f.seek(nbytes + 8, 1)
+        missing = [n for i, (n, _r) in IMAGE_SCALARS.items() if i <= 20 and n not in out]
+        if missing:
+            raise ValueError("%s: configuration fields missing: %s" % (path, ", ".join(missing)))
+        return out
 
 
 _BOARD_DTYPES = {"int8": L.BOARD_INT8, "float32": L.BOARD_F32}

@@ -60,6 +60,30 @@ class OnlineTrainer:
         self.train_seconds += time.perf_counter() - t0
         return True
 
+    def state(self):
+        """What a resumed run needs to train on exactly as this one would: n_trains (it seeds the batch draws), train_seconds, the current
+        weights and, once the trainer exists, its Yogi state (exp_avg, exp_avg_sq, step)."""
+        st = dict(n_trains=self.n_trains, train_seconds=self.train_seconds, weights=None if self.weights is None else self.weights.copy(),
+                  optimizer=None)
+        if self.model is not None and self.model._trainer is not None:
+            m, v, step = self.model._trainer.state()
+            st["optimizer"] = (m, v, step)
+        return st
+
+    def restore(self, state):
+        """The inverse of state(): weights into the engine's search and the trainer (created here if the state has optimiser moments)."""
+        self.n_trains, self.train_seconds = int(state["n_trains"]), float(state["train_seconds"])
+        if state["weights"] is not None:
+            self.weights = state["weights"]
+            self.eng.load_weights(self.weights)
+        if state["optimizer"] is not None:
+            m = self._model()
+            m.weights = self.weights
+            m._eng.load_weights(self.weights)
+            t = m._trainer_obj()
+            t.set_weights(self.weights)
+            t.set_state(*state["optimizer"])
+
     def close(self):
         if self.model is not None:
             self.model.close()

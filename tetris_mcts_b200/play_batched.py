@@ -16,6 +16,13 @@ rows (Model_VV.train_rows), saved to ./pytorch_model/model_checkpoint and swappe
   torchrun --nproc-per-node 8 -m tetris_mcts_b200.play_batched --agent_type ValueSimLP --online --n_parallel 32768 --endless
   python -m tetris_mcts_b200.play_batched --agent_type ValueSimLP --evaluator mynets:make_evaluator --n_parallel 4096 --endless
 
+--checkpoint_dir DIR writes a checkpoint there every --checkpoint_every moves (0: when the run ends), after the move's training: one engine image
+per rank (BatchedEngine.save) and the run's own state, as one generation DIR/gen<moves> that DIR/latest names once it is complete; --resume
+continues from that generation as the stopped processes would have gone on (DESIGN §4c: exactly so only where the run itself is
+deterministic, one game per rank under --online):
+
+  python -m tetris_mcts_b200.play_batched --agent_type ValueSimLP --online --endless --checkpoint_dir ckpt --checkpoint_every 100 --resume
+
 --evaluator MODULE:FACTORY searches with the caller's network instead of the built-in one: FACTORY(device) returns a device evaluator
 (BatchedEngine.run_sims: a torch tensor [n,1,20,10] of boards in, (v, var) out), and the engine runs eval_kind "external".
 
@@ -83,6 +90,110 @@ def save_suffix(rank, world):
     return "" if world == 1 else ".rank%d" % rank
 
 
+# flags a resumed run must share with the run that wrote the checkpoint (they change what the engine, the memory or the trainer hold)
+RESUME_FLAGS = ("agent_type", "n_parallel", "max_nodes", "seed", "eval_kind", "train_kind", "online", "memory_size", "accumulation_policy",
+                "episodes_per_train", "memory_growth_rate", "train_batch_size", "train_max_iters", "mcts_sims", "app", "tetris_scoring",
+                "tetris_randomizer", "save", "cycle")
+
+
+# A checkpoint is one generation: DIR/gen<moves>/ holds every rank's engine image and run state, each run state naming its image and the
+# image's size.  DIR/latest names the newest complete generation; rank 0 replaces it (written aside, synced, renamed) only after every rank
+# has written its files, and older generations are deleted only after that.  A run stopped at any point leaves `latest` on a generation
+# whose files are all there.  DIR is shared by the ranks.
+def generation_dir(directory, gen):
+    return os.path.join(directory, "gen%09d" % gen)
+
+
+def checkpoint_paths(directory, gen, rank):
+    d = generation_dir(directory, gen)
+    return os.path.join(d, "engine.rank%d" % rank), os.path.join(d, "run.rank%d" % rank)
+
+
+def _write_synced(path, data):
+    with open(path + ".tmp", "wb") as f:
+        f.write(data)
+        f.flush()
+        os.fsync(f.fileno())
+    os.replace(path + ".tmp", path)
+
+
+def write_latest(directory, gen):
+    _write_synced(os.path.join(directory, "latest"), b"%d\n" % gen)
+
+
+def read_latest(directory):
+    path = os.path.join(directory, "latest")
+    if not os.path.isfile(path):
+        raise ValueError("--resume: no checkpoint in %s (no %s)" % (directory, path))
+    with open(path) as f:
+        return int(f.read().strip())
+
+
+def write_run_state(path, state):
+    import pickle
+    _write_synced(path, pickle.dumps(state))
+
+
+def read_run_state(args, rank, world):
+    """(run state, engine image path) of rank `rank` in the generation DIR/latest names.  Raises ValueError when the checkpoint is missing,
+    when the run state and its image are not of one generation, when the checkpointed run had finished, or when it was written with other
+    flags (the message names them)."""
+    import pickle
+    gen = read_latest(args.checkpoint_dir)
+    image, path = checkpoint_paths(args.checkpoint_dir, gen, rank)
+    if not os.path.isfile(path):
+        raise ValueError("--resume: no run state at %s" % path)
+    with open(path, "rb") as f:
+        st = pickle.load(f)
+    if st.get("generation") != gen or st.get("moves") != gen:
+        raise ValueError("--resume: %s is the run state of move %s, not of generation %d" % (path, st.get("moves"), gen))
+    if st.get("image") != os.path.basename(image) or not os.path.isfile(image) or os.path.getsize(image) != st.get("image_bytes"):
+        raise ValueError("--resume: the engine image %s is not the one the run state %s names" % (image, path))
+    if st.get("finished"):
+        raise ValueError("--resume: the run checkpointed in %s had finished (--ngames reached)" % args.checkpoint_dir)
+    differ = ["world size (%d, checkpoint %d)" % (world, st["world"])] if st["world"] != world else []
+    differ += ["--%s (%r, checkpoint %r)" % (k, getattr(args, k), st["flags"].get(k)) for k in RESUME_FLAGS if st["flags"].get(k) != getattr(args, k)]
+    if differ:
+        raise ValueError("--resume: the checkpoint in %s was written with other settings: %s" % (args.checkpoint_dir, "; ".join(differ)))
+    return st, image
+
+
+def agree_on_generation(found):
+    """found: every rank's (generation, None) or (None, error message) -> the one generation; raises ValueError (on every rank) when a rank
+    failed or the ranks read different generations"""
+    errors = ["rank %d: %s" % (r, err) for r, (_g, err) in enumerate(found) if err]
+    if errors:
+        raise ValueError("; ".join(errors))
+    gens = [g for g, _e in found]
+    if len(set(gens)) != 1:
+        raise ValueError("--resume: the ranks found checkpoints of different moves: %s" % gens)
+    return gens[0]
+
+
+def drop_older_generations(directory, gen, rank):
+    """this rank's files of every generation but `gen` (after `latest` names gen)"""
+    for name in os.listdir(directory):
+        if not name.startswith("gen") or name == os.path.basename(generation_dir(directory, gen)):
+            continue
+        d = os.path.join(directory, name)
+        for f in ("engine.rank%d" % rank, "run.rank%d" % rank, "engine.rank%d.tmp" % rank, "run.rank%d.tmp" % rank):
+            if os.path.exists(os.path.join(d, f)):
+                os.remove(os.path.join(d, f))
+        try:
+            os.rmdir(d)
+        except OSError:
+            pass                                                                           # another rank's files are still there
+
+
+def drop_later_chunks(file_name, chunk):
+    """a resumed run rewrites the --save chunks from number `chunk` on: those the stopped run wrote after its checkpoint go"""
+    import glob
+    for f in glob.glob(glob.escape(file_name) + ".*.npy"):
+        idx = f[len(file_name) + 1:-4]
+        if idx.isdigit() and int(idx) >= chunk:
+            os.remove(f)
+
+
 def run(args, out=sys.stdout, timing=None):
     """timing: a dict, filled with moves, trainings and the wall-clock seconds of the run split into search (everything but training) and
     training (--online).
@@ -99,11 +210,24 @@ def run(args, out=sys.stdout, timing=None):
     mode, gamma, low = MODES[args.agent_type]
     env_args = ((20, 10), args.app, args.tetris_scoring, args.tetris_randomizer)           # play.py:75
     weights, evaluator = None, None
+    resumed = None
+    if args.resume:
+        try:
+            resumed, image = read_run_state(args, rank, world)
+            found = (resumed["generation"], None)
+        except ValueError as exc:
+            found = (None, str(exc))
+        if world > 1:                                                                      # every rank resumes from the same generation, or none
+            agree_on_generation(D.gather_objects(found))
+        elif found[1]:
+            raise ValueError(found[1])
     if args.evaluator:
         import importlib
         import torch
         module, factory = args.evaluator.split(":", 1)
         evaluator = getattr(importlib.import_module(module), factory)(torch.device("cuda", device))
+    elif mode != "vanilla" and resumed is not None:
+        weights = resumed["trainer"]["weights"] if resumed["trainer"] else None               # the engine image holds the search's own
     elif mode != "vanilla":
         from .model.model_vv import init_weights, load_checkpoint_weights
         if rank == 0:
@@ -115,20 +239,26 @@ def run(args, out=sys.stdout, timing=None):
         if weights is None:
             weights = init_weights(0)
     # k_init_arena seeds game g's search stream with seed + 0x9E3779B9 * (g + 1): offset by the shard's first global index
-    eng = BatchedEngine(hi - lo, max_nodes=args.max_nodes, mode=mode, gamma=gamma, low=low,
-                        eval_kind="external" if evaluator else (args.eval_kind if mode != "vanilla" else "synthetic"), weights=weights, env_args=env_args,
-                        seed=(args.seed + 0x9E3779B9 * lo) & 0xFFFFFFFF, device=device, overflow_reset=True)
-    eng.set_games(PT.new_games(hi - lo, env_args, D.shard_seeds(args.seed, args.n_parallel, rank, world)))
-    eng.set_gc_headroom(args.max_nodes * 5 // 32)
+    if resumed is not None:                                                               # trees, games, memory and policy as they were saved
+        eng = BatchedEngine.load(image, device=device)
+    else:
+        eng = BatchedEngine(hi - lo, max_nodes=args.max_nodes, mode=mode, gamma=gamma, low=low,
+                            eval_kind="external" if evaluator else (args.eval_kind if mode != "vanilla" else "synthetic"), weights=weights,
+                            env_args=env_args, seed=(args.seed + 0x9E3779B9 * lo) & 0xFFFFFFFF, device=device, overflow_reset=True)
+        eng.set_games(PT.new_games(hi - lo, env_args, D.shard_seeds(args.seed, args.n_parallel, rank, world)))
+        eng.set_gc_headroom(args.max_nodes * 5 // 32)
     online = args.online and not args.benchmark and mode != "vanilla"
     trainer, gcs, block = None, 0, None
     if online:                                                                             # ValueSim.py:21-37 memory, min_visits_to_store (25: ValueSimLP.py:11)
         from .online import OnlineTrainer
-        eng.replay_enable(min_visits=25 if mode == "lp" else 10, capacity=args.memory_size)
-        if rank == 0:
-            eng.replay_policy(args.accumulation_policy, episodes_per_train=args.episodes_per_train, memory_growth_rate=args.memory_growth_rate)
+        if resumed is None:
+            eng.replay_enable(min_visits=25 if mode == "lp" else 10, capacity=args.memory_size)
+            if rank == 0:
+                eng.replay_policy(args.accumulation_policy, episodes_per_train=args.episodes_per_train, memory_growth_rate=args.memory_growth_rate)
         trainer = OnlineTrainer(eng, weights, args.memory_size, batch_size=args.train_batch_size, max_iters=args.train_max_iters,
                                 train_kind=args.train_kind)   # ValueSim.py:180
+        if resumed is not None and resumed["trainer"]:
+            trainer.restore(resumed["trainer"])
         if world > 1:                                                                      # the rows one move's collections stored on this rank
             import torch
             block = torch.empty((args.memory_size, D.SAMPLE_BYTES), dtype=torch.uint8, device=trainer.buf.device)
@@ -140,6 +270,36 @@ def run(args, out=sys.stdout, timing=None):
         episode_of = np.zeros(hi - lo, np.int32)                                           # play.py passes ngames: the episode a row belongs to
     tracker = ScoreTracker()
     ngames, moves = 0, 0
+    if resumed is not None:
+        ngames, moves, gcs = resumed["ngames"], resumed["moves"], resumed["gcs"]
+        tracker.scores, tracker.lines = list(resumed["scores"]), list(resumed["lines"])
+        if saver:
+            episode_of[:] = resumed["episode_of"]
+            if not saver.hdf5:
+                saver.chunk = resumed["saver_chunk"]
+                drop_later_chunks(saver.file_name, saver.chunk)
+
+    def checkpoint(finished):
+        """after a completed move (and its training): every rank's engine image and run state in generation `moves`, then `latest`"""
+        if saver:
+            saver.flush()                                                                  # the rows so far are on disk: a resume appends the rest
+        os.makedirs(generation_dir(args.checkpoint_dir, moves), exist_ok=True)
+        if world > 1:
+            D.barrier()
+        image, state = checkpoint_paths(args.checkpoint_dir, moves, rank)
+        size = eng.save(image)
+        write_run_state(state, dict(world=world, flags={k: getattr(args, k) for k in RESUME_FLAGS}, generation=moves, ngames=ngames, moves=moves,
+                                    gcs=gcs, image=os.path.basename(image), image_bytes=size, finished=bool(finished),
+                                    scores=list(tracker.scores), lines=list(tracker.lines), trainer=trainer.state() if trainer else None,
+                                    episode_of=episode_of.copy() if saver else None,
+                                    saver_chunk=saver.chunk if saver and not saver.hdf5 else None))
+        if world > 1:
+            D.barrier()                                                                    # every rank's files of this generation are written
+        if rank == 0:
+            write_latest(args.checkpoint_dir, moves)
+        if world > 1:
+            D.barrier()
+        drop_older_generations(args.checkpoint_dir, moves, rank)
     t_start = time.perf_counter()
     try:
         while True:
@@ -185,7 +345,10 @@ def run(args, out=sys.stdout, timing=None):
                     train_now, n = D.broadcast_ints([train_now, n])
                 if train_now:
                     trainer.train(n, ngames)
-            if done or (args.max_moves and moves >= args.max_moves):
+            last = done or (args.max_moves and moves >= args.max_moves)
+            if args.checkpoint_dir and (last or (args.checkpoint_every and moves % args.checkpoint_every == 0)):
+                checkpoint(done)
+            if last:
                 break
     finally:
         if rank == 0:
@@ -253,7 +416,10 @@ def parse_args(argv=None):
     p.add_argument('--evaluator', default=None, metavar='MODULE:FACTORY',
                    help='search with the caller\'s network: FACTORY(device) returns a device evaluator (boards [n,1,20,10] -> (v, var)); '
                         'the engine runs eval_kind external.  Not with --online (the trainer trains the built-in network) nor Vanilla')
-    p.add_argument('--max_moves', default=0, type=int)
+    p.add_argument('--max_moves', default=0, type=int, help='stop after this many moves (counted from the start of the run, across --resume)')
+    p.add_argument('--checkpoint_dir', default=None, help='write checkpoints here (one engine image per rank and the run state)')
+    p.add_argument('--checkpoint_every', default=0, type=int, help='moves between checkpoints; 0 = only when the run ends')
+    p.add_argument('--resume', default=False, action='store_true', help='continue the run checkpointed in --checkpoint_dir')
     p.add_argument('--dist_backend', default='nccl', choices=('nccl', 'gloo'),
                    help='under torchrun: collectives over NCCL (one GPU per rank), or gloo through the host (several ranks may share a GPU)')
     args = p.parse_args(argv)
@@ -263,6 +429,12 @@ def parse_args(argv=None):
         p.error('--evaluator cannot be combined with --agent_type Vanilla: Vanilla evaluates leaves by random rollout')
     if args.evaluator and ':' not in args.evaluator:
         p.error('--evaluator takes MODULE:FACTORY')
+    if (args.resume or args.checkpoint_every) and not args.checkpoint_dir:
+        p.error('--resume and --checkpoint_every need --checkpoint_dir')
+    if args.checkpoint_dir and args.evaluator:
+        p.error('--checkpoint_dir cannot be combined with --evaluator: the caller\'s network is not part of the checkpoint')
+    if args.checkpoint_every < 0:
+        p.error('--checkpoint_every takes a number of moves >= 0')
     return args
 
 
