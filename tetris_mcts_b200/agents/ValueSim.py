@@ -13,9 +13,13 @@ class ValueSim(TreeAgent):
     _mode = "single"
 
     def __init__(self, online=True, memory_size=500000, min_visits_to_store=10, gamma=0.999, memory_growth_rate=5000, weights=None,
-                 train_kind="fp64", **kwargs):
+                 train_kind="fp64", train=None, train_on_device=False, **kwargs):
+        """train: the reference's train callback (OnlineMCTSAgent(..., train=), agents/ValueSimC.py), train(state, value, variance, visit,
+        size), called instead of the built-in trainer when online=True (online.CallbackTrainer): with evaluator= it updates that network in
+        place and returns None; without, it returns the new weights of the engine's network (a Model_VV state_dict or N_WEIGHTS floats) or
+        None.  train_on_device: hand it torch tensors on the engine's device instead of numpy arrays."""
         kwargs.pop("max_nodes", None)
-        if kwargs.get("evaluator") is not None and online and not kwargs.get("benchmark", False):
+        if kwargs.get("evaluator") is not None and online and not kwargs.get("benchmark", False) and train is None:
             raise ValueError("online=True trains the engine's Model_VV weights on the device, not the caller's evaluator: pass online=False")
         if weights is None and kwargs.get("evaluator") is None:
             # ValueSim.py:42-44: self.model = Model(); self.model.load(); self.model.training(False).  Model.load (model/model.py:163-174)
@@ -28,12 +32,16 @@ class ValueSim(TreeAgent):
         self.memory_size, self.memory_growth_rate, self.n_trains = memory_size, memory_growth_rate, 0   # ValueSim.py:21-37
         self._weights, self._online = np.asarray(weights, np.float32), None
         if online and not self.benchmark:                         # ValueSim.py:21-37: the replay memory lives on the device (k_gc fills it)
-            from ..online import OnlineTrainer
+            from ..online import CallbackTrainer, OnlineTrainer
             self._eng.replay_enable(min_visits=min_visits_to_store, capacity=memory_size)
             # accumulation policy 3 is train_nodes' rule: train once memory_index >= min(n_trains * memory_growth_rate, memory_size)
             self._eng.replay_policy(3, memory_growth_rate=memory_growth_rate)
-            self._online = OnlineTrainer(self._eng, self._weights, memory_size, batch_size=1024, iters_per_val=100, max_iters=50000,
-                                         train_kind=train_kind)   # ValueSim.py:180
+            if train is not None:
+                self._online = CallbackTrainer(self._eng, self._weights, memory_size, train, host=not train_on_device,
+                                               external=kwargs.get("evaluator") is not None)
+            else:
+                self._online = OnlineTrainer(self._eng, self._weights, memory_size, batch_size=1024, iters_per_val=100, max_iters=50000,
+                                             train_kind=train_kind)   # ValueSim.py:180
             self._gcs = 0
             print('online: freed observations are stored on the device as in ValueSim.store_nodes (ValueSim.py:122-159) and the value network '
                   'is trained on them after the collections that fill the memory (train_nodes, ValueSim.py:161-185)', **perr)

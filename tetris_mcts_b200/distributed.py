@@ -143,6 +143,16 @@ def broadcast_rows(buf, n):
     torch.cuda.current_stream(buf.device).synchronize()
 
 
+def broadcast_weights(weights):
+    """rank 0's float32 value-network weight vector (N_WEIGHTS floats) -> every rank, as a numpy float32 array; the other ranks pass None"""
+    from . import _lib as L
+    dev = "cuda" if on_device() else "cpu"
+    t = torch.as_tensor(np.ascontiguousarray(weights, np.float32)).to(dev) if dist.get_rank() == 0 else \
+        torch.empty(L.N_WEIGHTS, dtype=torch.float32, device=dev)
+    dist.broadcast(t, src=0)
+    return t.cpu().numpy()
+
+
 def broadcast_ints(values):
     """a list of ints of rank 0 -> every rank"""
     t = torch.tensor([int(v) for v in values], dtype=torch.int64, device="cuda" if on_device() else "cpu")

@@ -4,7 +4,9 @@ agent.cpp:619-708): once the engine's replay policy says train, the rows of the 
 weights, and the policy is told that the memory was trained on.  Used by agents.ValueSim (online=True) and play_batched --online.
 
 Under a torch.distributed process group (play_batched under torchrun) rank 0's engine holds the memory and the policy: rank 0 copies the rows
-out and broadcasts them into every rank's buffer, and all ranks train data-parallel on them (Model_VV.train_rows)."""
+out and broadcasts them into every rank's buffer, and all ranks train data-parallel on them (Model_VV.train_rows).
+
+CallbackTrainer hands the same rows to a caller-supplied training function instead (OnlineMCTSAgent's train callback, agent.cpp:698)."""
 import os
 import time
 
@@ -36,14 +38,18 @@ class OnlineTrainer:
             self.model._eng.load_weights(self.weights)
         return self.model
 
+    def _peek(self, n_rows):
+        """the first n_rows rows of rank 0's memory -> buf[:n_rows] on every rank, in place when this returns"""
+        if self.rank == 0:
+            self.eng.replay_peek_into(self.buf.data_ptr(), n_rows)  # synchronises the engine's stream
+        distributed.broadcast_rows(self.buf, n_rows)               # world > 1: rank 0's rows on every rank
+
     def train(self, n_rows, current_episode, dump_path=None):
         """Train on the first n_rows rows of the engine's memory (ValueSim.py:176-183 / agent.cpp:697-701).  dump_path: also write them as
         np.savez(dump_path, states=, values=, variance=, weights=) (ValueSim.py:176-177); the host rows are kept in last_rows.  Returns False
         (memory untouched, still collecting) when there are too few rows for a validation split."""
         t0 = time.perf_counter()
-        if self.rank == 0:
-            self.eng.replay_peek_into(self.buf.data_ptr(), n_rows)  # synchronises the engine's stream
-        distributed.broadcast_rows(self.buf, n_rows)               # world > 1: rank 0's rows on every rank
+        self._peek(n_rows)
         self.last_rows = None
         if dump_path and n_rows >= 10 and self.rank == 0:                             # fewer rows leave no validation split: train_rows skips them
             self.last_rows = self.buf[:n_rows].cpu().numpy()
@@ -88,3 +94,88 @@ class OnlineTrainer:
         if self.model is not None:
             self.model.close()
             self.model = None
+
+
+class CallbackTrainer(OnlineTrainer):
+    """OnlineTrainer's interface around the caller's training function: OnlineMCTSAgent(..., train=) (agent.cpp:588-616), called where
+    remove_nodes calls train(m_state, m_value, m_variance, m_visit, memory_index) (agent.cpp:698).
+
+    train(state, value, variance, visit, size) receives the first `size` rows of the memory as the reference's arrays: float32 states
+    [size,1,20,10] and value / variance / visit [size,1].  host=False: contiguous torch tensors on the engine's device, re-laid out from the
+    device rows (replay.rows_to_memory_dev) and valid until the call returns; host=True: numpy arrays (replay.rows_to_memory), so that a
+    ValueSimC-style training() runs as it is.
+
+    external=True (eval_kind "external"): the caller's network searches and the callback updates it in place; it returns None.  Otherwise
+    the engine's own network kernels search, and the callback returns the new weights (a Model_VV state_dict with out_ubound / out_lbound,
+    or a flat float32 array of N_WEIGHTS), which the engine loads, or None to keep the current ones.
+
+    A callback that raises, or weights the engine refuses (wrong form, or out of a tensor-core kind's limits), raise here before the memory
+    is marked trained or the search's weights change.  Under a process group every rank's callback receives rank 0's rows; rank 0's returned
+    weights are broadcast and loaded on every rank.  A caller's network (external) is the caller's to keep in step across ranks."""
+
+    def __init__(self, eng, weights, capacity, train, host=False, external=False):
+        super().__init__(eng, weights, capacity)
+        self.fn, self.host, self.external = train, bool(host), bool(external)
+
+    def train(self, n_rows, current_episode, dump_path=None):
+        import torch
+        t0 = time.perf_counter()
+        self._peek(n_rows)
+        rows = self.buf[:n_rows]
+        self.last_rows = rows.cpu().numpy() if self.host or (dump_path and self.rank == 0) else None
+        if dump_path and self.rank == 0:
+            os.makedirs(os.path.dirname(dump_path) or ".", exist_ok=True)
+            replay.dump(dump_path, self.last_rows)
+        memory = replay.rows_to_memory(self.last_rows) if self.host else replay.rows_to_memory_dev(rows)
+        result = self.fn(*memory, int(n_rows))
+        torch.cuda.synchronize(self.buf.device)                   # the caller's work on torch's streams ends before the engine's stream searches on
+        if self.external and result is not None:
+            raise ValueError("with the caller's evaluator (eval_kind external) the training callback updates that network in place and returns "
+                             "None, not weights")
+        if not self.external:
+            self._load(result)
+        if self.rank == 0:
+            self.eng.replay_policy_trained(current_episode)        # ++n_trains; memory_index = 0; last_training_episode (agent.cpp:699-701)
+        self.n_trains += 1
+        self.train_seconds += time.perf_counter() - t0
+        return True
+
+    def _load(self, result):
+        """rank 0's returned weights into every rank's engine (None: keep them).  Refused weights raise on every rank and change nothing."""
+        code, w, err = 0, None, None                               # 0 keep, 1 load w, 2 refused
+        if self.rank == 0 and result is not None:
+            try:
+                w = weights_vector(result)
+                self.eng.load_weights(w)                           # checks a tensor-core kind's limits before it changes anything
+                code = 1
+            except Exception as exc:                               # noqa: BLE001 (re-raised below, after the other ranks have heard of it)
+                code, err = 2, exc
+        if distributed.rank_world()[1] > 1:
+            code = distributed.broadcast_ints([code])[0]
+            if code == 1:
+                w = distributed.broadcast_weights(w)
+                if self.rank != 0:
+                    self.eng.load_weights(w)
+        if code == 2:
+            raise err if err is not None else ValueError("rank 0's training callback returned weights its engine refused")
+        if code == 1:
+            self.weights = w
+
+
+def weights_vector(w):
+    """A training callback's weights -> the engine's float32 vector: a Model_VV state_dict (model_vv.WEIGHT_KEYS, torch tensors or arrays)
+    or a flat float32 array / tensor of N_WEIGHTS.  Anything else raises ValueError."""
+    import numpy as np
+    from . import _lib as L
+    from .model.model_vv import WEIGHT_KEYS, state_dict_to_weights
+    if hasattr(w, "keys"):
+        missing = [k for k, _shape in WEIGHT_KEYS if k not in w]
+        if missing:
+            raise ValueError("the returned state_dict has no %s" % ", ".join(missing))
+        return state_dict_to_weights(w)
+    if hasattr(w, "detach"):
+        w = w.detach().cpu().numpy()
+    if not isinstance(w, np.ndarray) or w.dtype != np.float32 or w.shape != (L.N_WEIGHTS,):
+        raise ValueError("a training callback returns None, a Model_VV state_dict or float32 weights of shape (%d,); got %s" % (
+            L.N_WEIGHTS, (w.dtype, w.shape) if isinstance(w, np.ndarray) else type(w).__name__))
+    return w.copy()

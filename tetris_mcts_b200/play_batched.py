@@ -26,6 +26,15 @@ deterministic, one game per rank under --online):
 --evaluator MODULE:FACTORY searches with the caller's network instead of the built-in one: FACTORY(device) returns a device evaluator
 (BatchedEngine.run_sims: a torch tensor [n,1,20,10] of boards in, (v, var) out), and the engine runs eval_kind "external".
 
+--trainer MODULE:FACTORY (with --online) trains with the caller's function instead of the built-in trainer (OnlineMCTSAgent's train callback,
+online.CallbackTrainer): FACTORY(device) returns train(state, value, variance, visit, size), called with the memory's first `size` rows as
+float32 torch tensors on the device (--trainer_host: numpy arrays) each time the accumulation policy says train.  With --evaluator it trains
+that network in place and returns None; without, it returns new weights for the built-in network (a Model_VV state_dict or N_WEIGHTS floats),
+or None to keep them:
+
+  python -m tetris_mcts_b200.play_batched --agent_type ValueSimLP --online --evaluator mynets:make_evaluator --trainer mynets:make_trainer --endless
+  python -m tetris_mcts_b200.play_batched --agent_type ValueSimLP --online --eval_kind net_fp16 --trainer mytraining:make_trainer --endless
+
 Flags are play.py's (play.py:46-70) plus --n_parallel / --max_nodes / --device / --watch / --seed and the online agent's memory and training
 settings.  One "episode" is one finished game of any of the parallel games; episodes are numbered in the order (move, game index) they end."""
 import argparse
@@ -222,10 +231,7 @@ def run(args, out=sys.stdout, timing=None):
         elif found[1]:
             raise ValueError(found[1])
     if args.evaluator:
-        import importlib
-        import torch
-        module, factory = args.evaluator.split(":", 1)
-        evaluator = getattr(importlib.import_module(module), factory)(torch.device("cuda", device))
+        evaluator = _factory(args.evaluator)(_torch_device(device))
     elif mode != "vanilla" and resumed is not None:
         weights = resumed["trainer"]["weights"] if resumed["trainer"] else None               # the engine image holds the search's own
     elif mode != "vanilla":
@@ -250,13 +256,17 @@ def run(args, out=sys.stdout, timing=None):
     online = args.online and not args.benchmark and mode != "vanilla"
     trainer, gcs, block = None, 0, None
     if online:                                                                             # ValueSim.py:21-37 memory, min_visits_to_store (25: ValueSimLP.py:11)
-        from .online import OnlineTrainer
+        from .online import CallbackTrainer, OnlineTrainer
         if resumed is None:
             eng.replay_enable(min_visits=25 if mode == "lp" else 10, capacity=args.memory_size)
             if rank == 0:
                 eng.replay_policy(args.accumulation_policy, episodes_per_train=args.episodes_per_train, memory_growth_rate=args.memory_growth_rate)
-        trainer = OnlineTrainer(eng, weights, args.memory_size, batch_size=args.train_batch_size, max_iters=args.train_max_iters,
-                                train_kind=args.train_kind)   # ValueSim.py:180
+        if args.trainer:
+            trainer = CallbackTrainer(eng, weights, args.memory_size, _factory(args.trainer)(_torch_device(device)), host=args.trainer_host,
+                                      external=evaluator is not None)
+        else:
+            trainer = OnlineTrainer(eng, weights, args.memory_size, batch_size=args.train_batch_size, max_iters=args.train_max_iters,
+                                    train_kind=args.train_kind)   # ValueSim.py:180
         if resumed is not None and resumed["trainer"]:
             trainer.restore(resumed["trainer"])
         if world > 1:                                                                      # the rows one move's collections stored on this rank
@@ -345,6 +355,8 @@ def run(args, out=sys.stdout, timing=None):
                     train_now, n = D.broadcast_ints([train_now, n])
                 if train_now:
                     trainer.train(n, ngames)
+                    if args.trainer and rank == 0:
+                        print('Training complete.', **perr)                                   # agent.cpp:702
             last = done or (args.max_moves and moves >= args.max_moves)
             if args.checkpoint_dir and (last or (args.checkpoint_every and moves % args.checkpoint_every == 0)):
                 checkpoint(done)
@@ -363,6 +375,18 @@ def run(args, out=sys.stdout, timing=None):
         if saver:
             saver.close()                                                                   # play.py:183-184
     return ngames, moves, tracker
+
+
+def _factory(spec):
+    """MODULE:FACTORY -> the callable FACTORY of the imported MODULE"""
+    import importlib
+    module, factory = spec.split(":", 1)
+    return getattr(importlib.import_module(module), factory)
+
+
+def _torch_device(device):
+    import torch
+    return torch.device("cuda", device)
 
 
 def _exchange_rows(eng, block, staged, most, rank):
@@ -415,7 +439,13 @@ def parse_args(argv=None):
                         'product, about a third of the tensor-core work (DESIGN §5).  --online trains in fp32 / fp64 either way')
     p.add_argument('--evaluator', default=None, metavar='MODULE:FACTORY',
                    help='search with the caller\'s network: FACTORY(device) returns a device evaluator (boards [n,1,20,10] -> (v, var)); '
-                        'the engine runs eval_kind external.  Not with --online (the trainer trains the built-in network) nor Vanilla')
+                        'the engine runs eval_kind external.  Not with --online unless --trainer trains it, nor with Vanilla')
+    p.add_argument('--trainer', default=None, metavar='MODULE:FACTORY',
+                   help='--online: train with the caller\'s function instead of the built-in trainer: FACTORY(device) returns '
+                        'train(state, value, variance, visit, size), which trains the --evaluator network in place and returns None, or '
+                        'returns new weights for the built-in network (a Model_VV state_dict or N_WEIGHTS floats) or None')
+    p.add_argument('--trainer_host', default=False, action='store_true',
+                   help='hand --trainer numpy arrays instead of torch tensors on the device')
     p.add_argument('--max_moves', default=0, type=int, help='stop after this many moves (counted from the start of the run, across --resume)')
     p.add_argument('--checkpoint_dir', default=None, help='write checkpoints here (one engine image per rank and the run state)')
     p.add_argument('--checkpoint_every', default=0, type=int, help='moves between checkpoints; 0 = only when the run ends')
@@ -423,7 +453,23 @@ def parse_args(argv=None):
     p.add_argument('--dist_backend', default='nccl', choices=('nccl', 'gloo'),
                    help='under torchrun: collectives over NCCL (one GPU per rank), or gloo through the host (several ranks may share a GPU)')
     args = p.parse_args(argv)
-    if args.evaluator and args.online:
+    if args.trainer:
+        if not args.online:
+            p.error('--trainer needs --online: it is called when the online accumulation policy says train')
+        if args.agent_type == 'Vanilla':
+            p.error('--trainer cannot be combined with --agent_type Vanilla: Vanilla has no value network to train')
+        if ':' not in args.trainer:
+            p.error('--trainer takes MODULE:FACTORY')
+        if args.checkpoint_dir:
+            p.error('--checkpoint_dir cannot be combined with --trainer: the caller\'s training state is not part of the checkpoint')
+        given = _given_flags(p, argv)
+        clash = [f for f in ('train_kind', 'train_batch_size', 'train_max_iters') if f in given]
+        if clash:
+            p.error('--trainer cannot be combined with %s: they set the built-in trainer, which --trainer replaces'
+                    % ', '.join('--' + f for f in clash))
+    if args.trainer_host and not args.trainer:
+        p.error('--trainer_host needs --trainer')
+    if args.evaluator and args.online and not args.trainer:
         p.error('--evaluator cannot be combined with --online: the online trainer trains the built-in Model_VV weights')
     if args.evaluator and args.agent_type == 'Vanilla':
         p.error('--evaluator cannot be combined with --agent_type Vanilla: Vanilla evaluates leaves by random rollout')
@@ -436,6 +482,13 @@ def parse_args(argv=None):
     if args.checkpoint_every < 0:
         p.error('--checkpoint_every takes a number of moves >= 0')
     return args
+
+
+def _given_flags(p, argv):
+    """the destinations of the flags argv sets itself (abbreviations included), whatever their values"""
+    for a in p._actions:
+        a.default = argparse.SUPPRESS
+    return set(vars(p.parse_args(argv)))
 
 
 def main(argv=None, out=sys.stdout):

@@ -18,6 +18,18 @@ def rows_to_memory(rows):
     return [states, tail[:, 0:1].copy(), tail[:, 1:2].copy(), tail[:, 2:3].copy()]
 
 
+def rows_to_memory_dev(rows):
+    """The torch form of rows_to_memory: rows uint8 tensor [n, 212] (any device) -> four contiguous float32 tensors on that device, states
+    [n,1,20,10] and value / variance / visit [n,1], bit for bit the arrays rows_to_memory returns.  Issued on torch's current stream."""
+    import torch
+    rows = rows.reshape(-1, SAMPLE_BYTES)
+    n = rows.shape[0]
+    states = rows[:, :200].view(torch.int8).to(torch.float32).reshape(n, 1, 20, 10)
+    tail = rows[:, 200:212].contiguous().view(torch.float32)
+    col = lambda j: tail[:, j:j + 1].clone(memory_format=torch.contiguous_format)    # noqa: E731
+    return [states.contiguous(), col(0), col(1), col(2)]
+
+
 def memory_to_rows(states, values, variance, weights):
     """The inverse (e.g. to feed samples stored by the reference into the all-gather format)."""
     n = len(states)
