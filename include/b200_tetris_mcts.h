@@ -55,10 +55,16 @@ enum { B200_EVAL_SYNTHETIC = 0, /* test evaluator (hash of the observation), sha
                                    only in B200_MODE_DIST (b200_engine_create returns B200_ERR_BAD_ARG otherwise: net_fp16 is the value
                                    network's one-term kind); b200_load_weights returns B200_ERR_BAD_ARG (no value network);
                                    b200_load_dist_weights takes the weight limits of B200_EVAL_NET_TC. */
-       B200_EVAL_EXTERNAL = 5 }; /* the caller's evaluator (OnlineMCTSAgent(..., evaluator=, evaluation_type=0), agents/cppmodule/agent.cpp:
+       B200_EVAL_EXTERNAL = 5,  /* the caller's evaluator (OnlineMCTSAgent(..., evaluator=, evaluation_type=0), agents/cppmodule/agent.cpp:
                                    423-436; ValueSimLP.mcts' self.model.inference, agents/ValueSimLP.py:55-60): each simulation step is driven
                                    with b200_ext_step_begin / b200_ext_step_end below.  B200_MODE_LP, B200_MODE_SINGLE and B200_MODE_DIST
                                    (b200_engine_create returns B200_ERR_BAD_ARG in B200_MODE_VANILLA, whose evaluator is the rollout). */
+       B200_EVAL_EXTERNAL_GAME = 6 }; /* the caller's leaf-GAME evaluator (MCTSAgent(..., evaluator, evaluation_type=1), agent.cpp:449-455;
+                                   VanillaC's random_playout): in place of the rollout, each step hands the expanded leaf of every game as a
+                                   packed record to the caller, whose (value, variance) is backed up as it is (value not added to the leaf's
+                                   score, variance in place of rollout_variance).  Driven with b200_ext_step_begin(B200_BOARD_RECORD) /
+                                   b200_ext_step_end.  B200_MODE_VANILLA only (b200_engine_create returns B200_ERR_BAD_ARG otherwise).
+                                   Counter 5 (rollout steps) stays 0; counter 2 counts the leaves handed out. */
 
 typedef struct b200_engine b200_engine;
 
@@ -150,7 +156,8 @@ int b200_set_path_cache(b200_engine *e, int on);
 /* --- TreeAgent.mcts (agents/ValueSimLP.py:13, ValueSim.py:52, Vanilla.py:17): `sims` simulations on every game */
 int b200_run_sims(b200_engine *e, int sims);
 
-/* --- the caller's evaluator (B200_EVAL_EXTERNAL): one simulation step of every game in two halves around the caller's network.
+/* --- the caller's evaluator (B200_EVAL_EXTERNAL, B200_EVAL_EXTERNAL_GAME): one simulation step of every game in two halves around the
+ *   caller's network or leaf-game function.
  *   b200_ext_capacity: max_rows = the most rows one step hands out (7 * n_games in B200_MODE_LP, n_games otherwise); out_cols = 2 (v, var),
  *     or dist_bins in B200_MODE_DIST.
  *   b200_ext_step_begin: select + expand and the collections of one step (the code b200_run_sims runs), then this step's evaluation
@@ -170,8 +177,13 @@ int b200_run_sims(b200_engine *e, int sims);
  *   b200_load_dist_weights, b200_valuenet_forward, b200_distnet_forward and the b200_debug_* network readers; b200_set_deep_lane is
  *   ignored; counter 12 is the longest trace since the engine was created (only b200_run_sims resets it).  The kernels of the split
  *   count under phase 6 of b200_phase_ms. */
+/*   B200_EVAL_EXTERNAL_GAME: max_rows = n_games, out_cols = 2.  b200_ext_step_begin takes board_dtype B200_BOARD_RECORD (the only dtype it
+ *     takes; an external engine refuses it) and writes into boards_dev (DEVICE, 16-byte aligned) uint32 [n_games][20] the packed record
+ *     (SPEC_PYTETRIS §6) of the leaf of every game whose step expanded one (the games the rollout would play out), in ascending game
+ *     order; ids_dev[row] = the game.  b200_ext_step_end takes [n_rows][2] fp32 (value, variance) per row. */
 #define B200_BOARD_INT8 0
 #define B200_BOARD_F32 1
+#define B200_BOARD_RECORD 2
 int b200_ext_capacity(b200_engine *e, int32_t *max_rows, int32_t *out_cols);
 int b200_ext_step_begin(b200_engine *e, void *boards_dev, int board_dtype, int32_t *ids_dev, int32_t *n_rows);
 int b200_ext_step_end(b200_engine *e, const float *out_dev);
@@ -215,6 +227,19 @@ int b200_valuenet_forward(b200_engine *e, const int8_t *states, int k, float *v,
 int b200_tetris_new(uint32_t *recs, int n, int actions_per_drop, int scoring, int randomizer, const uint32_t *seeds, int reset);
 int b200_tetris_step(uint32_t *recs, const int32_t *actions, int n);
 int b200_tetris_state(const uint32_t *recs, int8_t *out, int n);
+/* --- the same on DEVICE records owned by the caller (e.g. the leaf games of B200_EVAL_EXTERNAL_GAME), for a leaf evaluator that runs at
+ *     device speed.  Unlike the engine's `_dev` calls these are ASYNCHRONOUS: each only enqueues its kernel on `stream` (a cudaStream_t
+ *     passed as void*; NULL = the legacy default stream) and returns; order the caller's work against that stream.  recs_dev is
+ *     uint32 [n][20], 16-byte aligned; n = 0 is a no-op.  No engine is involved.
+ *   b200_tetris_step_dev: one Tetris.play per record, in place; action ids outside 0..6 move nothing (SPEC §3: gravity still ticks).
+ *   b200_tetris_state_dev: getState() as int8 (B200_BOARD_INT8) or float32 (B200_BOARD_F32) [n][1][20][10]: the board bits and -1 on the
+ *     four falling-piece cells, the boards B200_EVAL_EXTERNAL hands out.
+ *   b200_tetris_playout_dev: random playouts (the rollout's loop): row i plays xorshift32(rng_dev[i]) % n_actions (1..8; 8 includes the
+ *     no-op 7, VanillaC's randint(0, 7)) until its game is over or after max_steps (>= 0) actions.  The final record and stream are written
+ *     back (a stream of 0 starts as 0x2545F491); steps_dev[i] (may be NULL) = the actions played. */
+int b200_tetris_step_dev(uint32_t *recs_dev, const int32_t *actions_dev, int n, void *stream);
+int b200_tetris_state_dev(const uint32_t *recs_dev, void *out_dev, int dtype, int n, void *stream);
+int b200_tetris_playout_dev(uint32_t *recs_dev, uint32_t *rng_dev, int n, int n_actions, int max_steps, int32_t *steps_dev, void *stream);
 
 /* --- single-call twins of agents/cppmodule/core.cpp:20-26 on the reference's own arrays (mutated in place) */
 int b200_select_trace_obs(int index, const int32_t *child, const int32_t *visit, const float *value,

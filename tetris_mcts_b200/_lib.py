@@ -14,8 +14,8 @@ N_ACTIONS = 7
 N_WEIGHTS = 478342
 
 MODE_LP, MODE_SINGLE, MODE_VANILLA, MODE_DIST = 0, 1, 2, 3
-EVAL_SYNTHETIC, EVAL_NET, EVAL_NET_TC, EVAL_NET_FP16, EVAL_DIST_FP16, EVAL_EXTERNAL = 0, 1, 2, 3, 4, 5
-BOARD_INT8, BOARD_F32 = 0, 1
+EVAL_SYNTHETIC, EVAL_NET, EVAL_NET_TC, EVAL_NET_FP16, EVAL_DIST_FP16, EVAL_EXTERNAL, EVAL_EXTERNAL_GAME = 0, 1, 2, 3, 4, 5, 6
+BOARD_INT8, BOARD_F32, BOARD_RECORD = 0, 1, 2
 ERR_NAMES = {1: "BAD_ARG", 2: "CUDA", 3: "ARENA_FULL", 4: "TRACE_FULL", 5: "NO_WEIGHTS"}
 
 
@@ -76,6 +76,9 @@ def lib():
         L.b200_tetris_step.argtypes = [P, P, C.c_int]
         L.b200_tetris_new.argtypes = [P, C.c_int, C.c_int, C.c_int, C.c_int, P, C.c_int]
         L.b200_tetris_state.argtypes = [P, P, C.c_int]
+        L.b200_tetris_step_dev.argtypes = [P, P, C.c_int, P]
+        L.b200_tetris_state_dev.argtypes = [P, P, C.c_int, C.c_int, P]
+        L.b200_tetris_playout_dev.argtypes = [P, P, C.c_int, C.c_int, C.c_int, P, P]
         L.b200_select_trace_obs.argtypes = [C.c_int] + [P] * 6 + [C.c_int, C.c_int, P, P, C.c_int, P]
         L.b200_backup_trace_obs.argtypes = [P, C.c_int] + [P] * 5 + [C.c_int, C.c_double, C.c_double, C.c_double]
         L.b200_backup_trace_obs_LP.argtypes = ([P, C.c_int] + [P] * 6 + [C.c_int, P, P, C.c_int, P, P, C.c_double,

@@ -84,14 +84,19 @@ struct b200_engine {
     int gc_pool_main = 0;          // collection scratch sets of the main k_gc launch; DEEP_GC_BLOCKS more follow for the deep lane's
     cudaGraphExec_t step_exec = nullptr; bool step_graph_failed = false;
     uint64_t step_launches[PH_N] = {0};
-    // caller-supplied evaluator (B200_EVAL_EXTERNAL): k_ext_order's marks and ordered rows; ext_open between b200_ext_step_begin and _end
+    // caller-supplied evaluator (B200_EVAL_EXTERNAL): k_ext_order's marks and ordered rows ({game, leaf} per game with
+    // B200_EVAL_EXTERNAL_GAME); ext_open between b200_ext_step_begin and _end
     int32_t *d_ext_mark = nullptr, *d_ext_n = nullptr; uint2 *d_ext_rows = nullptr;
     bool ext_open = false; int32_t ext_rows = 0;
 };
 
-static bool ext_kind(const b200_engine *e) { return e->cfg.eval_kind == B200_EVAL_EXTERNAL; }
+static bool ext_game_kind(const b200_engine *e) { return e->cfg.eval_kind == B200_EVAL_EXTERNAL_GAME; }
+static bool ext_kind(const b200_engine *e) { return e->cfg.eval_kind == B200_EVAL_EXTERNAL || ext_game_kind(e); }
 // the calls an external engine has no use for (it has no network of its own, and its steps need the caller's outputs)
 static int ext_refuse(const b200_engine *e, const char *fn) {
+    if (ext_game_kind(e))
+        return fail(B200_ERR_BAD_ARG, std::string(fn) + ": eval_kind external_game has no built-in evaluator; drive the search with "
+                                      "b200_ext_step_begin / b200_ext_step_end");
     return fail(B200_ERR_BAD_ARG, std::string(fn) + ": eval_kind external has no built-in network; drive the search with "
                                   "b200_ext_step_begin / b200_ext_step_end");
 }
@@ -210,6 +215,9 @@ extern "C" int b200_engine_create(const b200_config *cfg, b200_engine **out) {
         return fail(B200_ERR_BAD_ARG, "eval_kind net_fp16 has no distributional network: use net_tc or net in B200_MODE_DIST");
     if (cfg->mode == MODE_VANILLA && cfg->eval_kind == B200_EVAL_EXTERNAL)
         return fail(B200_ERR_BAD_ARG, "eval_kind external needs B200_MODE_LP, B200_MODE_SINGLE or B200_MODE_DIST (Vanilla evaluates by rollout)");
+    if (cfg->mode != MODE_VANILLA && cfg->eval_kind == B200_EVAL_EXTERNAL_GAME)
+        return fail(B200_ERR_BAD_ARG, "eval_kind external_game evaluates leaf games and needs B200_MODE_VANILLA: use eval_kind external "
+                                      "for a board evaluator in B200_MODE_LP, B200_MODE_SINGLE or B200_MODE_DIST");
     if (cfg->mode != MODE_DIST && cfg->eval_kind == B200_EVAL_DIST_FP16)
         return fail(B200_ERR_BAD_ARG, "eval_kind dist_fp16 is the distributional network's one-term form and needs B200_MODE_DIST: "
                                       "use net_fp16 for the value network");
@@ -262,6 +270,9 @@ extern "C" int b200_engine_create(const b200_config *cfg, b200_engine **out) {
     }
     if (cfg->eval_kind == B200_EVAL_EXTERNAL) {
         rc |= dalloc(e, &e->d_ext_mark, G * 8); rc |= dalloc(e, &e->d_ext_rows, G * 8); rc |= dalloc(e, &e->d_ext_n, 1);
+    }
+    if (cfg->eval_kind == B200_EVAL_EXTERNAL_GAME) {
+        rc |= dalloc(e, &e->d_ext_rows, G); rc |= dalloc(e, &e->d_ext_n, 1); rc |= dalloc(e, &A.rollout_var, G);
     }
     rc |= dalloc(e, &e->d_default_rec, REC_WORDS);
     rc |= dalloc(e, &e->d_stats, G * 21); rc |= dalloc(e, &e->d_action, G);
@@ -870,16 +881,24 @@ extern "C" int b200_run_sims(b200_engine *e, int sims) {
 extern "C" int b200_ext_capacity(b200_engine *e, int32_t *max_rows, int32_t *out_cols) {
     if (!e || !max_rows || !out_cols) return fail(B200_ERR_BAD_ARG, "null argument");
     if (!ext_kind(e)) return fail(B200_ERR_BAD_ARG, "b200_ext_capacity: the engine's eval_kind is not external");
-    *max_rows = e->A.G * (e->A.mode == MODE_LP ? 7 : 1);
+    *max_rows = e->A.G * (e->A.mode == MODE_LP ? 7 : 1);   // external_game: Vanilla, one leaf per game
     *out_cols = e->A.mode == MODE_DIST ? e->A.dist_bins : 2;
     return B200_OK;
 }
 
-// The first half of one simulation step (the same code as b200_run_sims'), then this step's requests in (game, slot) order as boards.
+// The first half of one simulation step (the same code as b200_run_sims'), then this step's requests in (game, slot) order as boards
+// (external) or the leaf games in game order as packed records (external_game).
 extern "C" int b200_ext_step_begin(b200_engine *e, void *boards_dev, int board_dtype, int32_t *ids_dev, int32_t *n_rows) {
-    if (!e || !boards_dev || !n_rows || (board_dtype != B200_BOARD_INT8 && board_dtype != B200_BOARD_F32))
-        return fail(B200_ERR_BAD_ARG, "bad argument (boards_dev and n_rows non-NULL, board_dtype B200_BOARD_INT8 or B200_BOARD_F32)");
+    if (!e || !boards_dev || !n_rows || (board_dtype != B200_BOARD_INT8 && board_dtype != B200_BOARD_F32 && board_dtype != B200_BOARD_RECORD))
+        return fail(B200_ERR_BAD_ARG, "bad argument (boards_dev and n_rows non-NULL, board_dtype B200_BOARD_INT8, B200_BOARD_F32 or B200_BOARD_RECORD)");
     if (!ext_kind(e)) return fail(B200_ERR_BAD_ARG, "b200_ext_step_begin: the engine's eval_kind is not external (use b200_run_sims)");
+    if (ext_game_kind(e) && board_dtype != B200_BOARD_RECORD)
+        return fail(B200_ERR_BAD_ARG, "b200_ext_step_begin: an external_game engine hands out leaf games: board_dtype B200_BOARD_RECORD");
+    if (!ext_game_kind(e) && board_dtype == B200_BOARD_RECORD)
+        return fail(B200_ERR_BAD_ARG, "b200_ext_step_begin: an external engine hands out boards: board_dtype B200_BOARD_INT8 or B200_BOARD_F32 "
+                                      "(B200_BOARD_RECORD is eval_kind external_game's)");
+    if (ext_game_kind(e) && ((uintptr_t)boards_dev & 15))
+        return fail(B200_ERR_BAD_ARG, "b200_ext_step_begin: the record buffer must be 16-byte aligned");
     if (e->ext_open) return fail(B200_ERR_BAD_ARG, "b200_ext_step_begin: a step is already open; finish it with b200_ext_step_end");
     CK(cudaSetDevice(e->cfg.device));
     const Arena &A = e->A;
@@ -888,9 +907,14 @@ extern "C" int b200_ext_step_begin(b200_engine *e, void *boards_dev, int board_d
     {
         PhaseTimer t(e, PH_MISC);
         const int grid = e->n_sm * 4;
-        k_ext_order<<<1, EXT_ORDER_THREADS, 0, e->stream>>>(A, e->d_ext_mark, e->d_ext_rows, e->d_ext_n);
-        if (board_dtype == B200_BOARD_INT8) k_ext_boards<int8_t><<<grid, 256, 0, e->stream>>>(A, e->d_ext_rows, e->d_ext_n, (int8_t *)boards_dev, ids_dev);
-        else k_ext_boards<float><<<grid, 256, 0, e->stream>>>(A, e->d_ext_rows, e->d_ext_n, (float *)boards_dev, ids_dev);
+        if (ext_game_kind(e)) {
+            k_ext_leaf_order<<<1, EXT_ORDER_THREADS, 0, e->stream>>>(A, e->d_ext_rows, e->d_ext_n);
+            k_ext_leaf_records<<<grid, 256, 0, e->stream>>>(A, e->d_ext_rows, e->d_ext_n, (uint32_t *)boards_dev, ids_dev);
+        } else {
+            k_ext_order<<<1, EXT_ORDER_THREADS, 0, e->stream>>>(A, e->d_ext_mark, e->d_ext_rows, e->d_ext_n);
+            if (board_dtype == B200_BOARD_INT8) k_ext_boards<int8_t><<<grid, 256, 0, e->stream>>>(A, e->d_ext_rows, e->d_ext_n, (int8_t *)boards_dev, ids_dev);
+            else k_ext_boards<float><<<grid, 256, 0, e->stream>>>(A, e->d_ext_rows, e->d_ext_n, (float *)boards_dev, ids_dev);
+        }
     }
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(&e->ext_rows, e->d_ext_n, sizeof(int32_t), cudaMemcpyDeviceToHost, e->stream));
@@ -911,9 +935,10 @@ extern "C" int b200_ext_step_end(b200_engine *e, const float *out_dev) {
     if (e->ext_rows > 0) {
         PhaseTimer t(e, PH_MISC);
         const int cols = A.mode == MODE_DIST ? A.dist_bins : 2;
-        const long long work = (long long)e->ext_rows * cols;
+        const long long work = ext_game_kind(e) ? e->ext_rows : (long long)e->ext_rows * cols;
         const int grid = (int)std::min<long long>((work + 255) / 256, (long long)e->n_sm * 4);
-        k_ext_scatter<<<grid, 256, 0, e->stream>>>(A, e->d_ext_rows, e->d_ext_n, out_dev, cols);
+        if (ext_game_kind(e)) k_ext_leaf_scatter<<<grid, 256, 0, e->stream>>>(A, e->d_ext_rows, e->d_ext_n, out_dev);
+        else k_ext_scatter<<<grid, 256, 0, e->stream>>>(A, e->d_ext_rows, e->d_ext_n, out_dev, cols);
     }
     step_backup(e);
     CK(cudaGetLastError());
@@ -1384,6 +1409,45 @@ extern "C" int b200_tetris_step(uint32_t *recs, const int32_t *actions, int n) {
 extern "C" int b200_tetris_state(const uint32_t *recs, int8_t *out, int n) {
     if (!recs || !out || n < 1) return fail(B200_ERR_BAD_ARG, "bad argument");
     return env_stream_op(const_cast<uint32_t *>(recs), nullptr, out, n);
+}
+
+// ---------------------------------------------------------------------------------------------------- caller-owned device games
+// Tetris.play / getState / random playouts on DEVICE records, asynchronous on the caller's stream (no engine, no copy, no synchronisation).
+static int dev_games_arg(const void *recs_dev, int n, const char *fn) {
+    if ((!recs_dev && n > 0) || n < 0) return fail(B200_ERR_BAD_ARG, std::string(fn) + ": recs_dev non-NULL and n >= 0");
+    if ((uintptr_t)recs_dev & 15) return fail(B200_ERR_BAD_ARG, std::string(fn) + ": recs_dev must be 16-byte aligned");
+    return B200_OK;
+}
+
+extern "C" int b200_tetris_step_dev(uint32_t *recs_dev, const int32_t *actions_dev, int n, void *stream) {
+    if (int rc = dev_games_arg(recs_dev, n, "b200_tetris_step_dev")) return rc;
+    if (!actions_dev && n > 0) return fail(B200_ERR_BAD_ARG, "b200_tetris_step_dev: actions_dev is NULL");
+    if (n == 0) return B200_OK;
+    k_env_step<<<(n + 127) / 128, 128, 0, (cudaStream_t)stream>>>(recs_dev, actions_dev, n);
+    CK(cudaGetLastError());
+    return B200_OK;
+}
+
+extern "C" int b200_tetris_state_dev(const uint32_t *recs_dev, void *out_dev, int dtype, int n, void *stream) {
+    if (int rc = dev_games_arg(recs_dev, n, "b200_tetris_state_dev")) return rc;
+    if ((!out_dev && n > 0) || (dtype != B200_BOARD_INT8 && dtype != B200_BOARD_F32))
+        return fail(B200_ERR_BAD_ARG, "b200_tetris_state_dev: out_dev non-NULL, dtype B200_BOARD_INT8 or B200_BOARD_F32");
+    if (n == 0) return B200_OK;
+    const int grid = (n + GAME_STATE_THREADS - 1) / GAME_STATE_THREADS;
+    if (dtype == B200_BOARD_INT8) k_game_state<int8_t><<<grid, GAME_STATE_THREADS, 0, (cudaStream_t)stream>>>(recs_dev, (int8_t *)out_dev, n);
+    else k_game_state<float><<<grid, GAME_STATE_THREADS, 0, (cudaStream_t)stream>>>(recs_dev, (float *)out_dev, n);
+    CK(cudaGetLastError());
+    return B200_OK;
+}
+
+extern "C" int b200_tetris_playout_dev(uint32_t *recs_dev, uint32_t *rng_dev, int n, int n_actions, int max_steps, int32_t *steps_dev, void *stream) {
+    if (int rc = dev_games_arg(recs_dev, n, "b200_tetris_playout_dev")) return rc;
+    if ((!rng_dev && n > 0) || n_actions < 1 || n_actions > 8 || max_steps < 0)
+        return fail(B200_ERR_BAD_ARG, "b200_tetris_playout_dev: rng_dev non-NULL, 1 <= n_actions <= 8, max_steps >= 0");
+    if (n == 0) return B200_OK;
+    k_game_playout<<<(n + 127) / 128, 128, 0, (cudaStream_t)stream>>>(recs_dev, rng_dev, n, n_actions, max_steps, steps_dev);
+    CK(cudaGetLastError());
+    return B200_OK;
 }
 
 // test aids on trees given in the reference's layout (agents/agent.py:58-88): every child id and observation id within [0, M)

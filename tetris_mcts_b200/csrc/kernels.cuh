@@ -680,7 +680,8 @@ __device__ __forceinline__ void backup_game(const Arena &A, int g, int lane, uns
             var = (double)e.y;
         }
     } else if (kind == LEAF_EXPANDED) {
-        v = (double)A.rollout_val[g]; var = A.rollout_variance;                // Vanilla.py:53-54
+        v = (double)A.rollout_val[g];                                          // Vanilla.py:53-54; agent.cpp:449-455 (evaluator type 1)
+        var = A.rollout_var ? (double)A.rollout_var[g] : A.rollout_variance;
     }
     // ---- core.h:244-259 along the trace, 32 levels per round
     for (int top = D - 1; top >= 0; top -= 32) {

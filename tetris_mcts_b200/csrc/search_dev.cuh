@@ -71,6 +71,7 @@ struct Arena {
     int32_t *fin_log; int32_t *fin_count; int fin_cap;
     float2 *eval_out;              // [G][8] (value, variance) per child slot; slot 7 = the leaf itself
     float *rollout_val;            // [G]
+    float *rollout_var;            // [G] the caller's leaf variances (B200_EVAL_EXTERNAL_GAME); nullptr: every leaf gets rollout_variance
     // distributional mode (agents/core_distributional.py; BASELINE config 5): node-indexed statistics and value histograms
     float *nstat; float *ndist; float *dist_eval; int dist_bins; double dist_vmin, dist_vmax;   // [G][M][8], [G][M][bins], [G][bins]
     // lanes (b200_set_deep_lane): the select / collect / resume kernels of a lane work on the games glist[0 .. *n_list); nullptr: every game

@@ -20,7 +20,7 @@ class BatchedEngine:
                  dist_weights=None, path_cache=None):
         mode_id = {"lp": L.MODE_LP, "single": L.MODE_SINGLE, "vanilla": L.MODE_VANILLA, "dist": L.MODE_DIST}[mode] if isinstance(mode, str) else int(mode)
         eval_id = {"synthetic": L.EVAL_SYNTHETIC, "net": L.EVAL_NET, "net_tc": L.EVAL_NET_TC, "net_fp16": L.EVAL_NET_FP16,
-                   "dist_fp16": L.EVAL_DIST_FP16, "external": L.EVAL_EXTERNAL}[eval_kind] if isinstance(eval_kind, str) else int(eval_kind)
+                   "dist_fp16": L.EVAL_DIST_FP16, "external": L.EVAL_EXTERNAL, "external_game": L.EVAL_EXTERNAL_GAME}[eval_kind] if isinstance(eval_kind, str) else int(eval_kind)
         if tuple(env_args[0]) != (20, 10):
             raise ValueError("only 20x10 boards (SPEC_PYTETRIS.md §1)")
         cfg = L.Config()
@@ -152,12 +152,23 @@ class BatchedEngine:
     def update_root(self, auto_reset=False):
         L.check(L.lib().b200_update_root(self.h, int(auto_reset)))
 
-    def run_sims(self, sims, evaluator=None, board_dtype="float32", host=False):
+    def run_sims(self, sims, evaluator=None, board_dtype="float32", host=False, game_evaluator=None):
         """`sims` simulation steps of every game.  evaluator (eval_kind "external" only) evaluates each step's boards:
         host=False: evaluator(boards) gets a torch tensor [n,1,20,10] (board_dtype "float32" or "int8") on the engine's device, called on
         the engine's stream, and returns (v, var) each [n] or [n,1] (in mode "dist": [n, atoms], or a list of one such), float32 on that
         device; the outputs go to the engine without a host round trip.  host=True: the reference's callback, evaluator(int8 ndarray
-        [n,1,20,10]) -> [v (n,1), var (n,1)] or [probs (n, atoms)] as numpy float32 (Model_VV.inference as it is)."""
+        [n,1,20,10]) -> [v (n,1), var (n,1)] or [probs (n, atoms)] as numpy float32 (Model_VV.inference as it is).
+        game_evaluator (eval_kind "external_game" only, mode "vanilla") evaluates each step's expanded leaf games in place of the rollout:
+        host=False: game_evaluator(recs) gets an int32 view [n,20] of the leaves' packed records (SPEC_PYTETRIS §6; pyTetris.step_games_dev,
+        states_of_dev, playout_dev and record_fields work on it) on the engine's device, called on the engine's stream, and returns (v, var)
+        each [n] or [n,1] float32 on that device.  host=True: numpy uint32 [n,20] in, numpy float32 out (pyTetris.per_game wraps a
+        reference-style f(Tetris)).  The value is backed up as it is (not added to the leaf's score), as agent.cpp's evaluator type 1 does."""
+        if game_evaluator is not None:
+            if evaluator is not None:
+                raise ValueError("pass evaluator (eval_kind external) or game_evaluator (eval_kind external_game), not both")
+            for _ in range(int(sims)):
+                self._ext_step(game_evaluator, "record", host)
+            return
         if evaluator is None:
             L.check(L.lib().b200_run_sims(self.h, int(sims)))
             return
@@ -174,11 +185,12 @@ class BatchedEngine:
         a = None if actions is None else np.ascontiguousarray(actions, np.int32)
         L.check(L.lib().b200_env_step(self.h, L.ptr(a)))
 
-    def play_move(self, sims, auto_reset=True, want_stats=True, evaluator=None, board_dtype="float32", host=False):
-        """One move of play.py:118-177 for every game. Returns (actions, stats).  evaluator / board_dtype / host: see run_sims (eval_kind
-        "external"); the move is then run_sims, get_stats, env_step, update_root, as b200_play_move does it."""
-        if evaluator is not None:
-            self.run_sims(sims, evaluator, board_dtype, host)
+    def play_move(self, sims, auto_reset=True, want_stats=True, evaluator=None, board_dtype="float32", host=False, game_evaluator=None):
+        """One move of play.py:118-177 for every game. Returns (actions, stats).  evaluator / board_dtype / host / game_evaluator: see
+        run_sims (eval_kind "external" / "external_game"); the move is then run_sims, get_stats, env_step, update_root, as b200_play_move
+        does it."""
+        if evaluator is not None or game_evaluator is not None:
+            self.run_sims(sims, evaluator, board_dtype, host, game_evaluator)
             stats, actions = self.get_stats()
             self.env_step(None)
             self.update_root(auto_reset)
@@ -278,15 +290,17 @@ class BatchedEngine:
 
     # ------------------------------------------------------------------ the caller's evaluator (eval_kind "external")
     def ext_capacity(self):
-        """(max_rows, out_cols): the most boards one step hands out (7 * n_games in LP, n_games otherwise) and the outputs per board
-        (2 = v, var; dist_bins in mode "dist")."""
+        """(max_rows, out_cols): the most boards (or leaf records) one step hands out (7 * n_games in LP, n_games otherwise) and the outputs
+        per row (2 = v, var; dist_bins in mode "dist")."""
         rows, cols = np.zeros(1, np.int32), np.zeros(1, np.int32)
         L.check(L.lib().b200_ext_capacity(self.h, L.ptr(rows), L.ptr(cols)))
         return int(rows[0]), int(cols[0])
 
     def ext_step_begin(self, boards, board_dtype="float32", ids=None):
         """First half of one simulation step: boards (a DEVICE tensor or pointer of max_rows * 200 elements) receive this step's boards in
-        ascending (game, slot) order; ids (optional, int32 DEVICE) = game * 8 + slot of each row.  Synchronises; returns n_rows."""
+        ascending (game, slot) order; ids (optional, int32 DEVICE) = game * 8 + slot of each row.  Synchronises; returns n_rows.
+        eval_kind "external_game": board_dtype "record", boards = max_rows * 20 words (16-byte aligned) receive the expanded leaves' packed
+        records in ascending game order, ids = the game of each row."""
         n = np.zeros(1, np.int32)
         L.check(L.lib().b200_ext_step_begin(self.h, C.c_void_p(_dev_ptr(boards)), _BOARD_DTYPES[board_dtype],
                                             None if ids is None else C.c_void_p(_dev_ptr(ids)), L.ptr(n)))
@@ -305,7 +319,9 @@ class BatchedEngine:
                              out=torch.empty((rows, cols), dtype=torch.float32, device=dev))
         ext = self._ext
         if board_dtype not in ext["boards"]:
-            ext["boards"][board_dtype] = torch.empty((ext["rows"], 1, 20, 10), dtype=getattr(torch, board_dtype), device=ext["device"])
+            shape = (ext["rows"], L.REC_WORDS) if board_dtype == "record" else (ext["rows"], 1, 20, 10)
+            ext["boards"][board_dtype] = torch.empty(shape, dtype=torch.int32 if board_dtype == "record" else getattr(torch, board_dtype),
+                                                     device=ext["device"])
         if ext["stream"] is None:
             ext["stream"] = torch.cuda.ExternalStream(self.get_stream(), device=ext["device"])
         return ext
@@ -321,7 +337,8 @@ class BatchedEngine:
             dist = self.mode == L.MODE_DIST
             with torch.cuda.stream(ext["stream"]):
                 if host:
-                    parts = ext_output_parts(evaluator(boards[:n].cpu().numpy()), n, ext["cols"], dist, host=True)
+                    rows = boards[:n].cpu().numpy()
+                    parts = ext_output_parts(evaluator(rows.view(np.uint32) if board_dtype == "record" else rows), n, ext["cols"], dist, host=True)
                     parts = [torch.from_numpy(p) for p in parts]
                 else:
                     parts = ext_output_parts(evaluator(boards[:n]), n, ext["cols"], dist, device=ext["device"])
@@ -421,7 +438,7 @@ def read_image_fields(path):
         return out
 
 
-_BOARD_DTYPES = {"int8": L.BOARD_INT8, "float32": L.BOARD_F32}
+_BOARD_DTYPES = {"int8": L.BOARD_INT8, "float32": L.BOARD_F32, "record": L.BOARD_RECORD}
 
 
 def _dev_ptr(x):

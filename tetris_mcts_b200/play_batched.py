@@ -35,6 +35,14 @@ or None to keep them:
   python -m tetris_mcts_b200.play_batched --agent_type ValueSimLP --online --evaluator mynets:make_evaluator --trainer mynets:make_trainer --endless
   python -m tetris_mcts_b200.play_batched --agent_type ValueSimLP --online --eval_kind net_fp16 --trainer mytraining:make_trainer --endless
 
+--agent_type VanillaC is the C++ agent's rollout search (agents/VanillaC.py): check_low with low=1 and the leaf game scored by one random
+playout over all eight action ids, backed up as (score, 1e5); the engine runs eval_kind "external_game".  --game_evaluator MODULE:FACTORY
+(Vanilla or VanillaC) scores each step's leaf games with the caller's function instead: FACTORY(device) returns a device game evaluator
+(BatchedEngine.run_sims: int32 packed records [n,20] in, (v, var) out; pyTetris.step_games_dev / states_of_dev / playout_dev work on them):
+
+  python -m tetris_mcts_b200.play_batched --agent_type VanillaC --n_parallel 4096 --mcts_sims 300 --endless
+  python -m tetris_mcts_b200.play_batched --agent_type Vanilla --game_evaluator mymod:make --n_parallel 4096 --mcts_sims 300 --endless
+
 Flags are play.py's (play.py:46-70) plus --n_parallel / --max_nodes / --device / --watch / --seed and the online agent's memory and training
 settings.  One "episode" is one finished game of any of the parallel games; episodes are numbered in the order (move, game index) they end."""
 import argparse
@@ -50,7 +58,7 @@ from .engine import BatchedEngine
 
 perr = dict(file=stderr, flush=True)
 EPISODE_FMT = 'Episode: {:>5} Score: {:>10} Lines Cleared: {:>10}'          # play.py:164
-MODES = {"ValueSimLP": ("lp", 0.999, 1), "ValueSim": ("single", 0.999, 1), "Vanilla": ("vanilla", 0.99, 5)}
+MODES = {"ValueSimLP": ("lp", 0.999, 1), "ValueSim": ("single", 0.999, 1), "Vanilla": ("vanilla", 0.99, 5), "VanillaC": ("vanilla", 0.99, 1)}
 
 
 class ScoreTracker:                                                          # play.py:9-41
@@ -218,7 +226,7 @@ def run(args, out=sys.stdout, timing=None):
     device = args.device if world == 1 else D.env_world()[1]
     mode, gamma, low = MODES[args.agent_type]
     env_args = ((20, 10), args.app, args.tetris_scoring, args.tetris_randomizer)           # play.py:75
-    weights, evaluator = None, None
+    weights, evaluator, game_evaluator = None, None, None
     resumed = None
     if args.resume:
         try:
@@ -232,6 +240,10 @@ def run(args, out=sys.stdout, timing=None):
             raise ValueError(found[1])
     if args.evaluator:
         evaluator = _factory(args.evaluator)(_torch_device(device))
+    elif args.game_evaluator:
+        game_evaluator = _factory(args.game_evaluator)(_torch_device(device))
+    elif args.agent_type == "VanillaC":                                                   # agents/VanillaC.py random_playout, on the device
+        game_evaluator = PT.playout_evaluator(n_actions=8, variance=1e5, seed=args.seed + lo)
     elif mode != "vanilla" and resumed is not None:
         weights = resumed["trainer"]["weights"] if resumed["trainer"] else None               # the engine image holds the search's own
     elif mode != "vanilla":
@@ -249,7 +261,8 @@ def run(args, out=sys.stdout, timing=None):
         eng = BatchedEngine.load(image, device=device)
     else:
         eng = BatchedEngine(hi - lo, max_nodes=args.max_nodes, mode=mode, gamma=gamma, low=low,
-                            eval_kind="external" if evaluator else (args.eval_kind if mode != "vanilla" else "synthetic"), weights=weights,
+                            eval_kind="external" if evaluator else "external_game" if game_evaluator else (args.eval_kind if mode != "vanilla" else "synthetic"),
+                            weights=weights,
                             env_args=env_args, seed=(args.seed + 0x9E3779B9 * lo) & 0xFFFFFFFF, device=device, overflow_reset=True)
         eng.set_games(PT.new_games(hi - lo, env_args, D.shard_seeds(args.seed, args.n_parallel, rank, world)))
         eng.set_gc_headroom(args.max_nodes * 5 // 32)
@@ -317,7 +330,7 @@ def run(args, out=sys.stdout, timing=None):
                 status.update(eng.get_games()[args.watch - lo])
             before = eng.get_games() if saver else None
             actions, stats = eng.play_move(args.mcts_sims, auto_reset=True, want_stats=saver is not None,
-                                           evaluator=evaluator)   # agent.play(); game.play(action); agent.update_root(game); reset
+                                           evaluator=evaluator, game_evaluator=game_evaluator)   # agent.play(); game.play(action); agent.update_root(game); reset
             if saver:
                 saver.add_rows(rows_from_move(before, actions, stats, args.cycle, episode_of))
             moves += 1
@@ -440,6 +453,9 @@ def parse_args(argv=None):
     p.add_argument('--evaluator', default=None, metavar='MODULE:FACTORY',
                    help='search with the caller\'s network: FACTORY(device) returns a device evaluator (boards [n,1,20,10] -> (v, var)); '
                         'the engine runs eval_kind external.  Not with --online unless --trainer trains it, nor with Vanilla')
+    p.add_argument('--game_evaluator', default=None, metavar='MODULE:FACTORY',
+                   help='Vanilla / VanillaC: score each step\'s leaf games with the caller\'s function instead of the rollout: FACTORY(device) '
+                        'returns a device game evaluator (int32 packed records [n,20] -> (v, var)); the engine runs eval_kind external_game')
     p.add_argument('--trainer', default=None, metavar='MODULE:FACTORY',
                    help='--online: train with the caller\'s function instead of the built-in trainer: FACTORY(device) returns '
                         'train(state, value, variance, visit, size), which trains the --evaluator network in place and returns None, or '
@@ -479,6 +495,23 @@ def parse_args(argv=None):
         p.error('--resume and --checkpoint_every need --checkpoint_dir')
     if args.checkpoint_dir and args.evaluator:
         p.error('--checkpoint_dir cannot be combined with --evaluator: the caller\'s network is not part of the checkpoint')
+    if args.game_evaluator:
+        if args.agent_type not in ('Vanilla', 'VanillaC'):
+            p.error('--game_evaluator needs --agent_type Vanilla or VanillaC: the other agents evaluate boards (see --evaluator)')
+        if args.evaluator:
+            p.error('--game_evaluator cannot be combined with --evaluator: the leaf games are scored by one of them')
+        if args.online:
+            p.error('--game_evaluator cannot be combined with --online: Vanilla has no value network to train')
+        if ':' not in args.game_evaluator:
+            p.error('--game_evaluator takes MODULE:FACTORY')
+    if args.agent_type == 'VanillaC':
+        if args.evaluator:
+            p.error('--evaluator cannot be combined with --agent_type VanillaC: VanillaC scores leaf games (see --game_evaluator)')
+        if args.trainer:
+            p.error('--trainer cannot be combined with --agent_type VanillaC: VanillaC has no value network to train')
+    if args.checkpoint_dir and (args.game_evaluator or args.agent_type == 'VanillaC'):
+        p.error('--checkpoint_dir cannot be combined with --game_evaluator or --agent_type VanillaC: the playouts\' random state is not '
+                'part of the checkpoint')
     if args.checkpoint_every < 0:
         p.error('--checkpoint_every takes a number of moves >= 0')
     return args

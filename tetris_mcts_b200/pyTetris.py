@@ -1,7 +1,12 @@
 """pyTetris.Tetris — drop-in for the (absent, third-party) hrpan/pyTetris module consumed by the reference:
 play.py:1,75-76,150,169, agents/agent.py:70,103,114,143-144.  The object is a handle around the 80-byte packed
 record of SPEC_PYTETRIS.md §6.  Construction, reset(), play() and getState() all run on the GPU through the C-ABI
-(b200_tetris_new / b200_tetris_step / b200_tetris_state); no rule of the game is implemented on the host."""
+(b200_tetris_new / b200_tetris_step / b200_tetris_state); no rule of the game is implemented on the host.
+
+The `_dev` functions below work on records that stay on the device (torch int32 [n, 20], e.g. the leaf games an eval_kind
+"external_game" engine hands to its game evaluator): they enqueue one kernel on the current torch stream and return."""
+import ctypes as C
+
 import numpy as np
 
 from . import _lib as L
@@ -116,3 +121,110 @@ def states_of(recs):
     out = np.zeros((len(recs), 20, 10), np.int8)
     L.check(L.lib().b200_tetris_state(L.ptr(recs), L.ptr(out), len(recs)))
     return out
+
+
+# ---------------------------------------------------------------------------------------------------- games on the device
+def _recs_dev(recs, name="recs"):
+    import torch
+    if not isinstance(recs, torch.Tensor) or recs.dtype != torch.int32 or recs.device.type != "cuda":
+        raise ValueError("%s: a torch int32 tensor on a CUDA device; got %s" % (
+            name, (recs.dtype, recs.device) if isinstance(recs, torch.Tensor) else type(recs).__name__))
+    if recs.dim() != 2 or recs.shape[1] != L.REC_WORDS or not recs.is_contiguous() or recs.data_ptr() % 16:
+        raise ValueError("%s: a contiguous, 16-byte aligned [n, %d] tensor; got shape %s" % (name, L.REC_WORDS, tuple(recs.shape)))
+    return recs
+
+
+def _same_device(t, recs, dtype, shape, name):
+    import torch
+    if not isinstance(t, torch.Tensor) or t.dtype != dtype or t.device != recs.device or tuple(t.shape) != shape or not t.is_contiguous():
+        raise ValueError("%s: a contiguous %s tensor of shape %s on %s" % (name, dtype, shape, recs.device))
+    return t
+
+
+def _stream(recs):
+    import torch
+    return C.c_void_p(torch.cuda.current_stream(recs.device).cuda_stream)
+
+
+def step_games_dev(recs, actions):
+    """Tetris.play of every row of recs (torch int32 [n, 20] on a CUDA device, changed in place) with actions (int32 [n], same device;
+    ids outside 0..6 move nothing), enqueued on the current stream."""
+    import torch
+    recs = _recs_dev(recs)
+    actions = _same_device(actions, recs, torch.int32, (recs.shape[0],), "actions")
+    L.check(L.lib().b200_tetris_step_dev(C.c_void_p(recs.data_ptr()), C.c_void_p(actions.data_ptr()), recs.shape[0], _stream(recs)))
+    return recs
+
+
+def states_of_dev(recs, dtype="float32", out=None):
+    """getState() of every row of recs as a [n, 1, 20, 10] tensor ("float32" or "int8") on the records' device: the boards an eval_kind
+    "external" engine hands to its evaluator (board bits, -1 on the falling piece), enqueued on the current stream."""
+    import torch
+    recs = _recs_dev(recs)
+    tdt = {"float32": torch.float32, "int8": torch.int8}[dtype]
+    n = recs.shape[0]
+    out = torch.empty((n, 1, 20, 10), dtype=tdt, device=recs.device) if out is None else _same_device(out, recs, tdt, (n, 1, 20, 10), "out")
+    kind = L.BOARD_F32 if dtype == "float32" else L.BOARD_INT8
+    L.check(L.lib().b200_tetris_state_dev(C.c_void_p(recs.data_ptr()), C.c_void_p(out.data_ptr()), kind, n, _stream(recs)))
+    return out
+
+
+def playout_dev(recs, rng, n_actions=7, max_steps=2**31 - 1):
+    """Random playouts of every row of recs in place (the rollout's loop): row i plays xorshift32(rng[i]) % n_actions (1..8; 8 includes the
+    no-op 7, VanillaC's randint(0, 7)) until game over or after max_steps actions.  rng (int32 [n] xorshift32 states, same device) is
+    advanced in place; a state of 0 starts as 0x2545F491.  Returns int32 [n], the actions each row played.  Enqueued on the current stream."""
+    import torch
+    recs = _recs_dev(recs)
+    n = recs.shape[0]
+    rng = _same_device(rng, recs, torch.int32, (n,), "rng")
+    steps = torch.empty(n, dtype=torch.int32, device=recs.device)
+    L.check(L.lib().b200_tetris_playout_dev(C.c_void_p(recs.data_ptr()), C.c_void_p(rng.data_ptr()), n, int(n_actions), int(max_steps),
+                                            C.c_void_p(steps.data_ptr()), _stream(recs)))
+    return steps
+
+
+def record_fields(recs):
+    """end, score, line_clears and combo of packed records (SPEC_PYTETRIS §6), decoded from their word offsets with torch bit operations:
+    a dict of [n] int32 tensors on the records' device, or of numpy int32 arrays for a numpy [n, 20] uint32 / int32 input."""
+    import torch
+    host = isinstance(recs, np.ndarray)
+    r = torch.from_numpy(np.ascontiguousarray(recs).reshape(-1, L.REC_WORDS).view(np.int32)) if host else recs
+    out = {"end": (r[:, 10] >> 21) & 1, "score": r[:, 13], "line_clears": r[:, 14], "combo": (r[:, 11] >> 8) & 0xffffff}
+    return {k: (v.numpy().astype(np.int32) if host else v) for k, v in out.items()}
+
+
+def per_game(f):
+    """A host game evaluator (BatchedEngine.run_sims(game_evaluator=, host=True)) from a reference-style f(Tetris) -> (value, variance),
+    e.g. VanillaC's random_playout unchanged: f gets one Tetris per leaf record, built from a copy, and the results come back as float32.
+    This is the drop-in for existing code, not a fast path: every Tetris.play is a device round trip."""
+    def evaluate(recs):
+        recs = np.asarray(recs, np.uint32).reshape(-1, L.REC_WORDS)
+        v = np.zeros(len(recs), np.float32)
+        var = np.zeros(len(recs), np.float32)
+        for i, rec in enumerate(recs):
+            v[i], var[i] = f(Tetris(_record=rec))
+        return v, var
+    return evaluate
+
+
+def playout_evaluator(n_actions=7, variance=1e5, seed=0, max_steps=2**31 - 1):
+    """A device game evaluator that scores each leaf record by one random playout (playout_dev) and returns (score, variance): with
+    n_actions=8 and variance=1e5 it is VanillaC's random_playout, restated on the device.  Row i of the c-th call starts its stream from a
+    hash of (seed, c, i, the record's piece-stream word), so two runs from the same start give the same playouts."""
+    import torch
+    calls = [0]
+
+    def evaluate(recs):
+        n = recs.shape[0]
+        row = torch.arange(n, dtype=torch.int64, device=recs.device)
+        x = (recs[:, 12].to(torch.int64) & 0xffffffff) ^ ((row * 0x9E3779B1 + calls[0] * 0x85EBCA77 + int(seed) * 0xC2B2AE3D) & 0xffffffff)
+        x = ((x ^ (x >> 16)) * 0x45D9F3B) & 0xffffffff
+        x = ((x ^ (x >> 16)) * 0x45D9F3B) & 0xffffffff
+        x = x ^ (x >> 16)
+        rng = torch.where(x >= 2**31, x - 2**32, x).to(torch.int32)       # the same 32 bits as int32
+        calls[0] += 1
+        games = recs.clone()
+        playout_dev(games, rng, n_actions, max_steps)
+        v = games[:, 13].to(torch.float32)
+        return v, torch.full_like(v, float(variance))
+    return evaluate
