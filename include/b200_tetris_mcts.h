@@ -7,6 +7,11 @@
  *   - pointers are HOST pointers unless the name says `_dev`;
  *   - every function returns 0 on success or a B200_ERR_* code; b200_last_error() gives the text;
  *   - one host thread per engine; all work of an engine is issued on ONE CUDA stream: its own, or the caller's (b200_engine_set_stream);
+ *   - different engines and trainers (b200_trainer_*) may be driven by different host threads at the same time: every entry point
+ *     that touches the device first makes its engine's or trainer's device current on the calling thread, the error texts
+ *     (b200_last_error, b200_trainer_last_error) are per thread, and the only other process-wide state, b200_snapshot_set_staging's
+ *     size, is set before such threads start.  Engines and trainers create non-blocking streams, so no work of one waits on another's
+ *     stream through the legacy default stream;
  *   - there is no CPU fallback: without a CUDA device every compute entry point returns B200_ERR_CUDA.
  * Games travel as the 80-byte packed record of SPEC_PYTETRIS.md §6 (20 uint32 words).
  */

@@ -302,6 +302,7 @@ extern "C" int b200_engine_create(const b200_config *cfg, b200_engine **out) {
 
 extern "C" int b200_engine_destroy(b200_engine *e) {
     if (!e) return B200_OK;
+    cudaSetDevice(e->cfg.device);                    // the current device is per host thread: this one may not have made it current
     if (e->stream) cudaStreamSynchronize(e->stream);
     if (e->step_exec) cudaGraphExecDestroy(e->step_exec);
     tc_destroy(e->tc_state);

@@ -974,6 +974,7 @@ extern "C" const char *b200_trainer_last_error(void) { return g_terr.c_str(); }
 
 extern "C" int b200_trainer_destroy(b200_trainer *t) {
     if (!t) return B200_OK;
+    cudaSetDevice(t->device);                        // the current device is per host thread: this one may not have made it current
     if (t->stream) cudaStreamSynchronize(t->stream);
     for (void *p : t->allocs) cudaFree(p);
     if (t->d_log) cudaFree(t->d_log);

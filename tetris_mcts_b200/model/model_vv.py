@@ -114,6 +114,15 @@ _TRAIN_ROWS_FIXED = dict(validation_fraction=0.1, sample_replacement=True, overs
                          early_stopping_patience=10, early_stopping_threshold=1., shuffle=False)
 
 
+def rows_validation_size(n_rows):
+    """train_rows' validation split of n_rows rows; 0 (after the message) means too few rows to train on, and train_rows skips them.  It
+    depends on n_rows alone, so a pipelined trainer (online.OnlineTrainer.start) decides the skip before its training starts."""
+    validation_size = int(int(n_rows) * _TRAIN_ROWS_FIXED["validation_fraction"])
+    if validation_size == 0:
+        print("Not enough training data ({} < {}), collecting more data.".format(int(n_rows), int(np.ceil(1 / _TRAIN_ROWS_FIXED["validation_fraction"]))), **perr)
+    return validation_size
+
+
 class Model_VV:
     """Model_VV().load(); .training(flag); .inference(batch); .train(batch); .train_data(data); .save()  (model/model_vv.py:104-231 on
     model/model.py:39-255).  Inference runs through the engine's network kernels, training through the device trainer."""
@@ -278,9 +287,8 @@ class Model_VV:
         if bad:
             raise ValueError("train_rows implements train_data with %s only; got %s" % (_TRAIN_ROWS_FIXED, bad))
         n_rows = int(n_rows)
-        validation_size = int(n_rows * _TRAIN_ROWS_FIXED["validation_fraction"])
+        validation_size = rows_validation_size(n_rows)
         if validation_size == 0:
-            print("Not enough training data ({} < {}), collecting more data.".format(n_rows, int(np.ceil(1 / _TRAIN_ROWS_FIXED["validation_fraction"]))), **perr)
             return False
         from .. import distributed as D
         rank, world = D.rank_world()

@@ -23,6 +23,12 @@ deterministic, one game per rank under --online):
 
   python -m tetris_mcts_b200.play_batched --agent_type ValueSimLP --online --endless --checkpoint_dir ckpt --checkpoint_every 100 --resume
 
+--train_lag L (with --online) trains on a thread of its own while the search plays on: a training started after move s reaches the search
+after move s + L, or at the next training point if that comes first.  0 is the reference's serial loop; with L > 0 the search evaluates with
+weights up to L moves older than the reference's would.  The run's results depend on its seeds and L alone, not on how long a training takes:
+
+  python -m tetris_mcts_b200.play_batched --agent_type ValueSimLP --online --train_kind tf32 --train_lag 4 --n_parallel 4096 --endless
+
 --evaluator MODULE:FACTORY searches with the caller's network instead of the built-in one: FACTORY(device) returns a device evaluator
 (BatchedEngine.run_sims: a torch tensor [n,1,20,10] of boards in, (v, var) out), and the engine runs eval_kind "external".
 
@@ -110,7 +116,8 @@ def save_suffix(rank, world):
 # flags a resumed run must share with the run that wrote the checkpoint (they change what the engine, the memory or the trainer hold)
 RESUME_FLAGS = ("agent_type", "n_parallel", "max_nodes", "seed", "eval_kind", "train_kind", "online", "memory_size", "accumulation_policy",
                 "episodes_per_train", "memory_growth_rate", "train_batch_size", "train_max_iters", "mcts_sims", "app", "tetris_scoring",
-                "tetris_randomizer", "save", "cycle")
+                "tetris_randomizer", "save", "cycle", "train_lag")
+RESUME_DEFAULTS = {"train_lag": 0}          # the value of a flag in checkpoints written before it existed
 
 
 # A checkpoint is one generation: DIR/gen<moves>/ holds every rank's engine image and run state, each run state naming its image and the
@@ -169,7 +176,7 @@ def read_run_state(args, rank, world):
     if st.get("finished"):
         raise ValueError("--resume: the run checkpointed in %s had finished (--ngames reached)" % args.checkpoint_dir)
     differ = ["world size (%d, checkpoint %d)" % (world, st["world"])] if st["world"] != world else []
-    differ += ["--%s (%r, checkpoint %r)" % (k, getattr(args, k), st["flags"].get(k)) for k in RESUME_FLAGS if st["flags"].get(k) != getattr(args, k)]
+    differ += ["--%s (%r, checkpoint %r)" % (k, getattr(args, k), st["flags"].get(k)) for k in RESUME_FLAGS if st["flags"].get(k, RESUME_DEFAULTS.get(k)) != getattr(args, k)]
     if differ:
         raise ValueError("--resume: the checkpoint in %s was written with other settings: %s" % (args.checkpoint_dir, "; ".join(differ)))
     return st, image
@@ -212,8 +219,8 @@ def drop_later_chunks(file_name, chunk):
 
 
 def run(args, out=sys.stdout, timing=None):
-    """timing: a dict, filled with moves, trainings and the wall-clock seconds of the run split into search (everything but training) and
-    training (--online).
+    """timing: a dict, filled with moves, trainings and wall-clock seconds: total_s, train_s (the trainings themselves, --online), wait_s
+    (this thread blocked on a training: all of it with --train_lag 0) and search_s = total_s - wait_s.
 
     Under a torch.distributed process group (main() under torchrun) rank r plays the games shard_range(n_parallel, r, world) on device
     LOCAL_RANK, with the piece seeds and search streams of their global indices, so every game plays as in a single-process run.  Finished
@@ -279,7 +286,7 @@ def run(args, out=sys.stdout, timing=None):
                                       external=evaluator is not None)
         else:
             trainer = OnlineTrainer(eng, weights, args.memory_size, batch_size=args.train_batch_size, max_iters=args.train_max_iters,
-                                    train_kind=args.train_kind)   # ValueSim.py:180
+                                    train_kind=args.train_kind, train_lag=args.train_lag)   # ValueSim.py:180
         if resumed is not None and resumed["trainer"]:
             trainer.restore(resumed["trainer"])
         if world > 1:                                                                      # the rows one move's collections stored on this rank
@@ -313,7 +320,7 @@ def run(args, out=sys.stdout, timing=None):
         size = eng.save(image)
         write_run_state(state, dict(world=world, flags={k: getattr(args, k) for k in RESUME_FLAGS}, generation=moves, ngames=ngames, moves=moves,
                                     gcs=gcs, image=os.path.basename(image), image_bytes=size, finished=bool(finished),
-                                    scores=list(tracker.scores), lines=list(tracker.lines), trainer=trainer.state() if trainer else None,
+                                    scores=list(tracker.scores), lines=list(tracker.lines), trainer=trainer.state() if trainer else None,   # a training in flight: joined, saved as pending
                                     episode_of=episode_of.copy() if saver else None,
                                     saver_chunk=saver.chunk if saver and not saver.hdf5 else None))
         if world > 1:
@@ -359,6 +366,8 @@ def run(args, out=sys.stdout, timing=None):
                 if ngames >= args.ngames:
                     done = True
                     break
+            if trainer:
+                trainer.after_move(moves)                                                   # installs a training started --train_lag moves ago
             if collected:
                 train_now, n = False, 0
                 if rank == 0:
@@ -367,10 +376,12 @@ def run(args, out=sys.stdout, timing=None):
                 if world > 1:
                     train_now, n = D.broadcast_ints([train_now, n])
                 if train_now:
-                    trainer.train(n, ngames)
+                    trainer.train(n, ngames)                                                # installs the one in flight first (--train_lag)
                     if args.trainer and rank == 0:
                         print('Training complete.', **perr)                                   # agent.cpp:702
             last = done or (args.max_moves and moves >= args.max_moves)
+            if last and trainer:
+                trainer.join()                                                              # the run's trainer state includes it
             if args.checkpoint_dir and (last or (args.checkpoint_every and moves % args.checkpoint_every == 0)):
                 checkpoint(done)
             if last:
@@ -380,8 +391,9 @@ def run(args, out=sys.stdout, timing=None):
             print(flush=True, file=out)                                                     # play.py:179
         if timing is not None:
             total = time.perf_counter() - t_start
-            timing.update(moves=moves, total_s=total, train_s=trainer.train_seconds if trainer else 0.0, trainings=trainer.n_trains if trainer else 0)
-            timing["search_s"] = total - timing["train_s"]
+            timing.update(moves=moves, total_s=total, train_s=trainer.train_seconds if trainer else 0.0, trainings=trainer.n_trains if trainer else 0,
+                          wait_s=trainer.wait_seconds if trainer else 0.0)
+            timing["search_s"] = total - timing["wait_s"]
         if trainer:
             trainer.close()
         eng.close()                                                                         # play.py:181
@@ -462,6 +474,12 @@ def parse_args(argv=None):
                         'returns new weights for the built-in network (a Model_VV state_dict or N_WEIGHTS floats) or None')
     p.add_argument('--trainer_host', default=False, action='store_true',
                    help='hand --trainer numpy arrays instead of torch tensors on the device')
+    p.add_argument('--train_lag', default=0, type=int,
+                   help='--online: train on a thread of its own while the search plays on, and install the new weights after move s + '
+                        'TRAIN_LAG for a training started after move s (a training point within the lag installs the previous training '
+                        'first).  0 = the reference\'s loop, which searches on only once the training has ended; > 0 departs from it: the '
+                        'search evaluates with weights up to TRAIN_LAG moves older.  The run\'s results depend on the seeds and TRAIN_LAG '
+                        'alone, not on timing')
     p.add_argument('--max_moves', default=0, type=int, help='stop after this many moves (counted from the start of the run, across --resume)')
     p.add_argument('--checkpoint_dir', default=None, help='write checkpoints here (one engine image per rank and the run state)')
     p.add_argument('--checkpoint_every', default=0, type=int, help='moves between checkpoints; 0 = only when the run ends')
@@ -514,6 +532,19 @@ def parse_args(argv=None):
                 'part of the checkpoint')
     if args.checkpoint_every < 0:
         p.error('--checkpoint_every takes a number of moves >= 0')
+    if args.train_lag < 0:
+        p.error('--train_lag takes a number of moves >= 0')
+    if args.train_lag > 0:
+        from . import distributed as D
+        if not args.online:
+            p.error('--train_lag needs --online: it delays the installation of the online trainings\' weights')
+        if D.env_world()[2] > 1:
+            p.error('--train_lag > 0 cannot run with a world size above 1: the data-parallel training\'s collectives would run beside '
+                    'the per-move exchange of rows and games')
+        if args.evaluator:
+            p.error('--train_lag > 0 cannot be combined with --evaluator: the caller\'s network would be trained in place while it searches')
+        if args.trainer:
+            p.error('--train_lag > 0 cannot be combined with --trainer: the caller\'s training function runs on the search\'s thread')
     return args
 
 
