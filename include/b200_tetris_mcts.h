@@ -313,6 +313,12 @@ int b200_debug_load_tree(b200_engine *e, int game, int M, const int32_t *child, 
                          const float *value, const float *variance, const uint8_t *end, int root, uint32_t rng_state);
 int b200_debug_game_state(b200_engine *e, int game, uint32_t *rng_state, int32_t *pc_len);
 int b200_export_dist(b200_engine *e, int game, float *node_stats /* [M][5] */, float *node_dist /* [M][bins] */);
+/* DistValueSimOnline.get_value (agents/DistValueSimOnline.py:106-116) of every game: out_dev (DEVICE) double[n_games][2] = {mean, var} of
+ * mean_variance (core_distributional.py:48-63) over the game's root node distribution, computed on the device by the routine that
+ * b200_dist_mean_variance runs (the same bits as b200_dist_mean_variance on that row).  Every game gets its root row's value
+ * whatever its status (a root without a backup yet holds zeros: {0, 0}).  B200_MODE_DIST only (B200_ERR_BAD_ARG otherwise); runs on the
+ * engine's stream and synchronises. */
+int b200_dist_root_values_dev(b200_engine *e, double *out_dev);
 
 /* --- replay samples of the live search (ValueSim.store_nodes, agents/ValueSim.py:122-159): observations with
  *     visit >= min_visits and not end, packed as {int8 state[200], f32 value, f32 variance, f32 visit} = 212 B.

@@ -3,6 +3,9 @@ Upstream the file is not runnable (it imports a module that does not exist and c
 the search loop it sketches (:36-75) is driven here on the reference's distributional cores
 (agents/core_distributional.py:82-124) by the CUDA engine in B200_MODE_DIST.  play.py does
 getattr(module, 'DistValueSimOnline') (play.py:82), so the class is exported under both names."""
+import os
+from collections.abc import Mapping
+
 import numpy as np
 
 from .. import _lib as L
@@ -20,17 +23,31 @@ def init_dist_weights(seed=0, atoms=50):
     return np.concatenate(parts)
 
 
+def _dist_weight_vector(w, atoms):
+    """a state_dict or a checkpoint path -> the weight vector (model/model_distributional.py); a vector passes as it is"""
+    from ..model.model_distributional import load_checkpoint_dist_weights, state_dict_to_dist_weights
+    if isinstance(w, (str, bytes, os.PathLike)):
+        if not os.path.isfile(w):
+            raise ValueError("no distributional checkpoint at %s" % (w,))
+        return load_checkpoint_dist_weights(w, atoms)
+    if isinstance(w, Mapping):
+        return state_dict_to_dist_weights(w, atoms)
+    return w
+
+
 class DistValueSim(TreeAgent):
     _mode = "dist"
 
     def __init__(self, atoms=50, vmin=0, vmax=5000, dist_weights=None, **kwargs):          # DistValueSimOnline.py:13
+        """dist_weights: None (init_dist_weights(0, atoms)), the flat weight vector, a Net(atoms) state_dict or the path of a checkpoint
+        Model_Dist.save / the reference's Model.save wrote (model/model_distributional.py)."""
         kwargs.pop("max_nodes", None)
         kwargs.pop("online", None)
         kwargs.pop("min_visit", None)
         self.atoms, self.vrange = atoms, (vmin, vmax)
         super().__init__(max_nodes=100000, low=5, eval_kind=kwargs.pop("eval_kind", "net"), **kwargs)
         if self._eng.eval_kind not in (L.EVAL_SYNTHETIC, L.EVAL_EXTERNAL):
-            self._eng.load_dist_weights(init_dist_weights(0, atoms) if dist_weights is None else dist_weights, atoms)
+            self._eng.load_dist_weights(init_dist_weights(0, atoms) if dist_weights is None else _dist_weight_vector(dist_weights, atoms), atoms)
 
     def _engine_kwargs(self):
         return dict(dist_bins=self.atoms, dist_vmin=self.vrange[0], dist_vmax=self.vrange[1])

@@ -1127,6 +1127,21 @@ extern "C" int b200_export_dist(b200_engine *e, int game, float *node_stats, flo
     return B200_OK;
 }
 
+// DistValueSimOnline.get_value of every game at once (k_dist_root_values): out_dev (DEVICE) double[G][2] = {mean, var} of each root's
+// distribution, without copying the arenas to the host
+extern "C" int b200_dist_root_values_dev(b200_engine *e, double *out_dev) {
+    if (!e || !out_dev) return fail(B200_ERR_BAD_ARG, "null argument");
+    if (e->A.mode != MODE_DIST || !e->A.ndist) return fail(B200_ERR_BAD_ARG, "b200_dist_root_values_dev needs B200_MODE_DIST");
+    CK(cudaSetDevice(e->cfg.device));
+    {
+        PhaseTimer t(e, PH_MISC);
+        k_dist_root_values<<<(e->A.G + 127) / 128, 128, 0, e->stream>>>(e->A, out_dev);
+    }
+    CK(cudaGetLastError());
+    CK(cudaStreamSynchronize(e->stream));
+    return B200_OK;
+}
+
 // ---------------------------------------------------------------------------------------------------- standalone value net
 __global__ void k_states_to_keys(const int8_t *states, int k, uint32_t *keys, uint2 *req) {
     int i = blockIdx.x * blockDim.x + threadIdx.x;

@@ -172,6 +172,19 @@ __device__ inline void dist_backup_trace_warp(const float *d, int bins, double v
     }
 }
 
+// mean_variance (core_distributional.py:48-63) of every game's root node distribution, as DistValueSimOnline.get_value reads it
+// (:106-116: arrays['value'][root]): out[g] = {mean, var} in double.  One thread per game runs dist_mean_variance, the routine of the operator
+// twin b200_dist_mean_variance, over the bins in ascending order: the same operations in the same order, so the same bits as the twin on
+// that row.  A game's root always names a slot of its arena (new_node gives slot 0 when it fails), so every game gets the twin's value of
+// its root row whatever its status: a root that has no backup yet holds zeros, for which the twin returns (0, 0).
+__global__ void __launch_bounds__(128) k_dist_root_values(Arena A, double *out) {
+    const int g = blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= A.G) return;
+    const int bins = A.dist_bins;
+    const float *row = A.ndist + ((size_t)g * A.M + (size_t)A.root[g]) * bins;
+    dist_mean_variance(row, bins, A.dist_vmin, A.dist_vmax, out[2 * g], out[2 * g + 1]);
+}
+
 // ---- single-call twins (operator-level parity entry points, not the throughput path)
 __global__ void k_dist_shift(const float *dist, int bins, double x, double vmin, double vmax, float *out) { dist_shift(dist, bins, x, vmin, vmax, out); }
 __global__ void k_dist_mean_variance(const float *dist, int bins, double vmin, double vmax, double *out) { dist_mean_variance(dist, bins, vmin, vmax, out[0], out[1]); }

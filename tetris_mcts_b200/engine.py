@@ -121,6 +121,26 @@ class BatchedEngine:
         L.check(L.lib().b200_export_dist(self.h, int(game), L.ptr(ns), L.ptr(nd)))
         return ns, nd
 
+    def dist_root_values(self, out=None):
+        """DistValueSimOnline.get_value (agents/DistValueSimOnline.py:106-116) of every game, computed on the device (b200_dist_root_values_dev):
+        {mean, var} float64 of each root's node distribution, bit for bit b200_dist_mean_variance of export_dist(g)'s root row.  out None:
+        returns a numpy [n_games, 2]; out a float64 torch tensor of n_games * 2 elements on the engine's device: filled and returned.
+        Mode dist only."""
+        import torch
+        if out is not None:
+            if not isinstance(out, torch.Tensor) or out.dtype != torch.float64 or out.numel() != 2 * self.n_games or not out.is_contiguous() \
+                    or out.device != torch.device("cuda", int(self.cfg.device)):
+                raise ValueError("out must be a contiguous float64 torch tensor of %d elements on cuda:%d" % (2 * self.n_games, int(self.cfg.device)))
+            L.check(L.lib().b200_dist_root_values_dev(self.h, C.c_void_p(out.data_ptr())))
+            return out
+        buf = getattr(self, "_root_values", None)
+        if buf is None:                                   # allocated once, on torch's stream: finished there before the engine's stream writes it
+            dev = torch.device("cuda", int(self.cfg.device))
+            buf = self._root_values = torch.empty((self.n_games, 2), dtype=torch.float64, device=dev)
+            torch.cuda.current_stream(dev).synchronize()
+        L.check(L.lib().b200_dist_root_values_dev(self.h, C.c_void_p(buf.data_ptr())))
+        return buf.cpu().numpy()
+
     # ------------------------------------------------------------------ games
     def set_games(self, recs):
         recs = np.ascontiguousarray(recs, np.uint32).reshape(self.n_games, L.REC_WORDS)
@@ -185,16 +205,24 @@ class BatchedEngine:
         a = None if actions is None else np.ascontiguousarray(actions, np.int32)
         L.check(L.lib().b200_env_step(self.h, L.ptr(a)))
 
-    def play_move(self, sims, auto_reset=True, want_stats=True, evaluator=None, board_dtype="float32", host=False, game_evaluator=None):
+    def play_move(self, sims, auto_reset=True, want_stats=True, evaluator=None, board_dtype="float32", host=False, game_evaluator=None,
+                  want_root_values=False):
         """One move of play.py:118-177 for every game. Returns (actions, stats).  evaluator / board_dtype / host / game_evaluator: see
         run_sims (eval_kind "external" / "external_game"); the move is then run_sims, get_stats, env_step, update_root, as b200_play_move
-        does it."""
-        if evaluator is not None or game_evaluator is not None:
-            self.run_sims(sims, evaluator, board_dtype, host, game_evaluator)
+        does it.  want_root_values (mode dist): returns (actions, stats, root_values), root_values = dist_root_values() read after the search
+        and before env_step / update_root, where play.py:131-132 saves its row and want_stats reads the statistics."""
+        if evaluator is not None or game_evaluator is not None or want_root_values:
+            if evaluator is not None or game_evaluator is not None:
+                self.run_sims(sims, evaluator, board_dtype, host, game_evaluator)
+            else:
+                L.check(L.lib().b200_run_sims(self.h, int(sims)))
             stats, actions = self.get_stats()
+            root_values = self.dist_root_values() if want_root_values else None
             self.env_step(None)
             self.update_root(auto_reset)
             self.sync()
+            if want_root_values:
+                return actions, (stats if want_stats else None), root_values
             return actions, (stats if want_stats else None)
         actions = np.zeros(self.n_games, np.int32)
         stats = np.zeros((self.n_games, 3, L.N_ACTIONS), np.float32) if want_stats else None

@@ -41,6 +41,15 @@ or None to keep them:
   python -m tetris_mcts_b200.play_batched --agent_type ValueSimLP --online --evaluator mynets:make_evaluator --trainer mynets:make_trainer --endless
   python -m tetris_mcts_b200.play_batched --agent_type ValueSimLP --online --eval_kind net_fp16 --trainer mytraining:make_trainer --endless
 
+--agent_type DistValueSimOnline (or DistValueSim) plays the distributional agent (agents/DistValueSimOnline.py, BASELINE configs[4]) with
+fixed weights: --dist_checkpoint PATH (Model_Dist.save / the reference's Model.save), else ./pytorch_model/model_checkpoint when it holds
+a distributional network, else init_dist_weights(0, atoms); --atoms / --vmin / --vmax set the histogram; --eval_kind net_tc, dist_fp16 or
+net, or --evaluator with a function returning probabilities [n, atoms].  --save rows carry the root's mean and variance
+(BatchedEngine.dist_root_values) as value / variance.  Training the distributional network is not built (no --online):
+
+  python -m tetris_mcts_b200.play_batched --agent_type DistValueSimOnline --n_parallel 2048 --max_nodes 32768 --mcts_sims 1500 --endless
+  torchrun --nproc-per-node 8 -m tetris_mcts_b200.play_batched --agent_type DistValueSimOnline --n_parallel 16384 --max_nodes 32768 --mcts_sims 1500 --endless
+
 --agent_type VanillaC is the C++ agent's rollout search (agents/VanillaC.py): check_low with low=1 and the leaf game scored by one random
 playout over all eight action ids, backed up as (score, 1e5); the engine runs eval_kind "external_game".  --game_evaluator MODULE:FACTORY
 (Vanilla or VanillaC) scores each step's leaf games with the caller's function instead: FACTORY(device) returns a device game evaluator
@@ -64,7 +73,8 @@ from .engine import BatchedEngine
 
 perr = dict(file=stderr, flush=True)
 EPISODE_FMT = 'Episode: {:>5} Score: {:>10} Lines Cleared: {:>10}'          # play.py:164
-MODES = {"ValueSimLP": ("lp", 0.999, 1), "ValueSim": ("single", 0.999, 1), "Vanilla": ("vanilla", 0.99, 5), "VanillaC": ("vanilla", 0.99, 1)}
+MODES = {"ValueSimLP": ("lp", 0.999, 1), "ValueSim": ("single", 0.999, 1), "Vanilla": ("vanilla", 0.99, 5), "VanillaC": ("vanilla", 0.99, 1),
+         "DistValueSimOnline": ("dist", 0.999, 5), "DistValueSim": ("dist", 0.999, 5)}   # select_trace_distributional(..., low=5), core_distributional.py:83
 
 
 class ScoreTracker:                                                          # play.py:9-41
@@ -116,8 +126,10 @@ def save_suffix(rank, world):
 # flags a resumed run must share with the run that wrote the checkpoint (they change what the engine, the memory or the trainer hold)
 RESUME_FLAGS = ("agent_type", "n_parallel", "max_nodes", "seed", "eval_kind", "train_kind", "online", "memory_size", "accumulation_policy",
                 "episodes_per_train", "memory_growth_rate", "train_batch_size", "train_max_iters", "mcts_sims", "app", "tetris_scoring",
-                "tetris_randomizer", "save", "cycle", "train_lag")
-RESUME_DEFAULTS = {"train_lag": 0}          # the value of a flag in checkpoints written before it existed
+                "tetris_randomizer", "save", "cycle", "train_lag", "atoms", "vmin", "vmax", "dist_checkpoint")
+# the value of a flag in checkpoints written before it existed
+RESUME_DEFAULTS = {"train_lag": 0, "atoms": 50, "vmin": 0.0, "vmax": 5000.0, "dist_checkpoint": None}
+DIST_DEFAULT_CHECKPOINT = "./pytorch_model/model_checkpoint"   # where DistValueSimOnline's self.model.load() looks (model/model.py:11)
 
 
 # A checkpoint is one generation: DIR/gen<moves>/ holds every rank's engine image and run state, each run state naming its image and the
@@ -232,8 +244,10 @@ def run(args, out=sys.stdout, timing=None):
     lo, hi = D.shard_range(args.n_parallel, rank, world)
     device = args.device if world == 1 else D.env_world()[1]
     mode, gamma, low = MODES[args.agent_type]
+    dist = mode == "dist"
     env_args = ((20, 10), args.app, args.tetris_scoring, args.tetris_randomizer)           # play.py:75
     weights, evaluator, game_evaluator = None, None, None
+    dist_weights, dist_source = None, None
     resumed = None
     if args.resume:
         try:
@@ -253,6 +267,9 @@ def run(args, out=sys.stdout, timing=None):
         game_evaluator = PT.playout_evaluator(n_actions=8, variance=1e5, seed=args.seed + lo)
     elif mode != "vanilla" and resumed is not None:
         weights = resumed["trainer"]["weights"] if resumed["trainer"] else None               # the engine image holds the search's own
+        dist_source = resumed.get("dist_weights")
+    elif dist:
+        dist_weights, dist_source = _dist_weights(args, rank)
     elif mode != "vanilla":
         from .model.model_vv import init_weights, load_checkpoint_weights
         if rank == 0:
@@ -267,10 +284,11 @@ def run(args, out=sys.stdout, timing=None):
     if resumed is not None:                                                               # trees, games, memory and policy as they were saved
         eng = BatchedEngine.load(image, device=device)
     else:
+        dist_kw = dict(dist_weights=dist_weights, dist_bins=args.atoms, dist_vmin=args.vmin, dist_vmax=args.vmax) if dist else {}
         eng = BatchedEngine(hi - lo, max_nodes=args.max_nodes, mode=mode, gamma=gamma, low=low,
                             eval_kind="external" if evaluator else "external_game" if game_evaluator else (args.eval_kind if mode != "vanilla" else "synthetic"),
                             weights=weights,
-                            env_args=env_args, seed=(args.seed + 0x9E3779B9 * lo) & 0xFFFFFFFF, device=device, overflow_reset=True)
+                            env_args=env_args, seed=(args.seed + 0x9E3779B9 * lo) & 0xFFFFFFFF, device=device, overflow_reset=True, **dist_kw)
         eng.set_games(PT.new_games(hi - lo, env_args, D.shard_seeds(args.seed, args.n_parallel, rank, world)))
         eng.set_gc_headroom(args.max_nodes * 5 // 32)
     online = args.online and not args.benchmark and mode != "vanilla"
@@ -322,7 +340,8 @@ def run(args, out=sys.stdout, timing=None):
                                     gcs=gcs, image=os.path.basename(image), image_bytes=size, finished=bool(finished),
                                     scores=list(tracker.scores), lines=list(tracker.lines), trainer=trainer.state() if trainer else None,   # a training in flight: joined, saved as pending
                                     episode_of=episode_of.copy() if saver else None,
-                                    saver_chunk=saver.chunk if saver and not saver.hdf5 else None))
+                                    saver_chunk=saver.chunk if saver and not saver.hdf5 else None,
+                                    dist_weights=dist_source))                              # where the image's distributional weights came from
         if world > 1:
             D.barrier()                                                                    # every rank's files of this generation are written
         if rank == 0:
@@ -336,10 +355,12 @@ def run(args, out=sys.stdout, timing=None):
             if status:
                 status.update(eng.get_games()[args.watch - lo])
             before = eng.get_games() if saver else None
-            actions, stats = eng.play_move(args.mcts_sims, auto_reset=True, want_stats=saver is not None,
-                                           evaluator=evaluator, game_evaluator=game_evaluator)   # agent.play(); game.play(action); agent.update_root(game); reset
-            if saver:
-                saver.add_rows(rows_from_move(before, actions, stats, args.cycle, episode_of))
+            played = eng.play_move(args.mcts_sims, auto_reset=True, want_stats=saver is not None, evaluator=evaluator,
+                                   game_evaluator=game_evaluator, want_root_values=bool(saver) and dist)   # agent.play(); game.play(action); agent.update_root(game); reset
+            actions, stats = played[0], played[1]
+            if saver:                                                                      # dist: value / variance = the root's mean / variance (DESIGN §2 (f)3)
+                value = (played[2][:, 0], played[2][:, 1]) if dist else ()
+                saver.add_rows(rows_from_move(before, actions, stats, args.cycle, episode_of, *value))
             moves += 1
             collected = online and eng.counters()["gcs"] != gcs                                # collections stored rows this move
             if collected:
@@ -414,6 +435,29 @@ def _torch_device(device):
     return torch.device("cuda", device)
 
 
+def _dist_weights(args, rank):
+    """The distributional agent's network (DistValueSimOnline.py:28-31, self.model.load()) -> (weights, where they came from): the
+    --dist_checkpoint file; without the flag DIST_DEFAULT_CHECKPOINT when it holds Net(atoms)'s state_dict (Model_VV checkpoints share
+    that path); otherwise init_dist_weights(0, atoms), which rank 0 says once."""
+    import contextlib
+    from .agents.DistValueSimOnline import init_dist_weights
+    from .model.model_distributional import holds_dist_state_dict, load_checkpoint_dist_weights
+    path = args.dist_checkpoint
+    if path is None and holds_dist_state_dict(DIST_DEFAULT_CHECKPOINT, args.atoms):
+        path = DIST_DEFAULT_CHECKPOINT
+    if path is not None:
+        with contextlib.ExitStack() as stack:
+            if rank != 0:                                                                   # the same file, without its message
+                stack.enter_context(contextlib.redirect_stdout(stack.enter_context(open(os.devnull, "w"))))
+            w = load_checkpoint_dist_weights(path, args.atoms)
+        if w is None:
+            raise ValueError("--dist_checkpoint: no file %s" % path)
+        return w, path
+    if rank == 0:
+        print("No distributional checkpoint at %s: using init_dist_weights(0, %d)" % (DIST_DEFAULT_CHECKPOINT, args.atoms), flush=True)
+    return init_dist_weights(0, args.atoms), "init_dist_weights(0, %d)" % args.atoms
+
+
 def _exchange_rows(eng, block, staged, most, rank):
     """All-gather the rows the ranks staged this move (`most` rows at most per rank); rank 0 appends those of ranks 1.. in rank order to its
     memory, as its own collections would have stored them."""
@@ -459,11 +503,19 @@ def parse_args(argv=None):
     p.add_argument('--train_kind', default='fp64', choices=('fp64', 'tc', 'tf32'),
                    help='trainer GEMMs (--online): fp64 CUDA cores, tc = Hopper tensor cores with the 3xTF32 split, or tf32 = one tf32 '
                         'term per operand with implicit-im2col convolutions (fastest, ~1e-3 of float64)')
-    p.add_argument('--eval_kind', default='net_tc', choices=('net_tc', 'net_fp16'),
-                   help='value network of the search (not Vanilla): net_tc = tensor cores within 1e-5 of fp32, net_fp16 = one fp16 product per '
-                        'product, about a third of the tensor-core work (DESIGN §5).  --online trains in fp32 / fp64 either way')
+    p.add_argument('--eval_kind', default='net_tc', choices=('net_tc', 'net_fp16', 'dist_fp16', 'net'),
+                   help='network of the search (not Vanilla): net_tc = tensor cores within 1e-5 of fp32, net_fp16 = one fp16 product per '
+                        'product, about a third of the tensor-core work (value agents, DESIGN §5), dist_fp16 = the same for the '
+                        'distributional network (DistValueSim*), net = fp32 CUDA cores.  --online trains in fp32 / fp64 either way')
+    p.add_argument('--atoms', default=50, type=int, help='DistValueSim*: bins of the value distribution (DistValueSimOnline.py:13; 2..64)')
+    p.add_argument('--vmin', default=0.0, type=float, help='DistValueSim*: low end of the value range (DistValueSimOnline.py:13)')
+    p.add_argument('--vmax', default=5000.0, type=float, help='DistValueSim*: high end of the value range (DistValueSimOnline.py:13)')
+    p.add_argument('--dist_checkpoint', default=None, metavar='PATH',
+                   help='DistValueSim*: the network\'s checkpoint (Model_Dist.save / the reference\'s Model.save layout); default: '
+                        + DIST_DEFAULT_CHECKPOINT + ' when it holds a distributional network, otherwise init_dist_weights(0, atoms)')
     p.add_argument('--evaluator', default=None, metavar='MODULE:FACTORY',
-                   help='search with the caller\'s network: FACTORY(device) returns a device evaluator (boards [n,1,20,10] -> (v, var)); '
+                   help='search with the caller\'s network: FACTORY(device) returns a device evaluator (boards [n,1,20,10] -> (v, var); '
+                        'DistValueSim*: -> probabilities [n, atoms] or [probs]); '
                         'the engine runs eval_kind external.  Not with --online unless --trainer trains it, nor with Vanilla')
     p.add_argument('--game_evaluator', default=None, metavar='MODULE:FACTORY',
                    help='Vanilla / VanillaC: score each step\'s leaf games with the caller\'s function instead of the rollout: FACTORY(device) '
@@ -487,6 +539,25 @@ def parse_args(argv=None):
     p.add_argument('--dist_backend', default='nccl', choices=('nccl', 'gloo'),
                    help='under torchrun: collectives over NCCL (one GPU per rank), or gloo through the host (several ranks may share a GPU)')
     args = p.parse_args(argv)
+    if MODES[args.agent_type][0] == 'dist':
+        if args.online or args.trainer or args.train_lag > 0:
+            p.error('--online, --trainer and --train_lag cannot be combined with --agent_type %s: training the distributional network is not '
+                    'built (the agent plays benchmark searches with fixed weights)' % args.agent_type)
+        if args.eval_kind == 'net_fp16':
+            p.error('--eval_kind net_fp16 has no distributional network: use net_tc, dist_fp16 or net with --agent_type %s' % args.agent_type)
+        if not 2 <= args.atoms <= 64:
+            p.error('--atoms takes 2 to 64 bins')
+        if not args.vmax > args.vmin:
+            p.error('--vmax must be above --vmin')
+        if args.evaluator and args.dist_checkpoint:
+            p.error('--dist_checkpoint cannot be combined with --evaluator: the caller\'s network evaluates the boards')
+    else:
+        if args.eval_kind == 'dist_fp16':
+            p.error('--eval_kind dist_fp16 is the distributional network\'s one-term form: it needs --agent_type DistValueSimOnline or '
+                    'DistValueSim (value agents: net_fp16)')
+        given = [f for f in ('atoms', 'vmin', 'vmax', 'dist_checkpoint') if getattr(args, f) != RESUME_DEFAULTS[f]]
+        if given:
+            p.error('%s set the distributional agent: they need --agent_type DistValueSimOnline or DistValueSim' % ', '.join('--' + f for f in given))
     if args.trainer:
         if not args.online:
             p.error('--trainer needs --online: it is called when the online accumulation policy says train')
